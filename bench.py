@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- candidate-GEMMs/s of the PTQ4ViT scale-factor search on B200.
+"""bench.py -- candidate-GEMMs/s of the PTQ4ViT scale-factor search on H100.
 
 A "step" = the full `calibration_step2` search of every wrapped Linear / MatMul of the workload
 (default: ViT-B/224, 32 synthetic images, W8A8, n_V=n_H=24 (qkv 72, head 1), n_a=1, eq_n=100, 3 rounds, hessian
@@ -9,12 +9,13 @@ metric = BASELINE.json configs[2] at one bit width) over tensors already residen
             host<->device copies inside the timing.
 `calib_wallclock` = the public `HessianQuantCalibrator(...).batching_quant_calib()` (capture + search + gather), the
             equivalent of what example/test_all.py:31-34 times.
-`reference_gpu` = the UNMODIFIED reference classes (baseline/_ref) on the same GPU, one layer per type, one round.
+`reference_gpu` = the UNMODIFIED reference classes (oracle/_ref, staged by build()) on the same GPU, one layer per type, one round.
 `cpu_baseline` / `--impl reference` = the reference classes on the host cores (bounded sample, see below).
 
   python bench.py --gpus 1 --steps 3 --warmup 3
   torchrun ... bench.py --gpus N ...          (layer-sharded, one all_gather of the step sizes per step)
   python bench.py --impl reference            (reference on the host cores)
+  python bench.py ... --dump-outputs DIR      (after the timed steps: the step sizes of every searched module, .npy)
 """
 import argparse
 import ctypes
@@ -53,6 +54,9 @@ def parse():
     ap.add_argument("--no-ref-gpu", action="store_true")
     ap.add_argument("--no-wallclock", action="store_true")
     ap.add_argument("--cpu-eq-n", type=int, default=20, help="candidates per search step of the CPU reference sample")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (every searched module's step sizes) as DIR/<module>.<name>.npy; "
+                         "under torchrun every rank writes the modules it searched, together the full set")
     return ap.parse_args()
 
 
@@ -137,6 +141,18 @@ def build_workload(a, device, rank, world):
     return net, wrapped, work, owner, names, cal
 
 
+def dump_outputs(work, out_dir):
+    """The step sizes each searched module holds after the last timed step -- what a caller of calibration_step2()
+    receives -- one float32 .npy per module and tensor (a few hundred KB for ViT-B)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, (m, _) in work.items():
+        for attr in ("w_interval", "a_interval", "A_interval", "B_interval", "split"):
+            v = getattr(m, attr, None)
+            if isinstance(v, torch.Tensor):
+                np.save(os.path.join(out_dir, f"{name}.{attr}.npy"), v.detach().float().cpu().numpy())
+
+
 def run_module(m, t):
     """One module's search through the reference-facing call, tensors already on the device."""
     if "x" in t:
@@ -204,7 +220,7 @@ def layer_types(a):
 
 
 def reference_rates(a, on_gpu, eq_n, only=None):
-    """Times the reference classes (oracle/ref_harness -> baseline/_ref; falls back to the oracle port) on one seeded
+    """Times the reference classes (oracle/ref_harness -> oracle/_ref; falls back to the oracle port) on one seeded
     synthetic layer of every type at the workload's sizes.  GPU: the whole calibration_step2() of one round, eq_n=100,
     the reference's own H2D copies included.  CPU: eq_n candidates per search step, the weight search of a Linear layer
     interrupted after one column block (+ one activation step).  Returns {type: (seconds, units)} and the kind."""
@@ -304,7 +320,7 @@ def reference_cpu_main(a):
             per_step.append({"value": round(v, 3), "job_s": round(job_s, 1), "sample_s": round(sum(s for s, _ in samples.values()), 2),
                              "rates": {k: round(r, 3) for k, r in rates.items()}})
     value = statistics.median(vals)
-    sample = (f"{'unmodified reference classes (baseline/_ref)' if kind == 'reference' else 'oracle port'} on {cores} threads "
+    sample = (f"{'unmodified reference classes (oracle/_ref)' if kind == 'reference' else 'oracle port'} on {cores} threads "
               f"(physical cores, torch.set_num_threads): one seeded synthetic layer per type (qkv, proj, fc1, fc2, head, matmul1, matmul2) at "
               f"the workload's sizes; Linear: one column block of the weight search + the activation search, {a.cpu_eq_n} candidates "
               f"each; MatMul: calibration_step2 with eq_n={a.cpu_eq_n}, one round; extrapolated by unit counts to the whole job; "
@@ -379,6 +395,8 @@ def main():
     sync_all()
     ms = e0.elapsed_time(e1)
     lib.p4v_profile_enable(0)
+    if a.dump_outputs:
+        dump_outputs(work, a.dump_outputs)
     prof = (ctypes.c_double * 12)()
     lib.p4v_profile_collect_kinds(prof, 12)
     launches = _lib.launch_count() - n0
@@ -469,10 +487,10 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    bf16_peak = peaks.get("bf16_tflops_sustained") or 1400.0
-    bf16_burst = peaks.get("bf16_tflops") or 1700.0
+    bf16_peak = peaks.get("bf16_tflops_sustained") or 989.0
+    bf16_burst = peaks.get("bf16_tflops") or 989.0
     peak_src = "MEASURED_PEAKS.json (cuBLAS bf16: sustained inside a long step, burst for a launch alone)" if peaks else \
-        "fallback 1.4 / 1.7 PFLOP/s (B200_PROFILING.md)"
+        "H100 SXM data sheet, dense bf16 989 TFLOP/s at 700 W (not a measured rate)"
     kinds = ["sweep_bf16", "sweep_int8", "gram_gemm"]
     kernels = {"sweep_bf16": "sweep_tc_kernel<f32 accumulators>", "sweep_int8": "sweep_tc_kernel<s32 accumulators>", "gram_gemm": "gram_gemm_kernel"}
     by_kind = {}
@@ -488,26 +506,15 @@ def main():
     top_kind = kinds[int(prof[11])]
     top_peak = bf16_burst * (2.0 if top_kind == "sweep_int8" else 1.0)
     top_ach = prof[10] / (prof[9] / 1e3) / 1e12 if prof[9] > 0 else 0.0
-    # DRAM bytes (read + write) of the longest launch from this round's `ncu --set full` capture (profiles/): a measured
-    # constant of the DEFAULT workload, omitted for any other arguments
-    traffic = None
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        if is_default_workload(a):
-            traffic = tr.get("dominant_launch_dram_bytes")
-    except Exception:
-        tr = {}
     roofline = {"bound": "tensor", "kernel": by_kind[dom]["kernel"], "achieved": by_kind[dom]["achieved"], "peak": by_kind[dom]["peak"],
-                "unit": by_kind[dom]["unit"], "frac": by_kind[dom]["frac"], "traffic": traffic,
-                "traffic_note": tr.get("note") if traffic is not None else "ncu DRAM bytes are recorded for the default workload only",
+                "unit": by_kind[dom]["unit"], "frac": by_kind[dom]["frac"], "traffic": None,
+                "traffic_note": "DRAM bytes not measured",
                 "by_kind": by_kind,
                 "longest_launch": {"kind": top_kind, "ms": prof[9], "achieved": top_ach, "peak": top_peak, "frac": top_ach / top_peak,
-                                   "peak_is": "burst (a launch timed alone)",
-                                   "traffic": tr.get("longest_launch_dram_bytes") if traffic is not None else None},
+                                   "peak_is": "burst (a launch timed alone)", "traffic": None},
                 "note": "achieved = EXECUTED tensor-core operations (slab-incremental search: only the K segment a candidate changes is "
                         "multiplied; Gram GEMM: three bf16 term products) / CUDA-event time of the launches of that kind on this rank; "
-                        "peak = " + peak_src + "; int8 launches are held against 2x the measured bf16 rate (stated, not measured: "
-                        "MEASURED_PEAKS.json has no int8 figure)"}
+                        "peak = " + peak_src + "; int8 launches are held against 2x the bf16 rate (stated, not measured)"}
     out = {"metric": metric_name(a), "value": value, "unit": UNIT, "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
            "ms_per_step": ms / a.steps, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
            "dtype": "int8/bf16-int operands, s32/f32 accumulate, f32 error", "data": "synthetic",

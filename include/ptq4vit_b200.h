@@ -1,4 +1,4 @@
-/* ptq4vit_b200 -- C ABI of the B200-native PTQ4ViT scale-factor search.
+/* ptq4vit_b200 -- C ABI of the H100-native (sm_90a) PTQ4ViT scale-factor search.
  *
  * Drop-in boundary (SURVEY.md section 8b): the reference has no FFI; its operator
  * surface for this path is the Python classes in quant_layers/{linear,matmul}.py.
@@ -27,9 +27,9 @@ extern "C" {
 #endif
 
 #define P4V_OPERAND_AUTO 0
-#define P4V_OPERAND_INT8 1 /* tcgen05.mma kind::i8, s32 accumulators            */
-#define P4V_OPERAND_BF16 2 /* integer-valued bf16, kind::f16, exact f32 accum.   */
-#define P4V_KERNEL_TCGEN05 0
+#define P4V_OPERAND_INT8 1 /* wgmma .s8.s8, s32 accumulators                     */
+#define P4V_OPERAND_BF16 2 /* integer-valued bf16, wgmma .bf16, exact f32 accum. */
+#define P4V_KERNEL_TCGEN05 0 /* the tensor-core (wgmma) sweep; the name is historical */
 #define P4V_KERNEL_SIMT 1 /* plain-CUDA cross-check kernel (bring-up / odd shapes) */
 
 /* One wrapped Linear: mirrors the constructor of PTQSLQuantLinear /

@@ -1,4 +1,4 @@
-"""ptq4vit_b200: B200-native (sm_100a) scale-factor search for PTQ4ViT's quant layers.
+"""ptq4vit_b200: H100-native (sm_90a) scale-factor search for PTQ4ViT's quant layers.
 
 Host side mirrors the reference's operator surface (quant_layers.*, utils.quant_calib,
 configs.PTQ4ViT.get_module); the arithmetic runs in hand-written CUDA behind the C ABI

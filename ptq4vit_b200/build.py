@@ -1,4 +1,4 @@
-"""Build the C-ABI shared library in-tree (nvcc cross-compiles sm_100a without a GPU)."""
+"""Build the C-ABI shared library in-tree (nvcc cross-compiles sm_90a without a GPU)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libptq4vit_b200.so")
 SOURCES = ["sweep_tc.cu", "sweep_simt.cu", "prep.cu", "gram.cu", "gram_gemm.cu", "linear_api.cu", "matmul_api.cu", "conv_api.cu",
            "export.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 
 
@@ -43,7 +44,7 @@ def build(force=False, verbose=False):
         if p.returncode != 0:
             raise RuntimeError(f"nvcc failed on {src}")
     if force or procs or _stale(LIB, objs):
-        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [nvcc, "-shared", "-o", LIB] + objs + GENCODE
         subprocess.check_call(cmd)
     return LIB
 

@@ -1,7 +1,7 @@
-// Shared device/host declarations for the PTQ4ViT scale-factor search on sm_100a.
+// Shared device/host declarations for the PTQ4ViT scale-factor search on sm_90a (H100).
 //
 // Data model (see DESIGN.md):
-//   * "operand image": a quantised matrix [rows][K] stored tile-wise in the tcgen05
+//   * "operand image": a quantised matrix [rows][K] stored tile-wise in the wgmma
 //     no-swizzle K-major canonical layout so that one contiguous bulk copy (TMA 1-D,
 //     cp.async.bulk) lands a ready-to-multiply tile in shared memory:
 //         image[tile][chunk][128 rows][16 bytes]      (chunk = 16 bytes of K)
@@ -9,14 +9,14 @@
 //     activation chunks, each padded to a multiple of 32 bytes) -- inside one
 //     segment both step sizes are constant, so the integer accumulation is exact.
 //   * "job": one <=128-byte-per-row slice of a segment = one shared-memory stage =
-//     up to 4 tcgen05.mma K-steps.  Consecutive jobs of a segment accumulate into
-//     one TMEM accumulator ("group"); the epilogue consumes one accumulator at a time.
+//     up to 4 wgmma K-steps.  Consecutive jobs of a segment accumulate into
+//     one register accumulator ("group"); the epilogue consumes one accumulator at a time.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
 
-#define P4V_TILE 128           // rows per operand tile == UMMA M == UMMA N
+#define P4V_TILE 128           // rows per operand tile == 2 x wgmma M == wgmma N
 #define P4V_JOB_KB 128         // max bytes of K per row and job
 #define P4V_MAX_JOBS 320
 #define P4V_MAX_GROUPS 96
@@ -77,8 +77,6 @@ struct SweepParams {
   int row_keys;             // single-segment steps: one score per ROW, partial = [tile][candidate][column half][128 rows]
   // shared-memory plan, filled by the launcher
   unsigned int stage_r_bytes, stage_c_bytes, n_stages, resident_bytes, resident_bufs, cres_bytes;
-  long long* trace;         // debug: clock64 timeline of CTA 0 ([3 roles][512 events][4]) or null
-  int debug_mode;           // debug (env P4V_SWEEP_DEBUG): 1 = no operand traffic / no MMA (epilogue + handshakes only), 2 = epilogue does no math
 };
 
 static inline __host__ __device__ int p4v_cdiv(int a, int b) { return (a + b - 1) / b; }

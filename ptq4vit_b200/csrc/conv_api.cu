@@ -39,7 +39,7 @@ int build_plan(const p4v_conv_desc* d, ConvPlan& p) {
   P4V_REQUIRE(p.P > 0 && p.O > 0 && p.K > 0 && p.L > 0, "conv: empty shape");
   P4V_REQUIRE(d->w_bit >= 2 && d->w_bit <= 8, "conv: w_bit must be in [2,8]");
   P4V_REQUIRE(d->eq_n >= 1 && d->eq_n <= P4V_MAX_CAND, "conv: eq_n must be in [1,%d]", P4V_MAX_CAND);
-  P4V_REQUIRE(d->kernel == P4V_KERNEL_TCGEN05, "conv: the channel-wise search runs on the tcgen05 kernel only");
+  P4V_REQUIRE(d->kernel == P4V_KERNEL_TCGEN05, "conv: the channel-wise search runs on the tensor-core kernel only");
   p.w_qmax = 1 << (d->w_bit - 1);
   p.tiles_o = p4v_cdiv(p.O, P4V_TILE); p.tiles_l = p4v_cdiv(p.L, P4V_TILE);
   p.kb = (int)align_up((size_t)p.K * 2, 32);                    // bf16 row bytes of one term
@@ -142,7 +142,7 @@ extern "C" int p4v_conv_calibrate(const p4v_conv_desc* d, const float* cols, con
   conv_fill_kernel<<<p4v_cdiv(d->eq_n, 128), 128, 0, st>>>(at<float>(ws, p.o_candA), at<float>(ws, p.o_factors), d->eq_n, at<float>(ws, p.o_candB));
   p4v_count_launch();
   const long long n = (long long)p.P * p.O * p.L;
-  conv_prescale_kernel<<<148 * 8, 256, 0, st>>>(raw_out, raw_grad, d->has_bias ? bias : nullptr, at<float>(ws, p.o_d0), p.O, p.L, n,
+  conv_prescale_kernel<<<132 * 8, 256, 0, st>>>(raw_out, raw_grad, d->has_bias ? bias : nullptr, at<float>(ws, p.o_d0), p.O, p.L, n,
                                                  at<float>(ws, p.o_Y), at<float>(ws, p.o_G));
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());

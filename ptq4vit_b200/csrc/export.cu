@@ -75,7 +75,7 @@ extern "C" int p4v_export_quantized(const float* src, long long rows, long long 
                mode, (float)(1 << (bit - 1)), d_neg, split, p4v_scalar_div_ieee()};
   const long long n = rows * cols;
   long long blocks = (n / 16 + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   if (blocks < 1) blocks = 1;
   export_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(a); p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());

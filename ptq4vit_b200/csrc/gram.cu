@@ -80,11 +80,11 @@ __global__ void pair_image_kernel(const int8_t* __restrict__ XqT, int Mp, int M,
   *reinterpret_cast<uint4*>(base_p + (size_t)term_bytes * GRAM_PT) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
 }
 
-// packed fp32x2 math (sm_100): one issue slot per two FMAs
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pack2(float a, float b) { f32x2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void unpack2(f32x2 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { f32x2 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
+// fp32 pairs: two independent fma.rn chains per pair (the even and odd k of the slab), summed in a fixed order
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 pack2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void unpack2(f32x2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 // D[o][k] = what the previous step's pick changed in the quantised weights of its column block (ks numbers per channel)
 __global__ void gram_delta_kernel(const float* __restrict__ W, int O, int K, int k_prev, int ks, int ldD,
@@ -120,7 +120,7 @@ __global__ void __launch_bounds__(256, 2) gram_update_kernel(const GramUpdateArg
   const int m_end = min(a.M, (int)((long long)nb16 * (blockIdx.y + 1) / gridDim.y) * 16);
   f32x2 dd[KS / 2], acc[KS / 2];
 #pragma unroll
-  for (int k = 0; k < KS / 2; ++k) { dd[k] = 0ull; acc[k] = 0ull; }
+  for (int k = 0; k < KS / 2; ++k) { dd[k] = pack2(0.f, 0.f); acc[k] = pack2(0.f, 0.f); }
   if (has_prev && ok_o) {
 #pragma unroll
     for (int k = 0; k < KS; k += 4) {
@@ -179,7 +179,7 @@ __global__ void __launch_bounds__(256, 2) gram_update_kernel(const GramUpdateArg
         if (mm < rows) {
           float ev = ec[u];
           if (has_prev) {
-            f32x2 s0 = 0ull, s1 = 0ull;
+            f32x2 s0 = pack2(0.f, 0.f), s1 = pack2(0.f, 0.f);
 #pragma unroll
             for (int k = 0; k < KS; k += 4) {
               const float4 xv = *reinterpret_cast<const float4*>(&xp[mm * KS + k]);

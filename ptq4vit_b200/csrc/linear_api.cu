@@ -81,10 +81,7 @@ static double sweep_ops(const SweepParams& sp, const P4VJob* host_jobs) {
   const double tiles = (double)sp.P * sp.tiles_m * sp.tiles_n;
   return 2.0 * P4V_TILE * P4V_TILE * tiles * (kf + kc * sp.n_cand);
 }
-static long long* g_trace = nullptr;
-extern "C" __attribute__((visibility("default"))) int p4v_debug_trace(void* dev_ptr) { g_trace = (long long*)dev_ptr; return 0; }
-int p4v_run_sweep(const SweepParams& sp_in, const P4VJob* host_jobs, int kernel, cudaStream_t st) {
-  SweepParams sp = sp_in; sp.trace = g_trace;
+int p4v_run_sweep(const SweepParams& sp, const P4VJob* host_jobs, int kernel, cudaStream_t st) {
   ++g_launches;
   cudaEvent_t e0 = nullptr;
   if (g_prof) p4v_prof_begin(st, &e0);
@@ -103,8 +100,8 @@ int p4v_num_sms() {
   static int sms = 0;
   if (sms == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
 }

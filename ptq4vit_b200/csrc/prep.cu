@@ -337,7 +337,7 @@ __global__ void commit_step_kernel(const CommitArgs a, int chunks_total) {
   }
 }
 
-int grid_for(long long total, int block, int cap = 148 * 16) {
+int grid_for(long long total, int block, int cap = 132 * 16) {
   long long g = (total + block - 1) / block;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
@@ -434,7 +434,7 @@ extern "C" int p4v_selftest_rint_div(unsigned long long n, unsigned long long se
   unsigned long long* d = nullptr;
   P4V_CUDA_OK(cudaMalloc(&d, 8));
   P4V_CUDA_OK(cudaMemsetAsync(d, 0, 8, st));
-  rint_div_selftest_kernel<<<148 * 8, 256, 0, st>>>(n, seed, d); p4v_count_launch();
+  rint_div_selftest_kernel<<<132 * 8, 256, 0, st>>>(n, seed, d); p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   P4V_CUDA_OK(cudaMemcpyAsync(mismatches, d, 8, cudaMemcpyDeviceToHost, st));
   P4V_CUDA_OK(cudaStreamSynchronize(st));
@@ -489,7 +489,7 @@ int p4v_select_step(const SelectArgs& a, cudaStream_t st) {
 int p4v_commit_step(const CommitArgs& a, cudaStream_t st) {
   if (a.nseg <= 0) return 0;
   const long long total = (long long)a.P * a.tiles * P4V_TILE * a.commit_chunks;
-  commit_step_kernel<<<grid_for(total, 256, 148 * 8), 256, 0, st>>>(a, a.commit_chunks); p4v_count_launch();
+  commit_step_kernel<<<grid_for(total, 256, 132 * 8), 256, 0, st>>>(a, a.commit_chunks); p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   return 0;
 }

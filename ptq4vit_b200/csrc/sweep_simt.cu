@@ -1,6 +1,6 @@
 // Plain-CUDA (no tensor core) evaluation of the same candidate sweep, same inputs,
 // same partial-score layout as sweep_tc.cu.  It exists for two reasons:
-//   * bring-up / bisecting: tests compare oracle <-> simt <-> tcgen05;
+//   * bring-up / bisecting: tests compare oracle <-> simt <-> tensor-core kernel;
 //   * geometries the tensor-core kernel does not take.
 // It is a GPU path (selected with desc.kernel = 1), never a CPU fallback.
 #include "common.cuh"

@@ -137,7 +137,7 @@ class ChannelwiseBatchingQuantConv2d(PTQSLQuantConv2d):
         """reference: conv.py:591-603.  The weight search does not depend on anything the rounds change when the
         activations are not quantized, so its result is the same in every round: it is run once."""
         if self.a_bit < 32:
-            raise NotImplementedError("ChannelwiseBatchingQuantConv2d: the B200 path implements a_bit >= 32 "
+            raise NotImplementedError("ChannelwiseBatchingQuantConv2d: the CUDA path implements a_bit >= 32 "
                                       "(activation quantizer off), as configs/PTQ4ViT.py:54 uses it")
         if self.groups != 1 or self.init_layerwise:
             raise NotImplementedError("ChannelwiseBatchingQuantConv2d: groups == 1 and init_layerwise=False only")

@@ -199,7 +199,7 @@ class PTQSLQuantLinear(MinMaxQuantLinear):
         self.crb_rows = out_features // n_V
         self.crb_cols = in_features // n_H  # ignore remnent != 0 situations
         self.crb_acts = in_features // n_a
-        self.parallel_eq_n = parallel_eq_n   # kept for signature parity; the B200 path holds a whole layer in HBM
+        self.parallel_eq_n = parallel_eq_n   # kept for signature parity; the CUDA path holds a whole layer in HBM
         self.init_layerwise = init_layerwise
         self.raw_grad = None
         self.last_scores = None              # optional per-step score tables (set P4V_SCORE_LOG=1 or keep_scores=True)
@@ -273,7 +273,7 @@ class PTQSLBatchingQuantLinear(PTQSLQuantLinear):
         self.calib_need_batching = False
 
     def _initialize_calib_parameters(self):
-        """reference: linear.py:365-378.  180 GB of HBM hold a whole layer: no batching."""
+        """reference: linear.py:365-378.  80 GB of HBM hold a whole layer: no batching."""
         self.calib_size = int(self.raw_input.shape[0])
         self.calib_batch_size = int(self.raw_input.shape[0])
         self.calib_need_batching = False

@@ -131,7 +131,7 @@ class MinMaxQuantMatMul(nn.Module):
 
 class PTQSLQuantMatMul(MinMaxQuantMatMul):
     """reference: quant_layers/matmul.py:62-282.  Block structure: only the head-wise layout that
-    the Batching classes force (n_G = heads, n_V = n_H = 1) is implemented by the B200 path."""
+    the Batching classes force (n_G = heads, n_V = n_H = 1) is implemented by the CUDA path."""
 
     def __init__(self, A_bit=8, B_bit=8, mode="raw", metric="L2_norm", search_round=1, eq_alpha=0.1, eq_beta=2,
                  eq_n=100, parallel_eq_n=10, n_G_A=1, n_V_A=1, n_H_A=1, n_G_B=1, n_V_B=1, n_H_B=1, init_layerwise=False):
@@ -157,7 +157,7 @@ class PTQSLQuantMatMul(MinMaxQuantMatMul):
     _force_headwise = False       # the Batching classes set n_G = heads (matmul.py:411-417)
 
     def _get_padding_parameters(self, A, B):
-        """reference: matmul.py:109-122 (groups of consecutive heads, zero padding).  The B200 path implements the two
+        """reference: matmul.py:109-122 (groups of consecutive heads, zero padding).  The CUDA path implements the two
         layouts PTQ4ViT meets: one group per head (what the Batching classes force, :411-417) and one group for all
         heads (the constructor default n_G = 1 of the non-batching classes)."""
         H = A.shape[1]

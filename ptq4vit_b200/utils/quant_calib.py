@@ -2,7 +2,7 @@
 
 `HessianQuantCalibrator(net, wrapped_modules, calib_loader, sequential=False, batch_size=1)
 .batching_quant_calib()` is the entry point the reference's experiments time
-(example/test_all.py:31-34).  B200-first changes, results unchanged:
+(example/test_all.py:31-34).  GPU-first changes, results unchanged:
 
 * capture: with sequential=False every module stays in "raw" mode while the others calibrate
   (quant_calib.py:369-372), so the captured (input, output, grad) tensors do not depend on the
@@ -82,17 +82,18 @@ def _cat_captured(module):
 
 
 # ---------------------------------------------------------------- work model + sharding
-# Measured on a B200 (profiles/README.md, round 2; ViT-B/224 x 32 images, one search round): qkv 11.4 ms, proj 5.9 ms,
-# fc1 14.3 ms, fc2 16.7 ms, head 2.7 ms, matmul1 6.0 ms, matmul2 5.0 ms, patch-embedding conv 5.1 ms (once).  A fixed
-# part per module and round (operand images, per-step launches) plus executed work at the rate each kernel family sustains.
-_ROUND_OVERHEAD_S = 2.5e-3
-_LINEAR_RATE = 4.2e14      # "units" below per second: eq_n * 2*M*K*O * (1 + n_a)
-_MATMUL_RATE = 1.1e14      # 2 * eq_n * 2*b*H*S1*S2*S3 per second (197-token tiles are 59 % full)
+# Measured on an H100 80GB HBM3 at a 400 W power limit (ViT-B/224 x 32 images, W8A8, one search round): qkv 20.9 ms,
+# proj 10.3 ms, fc1 27.1 ms, head 3.1 ms, matmul1 7.7 ms.  A fixed part per module and round (operand images, per-step
+# launches) plus executed work at the rate each kernel family sustains.  The conv rate is not measured on the H100; it only
+# places the single patch-embedding module.
+_ROUND_OVERHEAD_S = 4.7e-3
+_LINEAR_RATE = 2.66e14     # "units" below per second: eq_n * 2*M*K*O * (1 + n_a)
+_MATMUL_RATE = 1.29e14     # 2 * eq_n * 2*b*H*S1*S2*S3 per second (197-token tiles are 59 % full)
 _CONV_RATE = 1.5e13        # eq_n * 2 * MACs per second (three bf16 term products per MAC)
 
 
 def module_cost(module, n_img, shapes=None, tokens_hint=197):
-    """Estimated seconds of one module's search on a B200 (only ratios matter for the sharding).
+    """Estimated seconds of one module's search on an H100 (only ratios matter for the sharding).
     Linear  : rounds * (overhead + eq_n * 2*M*K*O * (1 [all weight steps together multiply each K slab once] + n_a) / rate)
     MatMul  : rounds * (overhead + 2 * eq_n * 2*b*H*S1*S2*S3 / rate)
     `shapes` = per-image input shapes recorded by a probe forward ({"x": (lead, tokens.., K)} / {"A": (lead, H, S1, S2), ...});

@@ -2,10 +2,11 @@
 .batching_quant_calib()` on a 2-block synthetic ViT, against
 
   * the UNMODIFIED reference calibrator (utils/quant_calib.py:300-378 + utils/net_wrap.py + configs/PTQ4ViT.py from
-    baseline/_ref) running on the same GPU: captured x / y / grad tensors and every chosen step size;
-  * tests/golden/calib_tiny_vit.npz (the same reference run, CPU, dev container) -- the check that remains when the
-    staged tree is absent.  CPU and GPU capture numerics differ in the last bits, so near-tie picks may move by a grid
-    step: the comparison counts differing entries.
+    oracle/_ref, staged by build()) running on the same GPU: captured x / y / grad tensors and every chosen step size;
+  * tests/golden/calib_tiny_vit_gpu.npz (the same reference run on the GPU, tests/golden/make_calib_gpu_golden.py:
+    step sizes and a seeded sample of every captured tensor) where the reference is not installed;
+  * tests/golden/calib_tiny_vit.npz (the same reference run on the CPU).  CPU and GPU capture numerics differ in the
+    last bits, so near-tie picks may move by a grid step: the comparison counts differing entries.
 
 Also: single-pass capture == the reference's one-sweep-per-module capture (SURVEY.md 8f rank 1), sequential=True works
 (gradients reach the modules behind an already quantized layer), QuantCalibrator.{parallel,sequential}_quant_calib and
@@ -13,6 +14,7 @@ the base batching_quant_calib run on the non-batching / L2 configurations.
 """
 import importlib
 import os
+import zlib
 
 import numpy as np
 import pytest
@@ -24,10 +26,19 @@ from oracle import ref_harness as RH
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "calib_tiny_vit.npz")
+GOLD_GPU = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "calib_tiny_vit_gpu.npz")
+CAPTURE_SAMPLE = 2048
 GRID = (1.2 - 0.01) / 100
 
 
 TINY_SWIN = dict(img_size=32, patch=4, dim=32, depths=(2, 2), num_heads=(2, 4), window_size=4, num_classes=10)
+
+
+@pytest.fixture(autouse=True)
+def _fp32_convolutions():
+    """Both calibrators capture through the net's patch-embedding convolution: compared in fp32 (no TF32)."""
+    with RH.fp32_convolutions():
+        yield
 
 
 def _net(kind="vit"):
@@ -73,10 +84,16 @@ def _count_diff(got, ref, what, max_frac, max_steps=3):
     return bad, n
 
 
+def sample_capture(numel, name, key):
+    """Fixed flat indices (sorted, without repetition) of the stored sample of captured tensor `name.key`."""
+    rng = np.random.default_rng(zlib.crc32(f"{name}|{key}".encode()))
+    return np.sort(rng.choice(numel, size=min(numel, CAPTURE_SAMPLE), replace=False)).astype(np.int64)
+
+
 def _as_dict(npz, prefix):
     out = {}
     for k in npz.files:
-        p, name, key = k.split("|")
+        p, name, key = k.split("|")[:3]
         if p == prefix:
             out.setdefault(name, {})[key] = torch.from_numpy(npz[k])
     return out
@@ -86,17 +103,29 @@ def test_batching_quant_calib_matches_reference_calibrator_on_gpu():
     snap_ours, snap_ref = {}, {}
     got, net, wrapped, cal = _ours(keep=snap_ours)
     assert cal.timings["single_pass"] and cal.timings["total_s"] > 0
-    if not RH.available():
-        pytest.skip("baseline/_ref not staged: covered by the golden comparison below")
-    ref, _, wrapped_r = RH.run_reference_calibrator(_net(), RH.tiny_images(), batch_size=4, sequential=False, snapshot=snap_ref)
-    # captured tensors: same net, same ops, same device
     worst = 0.0
-    for name, d in snap_ours.items():
-        for key, t in d.items():
-            r = snap_ref[name][key].to(t.device)
-            err = float((t - r).abs().max() / (r.abs().max() + 1e-30))
-            worst = max(worst, err)
-            assert err < 1e-4, f"captured {name}.{key} differs from the reference's capture: {err:.2e}"
+    if RH.available():
+        ref, _, wrapped_r = RH.run_reference_calibrator(_net(), RH.tiny_images(), batch_size=4, sequential=False, snapshot=snap_ref)
+        # captured tensors: same net, same ops, same device
+        for name, d in snap_ours.items():
+            for key, t in d.items():
+                r = snap_ref[name][key].to(t.device)
+                err = float((t - r).abs().max() / (r.abs().max() + 1e-30))
+                worst = max(worst, err)
+                assert err < 1e-4, f"captured {name}.{key} differs from the reference's capture: {err:.2e}"
+    else:
+        # the same reference run on the GPU, stored: step sizes and a seeded sample of every captured tensor
+        z = np.load(GOLD_GPU)
+        ref = _as_dict(z, "par")
+        for name, d in snap_ours.items():
+            for key, t in d.items():
+                if t is None:
+                    continue
+                r = torch.from_numpy(z[f"cap|{name}|{key}|val"])
+                mine = t.detach().reshape(-1).float().cpu()[torch.from_numpy(sample_capture(t.numel(), name, key))]
+                err = float((mine - r).abs().max() / (float(z[f"cap|{name}|{key}|max"]) + 1e-30))
+                worst = max(worst, err)
+                assert err < 1e-4, f"captured {name}.{key} differs from the reference's capture: {err:.2e}"
     bad, n = _count_diff(got, ref, "vs reference on GPU", max_frac=0.05)
     print(f"[calibrator parity] {len(snap_ours)} modules, captured tensors worst rel diff {worst:.2e}; {bad}/{n} step sizes differ")
     # the calibrated nets agree on the calibration images
@@ -109,7 +138,7 @@ def test_swin_windowed_attention_and_reduction_match_reference_calibrator():
     """BASELINE.json configs[4] geometry in small: shifted windows, window attention MatMuls with the batch dimension
     images x windows (reference utils/models.py:28-56) and the `reduction` Linear of patch merging (utils/net_wrap.py:42)."""
     if not RH.available():
-        pytest.skip("needs the staged reference (baseline/_ref)")
+        pytest.skip("needs the reference staged by build() (oracle/_ref)")
     snap_ours, snap_ref = {}, {}
     got, net, wrapped, cal = _ours(keep=snap_ours, kind="swin")
     assert any(n.endswith("downsample.reduction") for n in wrapped) and any("layers.0.blocks.1.attn.matmul1" == n for n in wrapped)
@@ -214,7 +243,7 @@ def test_hessian_quant_calib_non_batching_driver_matches_reference():
     sweep, then `calibration_step2(x)` / `(A, B)` of the NON-batching classes with the hessian metric -- against the
     reference's same driver on its own non-batching classes (Linear and MatMul modules; both nets wrapped by hand)."""
     if not RH.available():
-        pytest.skip("needs the staged reference (baseline/_ref)")
+        pytest.skip("needs the reference staged by build() (oracle/_ref)")
     import copy
     from ptq4vit_b200.quant_layers import linear as L, matmul as M
     from ptq4vit_b200.utils import quant_calib as Q

@@ -71,7 +71,8 @@ def test_vitb_patch_embedding_matches_reference_on_gpu(bit):
         ref = RH.run_conv(x, W, b, y, g, stride=16, search_round=1, w_bit=bit)
         ref_w, ref_scores, kind, ref_s = ref["w_interval"].numpy(), ref["scores"][0].numpy(), "reference", ref["seconds"]
     else:
-        wi, sc = O.conv_calibrate(W.cuda(), b.cuda(), x.cuda(), y.cuda(), g.cuda(), stride=16, w_bit=bit)
+        with RH.fp32_convolutions():
+            wi, sc = O.conv_calibrate(W.cuda(), b.cuda(), x.cuda(), y.cuda(), g.cuda(), stride=16, w_bit=bit)
         ref_w, ref_scores, kind, ref_s = wi.cpu().numpy(), sc.cpu().numpy(), "oracle-on-device", float("nan")
     m = _ours(x, W, b, y, g, stride=16, w_bit=bit)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

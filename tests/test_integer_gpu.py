@@ -1,5 +1,5 @@
 """Integer export (SURVEY.md 8f rank 3): ptq4vit_b200.utils.integer against the reference's utils/integer.py functions
-running on the same GPU (baseline/_ref) and against the oracle's restatement of their formulas."""
+running on the same GPU (oracle/_ref) and against the oracle's restatement of their formulas."""
 import pytest
 import torch
 

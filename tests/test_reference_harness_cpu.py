@@ -1,6 +1,6 @@
 """Checks of the test / baseline infrastructure itself on the CPU (dev container): the oracle's restatements of
 utils/integer.py against the reference's functions, the reference timing helpers bench.py uses, and bench.py's unit /
-extrapolation arithmetic.  Skipped where neither baseline/_ref nor /root/reference exists."""
+extrapolation arithmetic.  The reference checks need the copy build() stages under oracle/_ref."""
 import argparse
 
 import pytest
@@ -73,11 +73,11 @@ def test_module_cost_uses_probed_shapes():
     mm = M.PTQSLBatchingQuantMatMul(search_round=3)
     cm = Q.module_cost(mm, 32, {"A": (64, 4, 144, 32), "B": (64, 4, 32, 144)})
     assert abs(cm - 3 * (Q._ROUND_OVERHEAD_S + 2 * 100 * 2.0 * 32 * 64 * 4 * 144 * 32 * 144 / Q._MATMUL_RATE)) < 1e-9
-    # ViT-B/224 x 32 images at n_V = n_H = 24: the model reproduces the measured per-round times within 20 %
+    # ViT-B/224 x 32 images at n_V = n_H = 24: the model reproduces the per-round times measured on an H100 within 20 %
     qkv = L.PTQSLBatchingQuantLinear(768, 2304, n_V=72, n_H=24, search_round=1)
     qk = M.PTQSLBatchingQuantMatMul(search_round=1)
-    assert abs(Q.module_cost(qkv, 32, {"x": (1, 197, 768)}) / 11.4e-3 - 1) < 0.2
-    assert abs(Q.module_cost(qk, 32, {"A": (1, 12, 197, 64), "B": (1, 12, 64, 197)}) / 6.0e-3 - 1) < 0.2
+    assert abs(Q.module_cost(qkv, 32, {"x": (1, 197, 768)}) / 20.9e-3 - 1) < 0.2
+    assert abs(Q.module_cost(qk, 32, {"A": (1, 12, 197, 64), "B": (1, 12, 64, 197)}) / 7.7e-3 - 1) < 0.2
 
 
 @needs_ref

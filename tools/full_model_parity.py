@@ -1,8 +1,8 @@
 """GPU box: calibrate a whole synthetic ViT (timm names, ptq4vit_b200.utils.models) twice -- with the UNMODIFIED
-reference (its own net_wrap / configs/PTQ4ViT.py / HessianQuantCalibrator.batching_quant_calib from baseline/_ref) and with
+reference (its own net_wrap / configs/PTQ4ViT.py / HessianQuantCalibrator.batching_quant_calib from oracle/_ref) and with
 this package -- and compare every step size of every wrapped module.  BASELINE.json configs[1]: ViT-S/224, 32 images,
 reference defaults (n_V = n_H = 1, qkv n_V = 3, 3 rounds, hessian, W8A8).
-usage: full_model_parity.py [model] [images] [n_V=n_H] > profiles/r02_full_model_parity_<model>.json"""
+usage: full_model_parity.py [model] [images] [n_V=n_H] > full_model_parity_<model>.json"""
 import importlib
 import json
 import os
