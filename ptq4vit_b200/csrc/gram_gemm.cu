@@ -44,14 +44,23 @@ __device__ __forceinline__ bool mbar_try(uint32_t addr, uint32_t parity) {
                : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
   return ok != 0;
 }
-__device__ __noinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity) {     // bounded: a protocol bug traps, never hangs
+// Bounded: a protocol bug traps, never hangs.  Inline and call-free (a call splits the wgmma pipeline, C7510); on timeout
+// (block << 32 | thread << 20 | barrier smem address) is left in g_gram_timeout, and printed with -DP4V_SWEEP_DEBUG_PRINTF.
+__device__ unsigned long long g_gram_timeout;
+[[noreturn]] __device__ __forceinline__ void mbar_timeout(uint32_t addr, uint32_t parity) {
+  g_gram_timeout = ((unsigned long long)blockIdx.x << 32) | ((unsigned long long)threadIdx.x << 20) | (addr & 0xFFFFFu);
+  __threadfence();
+#ifdef P4V_SWEEP_DEBUG_PRINTF
+  printf("ptq4vit gram gemm: mbarrier wait timed out (block %d thread %d smem 0x%x parity %u)\n", (int)blockIdx.x,
+         (int)threadIdx.x, addr, parity);
+#endif
+  __trap();
+  while (true) {}
+}
+__device__ __forceinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity) {
   const long long t0 = clock64();
   while (!mbar_try(addr, parity))
-    if (clock64() - t0 > 20000000000ll) {
-      printf("ptq4vit gram gemm: mbarrier wait timed out (block %d thread %d smem 0x%x parity %u)\n", (int)blockIdx.x,
-             (int)threadIdx.x, addr, parity);
-      __trap();
-    }
+    if (clock64() - t0 > 20000000000ll) mbar_timeout(addr, parity);
 }
 __device__ __forceinline__ void mbar_wait(void* bar, uint32_t parity) {
   const uint32_t addr = smem_u32(bar);
@@ -157,13 +166,20 @@ __global__ void __launch_bounds__(kThreads, 1) gram_gemm_kernel(const __grid_con
       const uint32_t s0 = ring + stage * kStageBytes;
       const uint64_t rhi = make_desc(s0) + a_off, rlo = make_desc(s0 + kTerm) + a_off;
       const uint64_t chi = make_desc(s0 + 2 * kTerm), clo = make_desc(s0 + 3 * kTerm);
-      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
-      for (uint32_t ks = 0; ks * 32 < kb; ++ks) {          // one K step = 16 bf16 = two 16-byte chunks
+      // one K step = 16 bf16 = two 16-byte chunks; a stage holds two (kb = 64) or, at the end of a term, one (kb = 32).
+      // Each case is one straight-line batch: a loop or branch between the wgmmas of a batch makes ptxas wait for each
+      // one before issuing the next (C7520).
+      auto kstep = [&](const uint32_t ks, const uint32_t accumulate) {
         const uint64_t k16 = ks * ((2u * 128 * 16) >> 4);
-        wgmma_bf16(acc, rhi + k16, chi + k16, (!first || ks) ? 1u : 0u);
+        wgmma_bf16(acc, rhi + k16, chi + k16, accumulate);
         wgmma_bf16(acc, rhi + k16, clo + k16, 1u);
         wgmma_bf16(acc, rlo + k16, chi + k16, 1u);
-      }
+      };
+      // (the count is broadcast from lane 0 after the per-lane spin wait, so that ptxas can prove the branch warp-uniform)
+      const bool two = __shfl_sync(0xffffffffu, kb == kStageKB ? 1 : 0, 0) != 0;
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+      if (two) { kstep(0, first ? 0u : 1u); kstep(1, 1u); }
+      else     { kstep(0, first ? 0u : 1u); }
       asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
       asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
       __syncwarp();

@@ -20,9 +20,11 @@
 // accumulator each (P4VJob::nsub); operands that do not change between candidates stay resident in shared memory.
 // Roles: warp 0 = bulk-copy producer; warpgroups 1-2 = consumers, each issuing wgmma m64n128 for its 64 rows of the
 // tile and running the epilogue on the fragment it holds.  The two consumer warpgroups share the tensor cores: while
-// one runs its epilogue the other's MMAs proceed.  Every thread has the launch budget of 168 registers (384 threads);
-// the consumers hold r and the accumulator (128 registers) and spill ~250 bytes per thread (ptxas -v).  ptxas serialises
-// the wgmma sequences (C7520), which costs nothing here: every sequence is waited for before its accumulator is read.
+// one runs its epilogue the other's MMAs proceed.  The launch budget is 168 registers per thread (384 threads); setmaxnreg
+// moves it to the consumers (warpgroup 0: 56, consumers: 224), which hold r and the accumulator (128 registers) without
+// spilling (ptxas -v: 0 bytes).  That needs a kernel without calls (ptxas drops setmaxnreg otherwise, C7507): the
+// bounded mbarrier wait is inline and the scheduler divides in 32 bits.  The k32 steps of a stage are issued as one
+// straight-line batch selected by a warp-uniform count, so ptxas pipelines them instead of waiting on each (C7520).
 #include "common.cuh"
 #include <algorithm>
 #include <cstdio>
@@ -75,14 +77,21 @@ __device__ __forceinline__ bool mbar_try(uint32_t addr, uint32_t parity) {
 }
 // Bounded wait: a protocol bug must surface as a trapped launch (cudaErrorLaunchFailure), never as a hung GPU.  The bound
 // is ~10 s of SM clocks: clock64 keeps counting while a context is time-sliced, a legitimate wait of a sub-millisecond
-// kernel must never reach it.
-[[noreturn]] __device__ __noinline__ void mbar_timeout(uint32_t addr, uint32_t parity) {
+// kernel must never reach it.  The wait is inline and makes no call: a call anywhere in the kernel makes ptxas ignore
+// setmaxnreg (C7507).  On timeout it leaves (block << 32 | thread << 20 | barrier smem address) in g_sweep_timeout for
+// a debugger-free post-mortem; building with -DP4V_SWEEP_DEBUG_PRINTF also prints it.
+__device__ unsigned long long g_sweep_timeout;
+[[noreturn]] __device__ __forceinline__ void mbar_timeout(uint32_t addr, uint32_t parity) {
+  g_sweep_timeout = ((unsigned long long)blockIdx.x << 32) | ((unsigned long long)threadIdx.x << 20) | (addr & 0xFFFFFu);
+  __threadfence();
+#ifdef P4V_SWEEP_DEBUG_PRINTF
   printf("ptq4vit sweep: mbarrier wait timed out (block %d thread %d smem 0x%x parity %u)\n",
          (int)blockIdx.x, (int)threadIdx.x, addr, parity);
+#endif
   __trap();
   while (true) {}
 }
-__device__ __noinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity) {
+__device__ __forceinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity) {
   const long long t0 = clock64();
   while (!mbar_try(addr, parity))
     if (clock64() - t0 > 20000000000ll) mbar_timeout(addr, parity);
@@ -146,19 +155,47 @@ __device__ __forceinline__ void wgmma_k32(uint32_t (&d)[64], uint64_t da, uint64
                "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 " P4V_WG_D64 ", %64, %65, p;\n\t}"
                : P4V_WG_OP64(P4V_R) : "l"(da), "l"(db), "r"(accumulate));
 }
+// One stage = nk (1..4) k32 steps, issued as one committed batch.  Each count has its own straight-line sequence: a
+// data-dependent branch between the wgmmas of a batch makes ptxas wait for each one before issuing the next (C7520).
+template <int N, typename AccT>
+__device__ __forceinline__ void wgmma_seq(AccT (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  wgmma_k32(d, da, db, accumulate);
+#pragma unroll
+  for (int k = 1; k < N; ++k) wgmma_k32(d, da + 256 * k, db + 256 * k, 1u);   // +32 bytes of K = 2 x 128 rows x 16 B
+}
+template <typename AccT>
+__device__ __forceinline__ void wgmma_stage(AccT (&d)[64], uint32_t nk, uint64_t da, uint64_t db, uint32_t accumulate) {
+  wg_fence();
+  switch (nk) {
+    case 1: wgmma_seq<1>(d, da, db, accumulate); break;
+    case 2: wgmma_seq<2>(d, da, db, accumulate); break;
+    case 3: wgmma_seq<3>(d, da, db, accumulate); break;
+    default: wgmma_seq<4>(d, da, db, accumulate); break;
+  }
+  wg_commit();
+}
+
+// Register reallocation between the warpgroups (all four warps of a warpgroup execute it): the producer warpgroup
+// gives registers back, the consumer warpgroups take them.  128 * 56 + 256 * 224 = 384 * 168, the launch budget.
+// ptxas -v: no spills in any instantiation (40 / 232 leaves the producer spilling 12-20 bytes).
+constexpr int kProducerRegs = 56, kConsumerRegs = 224;
+__device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs)); }
+__device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs)); }
 
 // ---- work distribution -------------------------------------------------------------------------
 struct Frag { int tile, p, tm, tn, c0, c1; };
+// The tail wave has fewer than gridDim.x (<= SM count) tiles of at most P4V_MAX_CAND candidates, so its unit arithmetic
+// fits 32 bits (and compiles to inline code: a 64-bit division is a subroutine call, which would void setmaxnreg).
 struct Sched {
   int waves, k;                 // whole-tile waves, next wave index
-  long long u, u_end;           // candidate-granular units of the tail wave
+  unsigned u, u_end;            // candidate-granular units of the tail wave
   int tail_tile0;
 };
 __device__ __forceinline__ void sched_init(const SweepParams& P, Sched& s) {
   const int tiles = P.P * P.tiles_m * P.tiles_n;
   const int G = gridDim.x;
   s.waves = tiles / G; s.k = 0;
-  const long long tail_units = (long long)(tiles % G) * P.n_cand;
+  const unsigned tail_units = (unsigned)(tiles % G) * (unsigned)P.n_cand;
   s.u = tail_units * blockIdx.x / G; s.u_end = tail_units * (blockIdx.x + 1) / G;
   s.tail_tile0 = s.waves * G;
 }
@@ -169,8 +206,8 @@ __device__ __forceinline__ bool next_frag(const SweepParams& P, Sched& s, Frag& 
     if (s.u >= s.u_end) return false;
     f.tile = s.tail_tile0 + (int)(s.u / P.n_cand);
     f.c0 = (int)(s.u % P.n_cand);
-    const long long rem = s.u_end - s.u;
-    f.c1 = (int)((rem < (long long)(P.n_cand - f.c0)) ? f.c0 + rem : P.n_cand);
+    const unsigned rem = s.u_end - s.u;
+    f.c1 = (rem < (unsigned)(P.n_cand - f.c0)) ? f.c0 + (int)rem : P.n_cand;
     s.u += f.c1 - f.c0;
   }
   const int per_p = P.tiles_m * P.tiles_n;
@@ -234,6 +271,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
   Frag f;
 
   if (warp < 4) {
+    regs_dec();
     if (warp != 0) return;
     // ======================= bulk-copy producer (whole warp runs the loop, one elected lane issues) =======================
     uint32_t stage = 0, phase = 0, rbuf = 0, rphase = 0, cphase = 0;
@@ -294,6 +332,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
   // Registers hold the residual r and the accumulator fragment.  This thread's slice of shared memory ([fragment value
   // pair][consumer thread] float2) parks g in single-segment steps and, in multi-segment steps, the residual every
   // candidate starts from (g is then read from global memory once per candidate).
+  regs_inc();
   const int et = threadIdx.x - 128;                  // 0..255
   const int wg = et >> 7;                            // row half of the tile
   const int cw = et >> 5;                            // consumer warp 0..7 = 16-row slice
@@ -321,12 +360,11 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
     uint32_t b16 = (flags & P4V_JOB_CRES) ? resC16 + (jb.c_off >> 4) : ringC16 + stage * sC16;
     for (uint32_t sub = 0; sub < nsub; ++sub) {
       const uint64_t da = dconst | (uint64_t)a16, db = dconst | (uint64_t)b16;
-      wg_fence();
-      wgmma_k32(acc, da, db, (flags & P4V_JOB_FIRST) ? 0u : 1u);
-      if (kb > 32) wgmma_k32(acc, da + 256, db + 256, 1u);
-      if (kb > 64) wgmma_k32(acc, da + 512, db + 512, 1u);
-      if (kb > 96) wgmma_k32(acc, da + 768, db + 768, 1u);
-      wg_commit();
+      // k32 steps, broadcast from lane 0 right before the batch so that ptxas can prove the dispatch warp-uniform
+      // (neither a value read from shared memory nor code behind the per-lane spin wait is, and a possibly divergent
+      // branch around a wgmma batch serialises it, C7520)
+      const uint32_t nk = __shfl_sync(0xffffffffu, kb >> 5, 0);
+      wgmma_stage(acc, nk, da, db, (flags & P4V_JOB_FIRST) ? 0u : 1u);
       wg_wait0();
       if (sub + 1 == nsub) warp_arrive(&S.empty[stage], lane);
       if (flags & P4V_JOB_LAST) on_last();
