@@ -49,6 +49,10 @@ typedef struct p4v_linear_desc {
   int32_t operand;   /* P4V_OPERAND_*  */
   int32_t kernel;    /* P4V_KERNEL_*   */
   int32_t init_layerwise; /* 1: every block starts from the layer-wise min-max step size (linear.py:382-383, :393-394) */
+  int32_t rows_per_chunk; /* 0: search the whole layer at once.  > 0: a multiple of 128, at most rows: the search builds
+                           * its row-dependent operand images (activations) for one chunk of rows at a time and adds the
+                           * chunks' scores; the workspace holds one chunk (the reference's calib_batch_size batching,
+                           * linear.py:365-378, :458-492). */
 } p4v_linear_desc;
 
 /* bytes of device workspace p4v_linear_* needs for this layer */
@@ -64,7 +68,12 @@ P4V_API int p4v_linear_score_log_floats(const p4v_linear_desc* d, size_t* n);
  *   (:497-533 / :609-642) }.
  * in : x [rows,in], weight [out,in], bias [out] or NULL, raw_out [rows,out], raw_grad [rows,out]
  * out: w_interval [n_V*n_H] (reference shape n_V,1,n_H,1), a_interval [n_a] (n_a,1),
- *      score_log (NULL or p4v_linear_score_log_floats floats).                         */
+ *      score_log (NULL or p4v_linear_score_log_floats floats).
+ * With d->rows_per_chunk > 0 every search step loops over the row chunks: it quantises the chunk's activations (current
+ * image, and the candidate planes in an activation step), sweeps them and adds the chunk's partial scores into the fp64
+ * score table; the pick follows the last chunk.  The initial step sizes and the gradient scale are taken over all rows
+ * first, so the result equals the unchunked search up to the order of the fp64 score sums.  The step-wise surface below
+ * (begin / search_w / search_a) takes whole layers only. */
 P4V_API int p4v_linear_calibrate(const p4v_linear_desc* d, const float* x, const float* weight, const float* bias,
                          const float* raw_out, const float* raw_grad, void* workspace, size_t workspace_bytes,
                          float* w_interval, float* a_interval, float* score_log, void* stream);
@@ -102,13 +111,20 @@ typedef struct p4v_matmul_desc {
   int32_t operand;
   int32_t kernel;
   int32_t init_layerwise; /* 1: every head starts from the layer-wise min-max step size (matmul.py:430-432) */
+  int32_t images_per_chunk; /* 0: search the whole layer at once.  > 0 (at most batch): operand images are built for
+                             * this many images at a time and the chunks' scores are added (matmul.py:396-409, :490-518) */
 } p4v_matmul_desc;
 
 P4V_API int p4v_matmul_workspace_bytes(const p4v_matmul_desc* d, size_t* bytes);
 P4V_API int p4v_matmul_score_log_floats(const p4v_matmul_desc* d, size_t* n);
 /* Replaces PTQSLBatchingQuantMatMul.calibration_step2() (matmul.py:565-576) and
  * SoSPTQSLBatchingQuantMatMul.calibration_step2() (matmul.py:633-644).
- * out: A_interval [heads] (sos: A_interval[0] = split/(qmax-1)), B_interval [heads], split [1] (sos) */
+ * out: A_interval [heads] (sos: A_interval[0] = split/(qmax-1)), B_interval [heads], split [1] (sos)
+ * With d->images_per_chunk > 0 every search step loops over the image chunks: it builds the chunk's A and B images
+ * (current and candidate planes; split-of-softmax: the split candidates and the exact split of B), sweeps them and adds
+ * the chunk's partial scores into the fp64 score table; the pick follows the last chunk.  Head-wise maxima and the
+ * gradient scale are taken over all images first, so the result equals the unchunked search up to the order of the fp64
+ * score sums. */
 P4V_API int p4v_matmul_calibrate(const p4v_matmul_desc* d, const float* A, const float* B, const float* raw_out,
                          const float* raw_grad, void* workspace, size_t workspace_bytes, float* A_interval,
                          float* B_interval, float* split, float* score_log, void* stream);

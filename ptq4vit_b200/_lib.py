@@ -18,14 +18,14 @@ class LinearDesc(C.Structure):
                 ("n_V", C.c_int32), ("n_H", C.c_int32), ("n_a", C.c_int32), ("w_bit", C.c_int32), ("a_bit", C.c_int32),
                 ("eq_n", C.c_int32), ("search_round", C.c_int32), ("eq_alpha", C.c_double), ("eq_beta", C.c_double),
                 ("post_gelu", C.c_int32), ("has_bias", C.c_int32), ("operand", C.c_int32), ("kernel", C.c_int32),
-                ("init_layerwise", C.c_int32)]
+                ("init_layerwise", C.c_int32), ("rows_per_chunk", C.c_int32)]
 
 
 class MatMulDesc(C.Structure):
     _fields_ = [("batch", C.c_int32), ("heads", C.c_int32), ("S1", C.c_int32), ("S2", C.c_int32), ("S3", C.c_int32),
                 ("A_bit", C.c_int32), ("B_bit", C.c_int32), ("eq_n", C.c_int32), ("search_round", C.c_int32),
                 ("eq_alpha", C.c_double), ("eq_beta", C.c_double), ("sos", C.c_int32), ("operand", C.c_int32),
-                ("kernel", C.c_int32), ("init_layerwise", C.c_int32)]
+                ("kernel", C.c_int32), ("init_layerwise", C.c_int32), ("images_per_chunk", C.c_int32)]
 
 
 class ConvDesc(C.Structure):

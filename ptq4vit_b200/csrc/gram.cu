@@ -216,18 +216,18 @@ __global__ void __launch_bounds__(256, 2) gram_update_kernel(const GramUpdateArg
 
 // U[o][k] = sum over token blocks (fixed order), E2[o] likewise.  thread = (o, k) ; k == ks handles E2.
 __global__ void gram_reduce_kernel(const float* __restrict__ Upart, const float* __restrict__ E2part, int n_mblk, int O, int ks,
-                                   float* __restrict__ U, float* __restrict__ E2) {
+                                   float* __restrict__ U, float* __restrict__ E2, int accumulate) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long nU = (long long)O * ks;
   if (i < nU) {
     float s = 0.f;
     for (int b = 0; b < n_mblk; ++b) s += Upart[(size_t)b * nU + i];
-    U[i] = s;
+    U[i] = accumulate ? U[i] + s : s;
   } else if (i < nU + O) {
     const int o = (int)(i - nU);
     float s = 0.f;
     for (int b = 0; b < n_mblk; ++b) s += E2part[(size_t)b * O + o];
-    E2[o] = s;
+    E2[o] = accumulate ? E2[o] + s : s;
   }
 }
 
@@ -342,9 +342,10 @@ int p4v_gram_update_splits(int O, int M) {      // token splits: one wave of two
   return s < 1 ? 1 : s;
 }
 
-int p4v_gram_reduce(const float* Upart, const float* E2part, int n_mblk, int O, int ks, float* U, float* E2, cudaStream_t st) {
+int p4v_gram_reduce(const float* Upart, const float* E2part, int n_mblk, int O, int ks, float* U, float* E2, int accumulate,
+                    cudaStream_t st) {
   const long long n = (long long)O * ks + O;
-  gram_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(Upart, E2part, n_mblk, O, ks, U, E2); p4v_count_launch();
+  gram_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(Upart, E2part, n_mblk, O, ks, U, E2, accumulate); p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -38,7 +38,9 @@ struct GramEvalArgs {
   double* sums2;                                       // [n_cand][n_groups]: the same summed per row block
 };
 int p4v_gram_eval(const GramEvalArgs& a, cudaStream_t st);
-int p4v_gram_reduce(const float* Upart, const float* E2part, int n_mblk, int O, int ks, float* U, float* E2, cudaStream_t st);
+// accumulate = 1: add to U and E2 (later row chunks of a chunked search) instead of overwriting them
+int p4v_gram_reduce(const float* Upart, const float* E2part, int n_mblk, int O, int ks, float* U, float* E2, int accumulate,
+                    cudaStream_t st);
 
 int p4v_xq_transpose(const float* x, int M, int K, int Mp, const float* dX, int crb_acts, float qlo, float qhi, int8_t* out, cudaStream_t st);
 // Z image of n_blocks column blocks starting at weight column k_first: row (b * npairs + pair) of 256-row tiles
@@ -52,5 +54,6 @@ struct GramGemmArgs {
   unsigned int term_bytes;                             // bytes of K (tokens * 2, padded to 32) of one term
   int tiles_o, tiles_p, O;
   float* H; long long ldH;                             // [O][ldH], ldH >= tiles_p * 256
+  int accumulate;                                      // 1: the running sum starts from the stored H (row chunks)
 };
 int p4v_gram_gemm(const GramGemmArgs& a, cudaStream_t st);

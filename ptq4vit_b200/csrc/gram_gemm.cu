@@ -8,7 +8,8 @@
 // The tensor core adds into the fp32 accumulator with truncation, so a long contraction of same-signed terms (the
 // diagonal of H: 6304 tokens x 3 products) drifts by ~1e-5 relative.  The contraction is therefore cut into splits of
 // `kSplitChunks` stages (256 tokens): each split starts a fresh accumulator and the consumer adds the splits in
-// registers with round-to-nearest fp32 adds.
+// registers with round-to-nearest fp32 adds.  With `accumulate` (row chunks of a chunked search) that running sum starts
+// from the stored H, so chunks whose boundaries fall on multiples of 256 tokens add in the order of one pass.
 // Roles: warp 0 = bulk-copy producer; warpgroups 1-2 = consumers, each issuing wgmma m64n128 for 64 of the 128 output
 // channels of the tile.
 #include "gram.cuh"
@@ -159,6 +160,21 @@ __global__ void __launch_bounds__(kThreads, 1) gram_gemm_kernel(const __grid_con
     float sum[64], acc[64];
 #pragma unroll
     for (int j = 0; j < 64; ++j) { sum[j] = 0.f; acc[j] = 0.f; }
+    float* hbase = a.H + (size_t)(q >> 1) * 256 + (q & 1) * 128 + 2 * (lane & 3);
+    if (a.accumulate) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int oo = o + 8 * h;
+        if (oo < a.O) {
+          const float* hrow = hbase + (size_t)oo * a.ldH;
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const float2 v = *reinterpret_cast<const float2*>(hrow + 8 * i);
+            sum[4 * i + 2 * h] = v.x; sum[4 * i + 2 * h + 1] = v.y;
+          }
+        }
+      }
+    }
     for (int ch = 0; ch < n_chunks; ++ch) {
       const bool first = ch % kSplitChunks == 0, last = (ch % kSplitChunks == kSplitChunks - 1) || ch == n_chunks - 1;
       const uint32_t k0 = ch * kStageKB, kb = (term - k0 < kStageKB) ? term - k0 : kStageKB;
@@ -190,7 +206,6 @@ __global__ void __launch_bounds__(kThreads, 1) gram_gemm_kernel(const __grid_con
         for (int j = 0; j < 64; ++j) sum[j] += acc[j];
       }
     }
-    float* hbase = a.H + (size_t)(q >> 1) * 256 + (q & 1) * 128 + 2 * (lane & 3);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int oo = o + 8 * h;

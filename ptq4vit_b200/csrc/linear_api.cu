@@ -109,6 +109,8 @@ int p4v_num_sms() {
 namespace {
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+// bytes of K of one bf16 term of the Gram operands for n tokens
+inline unsigned gram_term(int n) { return (unsigned)align_up((size_t)n * 2, 32); }
 
 struct BSeg { int k0, klen, h, a, kb; int woff, xoff_p, xoff_n, xcoff; };   // offsets: bytes in the padded row
 struct Step { int job_off, nfj, ncj, nfg, ncg, meta_fix, meta_cand, commit_off, ncommit, commit_chunks; };
@@ -117,6 +119,7 @@ struct LinPlan {
   p4v_linear_desc d;
   bool i8, twin;
   int ew, M, K, O, tiles_m, tiles_o, nsg, crb_rows, crb_cols, crb_acts, w_qmax, a_qmax;
+  bool chunked; int chunk_rows, tiles_mc;   // rows of one chunk (M unchunked) and their 128-row tiles: the X images hold one chunk
   float d_neg;
   std::vector<BSeg> segs;
   int KB_W, KB_X, KB_Xc;
@@ -198,12 +201,17 @@ int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search) {
   P4V_REQUIRE(d->tokens >= 1 && p.M % d->tokens == 0, "linear: rows must be a multiple of tokens");
   P4V_REQUIRE(d->w_bit >= 2 && d->w_bit <= 8 && d->a_bit >= 2 && d->a_bit <= 8, "linear: bit widths must be in [2,8]");
   P4V_REQUIRE(d->eq_n >= 1 && d->eq_n <= P4V_MAX_CAND, "linear: eq_n must be in [1,%d]", P4V_MAX_CAND);
+  P4V_REQUIRE(d->rows_per_chunk >= 0 && d->rows_per_chunk % P4V_TILE == 0 && d->rows_per_chunk <= p.M,
+              "linear: rows_per_chunk must be a multiple of %d in [0, rows=%d] (got %d; 0 = whole layer)", P4V_TILE, p.M,
+              d->rows_per_chunk);
   p.crb_rows = p.O / d->n_V; p.crb_cols = p.K / d->n_H; p.crb_acts = p.K / d->n_a;
   P4V_REQUIRE(d->n_V == 1 || p.crb_rows % P4V_CG == 0, "linear: out_features/n_V must be a multiple of 16 (got %d)", p.crb_rows);
   p.w_qmax = 1 << (d->w_bit - 1); p.a_qmax = 1 << (d->a_bit - 1);
   p.twin = d->post_gelu != 0;
   p.d_neg = (float)(0.16997124254703522 / (double)p.a_qmax);
   p.tiles_m = p4v_cdiv(p.M, P4V_TILE); p.tiles_o = p4v_cdiv(p.O, P4V_TILE);
+  p.chunked = with_search && d->rows_per_chunk > 0;
+  p.chunk_rows = p.chunked ? d->rows_per_chunk : p.M; p.tiles_mc = p4v_cdiv(p.chunk_rows, P4V_TILE);
   p.nsg = p.tiles_o * P4V_TILE_CG;
 
   // K segments = intersections of the weight column blocks and the activation chunks
@@ -339,24 +347,26 @@ int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search) {
   p.o_segsX = take(p.segsX.size() * sizeof(P4VSeg));
   p.o_segsXc = take(p.segsXc.size() * sizeof(P4VSeg));
   p.o_commits = take(std::max<size_t>(1, p.commits.size()) * sizeof(CommitSeg));
-  p.o_partial = take(with_search ? (size_t)p.tiles_m * p.tiles_o * n_c * 32 * 4 : 4);
+  p.o_partial = take(with_search ? (size_t)p.tiles_mc * p.tiles_o * n_c * 32 * 4 : 4);
   p.o_Wcur = take((size_t)p.tiles_o * P4V_TILE * p.KB_W);
-  p.o_Xcur = take((size_t)p.tiles_m * P4V_TILE * p.KB_X);
+  p.o_Xcur = take((size_t)p.tiles_mc * P4V_TILE * p.KB_X);
   p.o_Wcand = take(with_search ? (size_t)n_c * p.tiles_o * P4V_TILE * p.KB_W : 4);
-  p.o_Xcand = take(with_search ? (size_t)n_c * p.tiles_m * P4V_TILE * p.KB_Xc : 4);
-  // normal-equation W search: narrow column blocks inside one activation chunk, plain (non twin) activations
+  p.o_Xcand = take(with_search ? (size_t)n_c * p.tiles_mc * P4V_TILE * p.KB_Xc : 4);
+  // normal-equation W search: narrow column blocks inside one activation chunk, plain (non twin) activations.
+  // Chunked: the residual e and the token-major activations stay whole-layer, the (gs*g)^2 and pair images hold one chunk
+  // of rows; H, U and sum (g e)^2 accumulate over the chunks.
   p.gram = false;
   {
     const char* env = getenv("P4V_GRAM");
     const bool want = with_search && (env ? atoi(env) != 0 : true) && d->kernel == P4V_KERNEL_TCGEN05;
-    const unsigned term = (unsigned)align_up((size_t)p.M * 2, 32);
+    const unsigned term = gram_term(p.chunk_rows);
     if (want && !p.twin && p.crb_cols <= 64 && p.crb_cols % 4 == 0 && p.crb_acts % p.crb_cols == 0) {
       p.gram = true;
       p.g_ks = p.crb_cols; p.g_term_bytes = term;
       p.g_Mp = (int)align_up((size_t)p.M, 16) + 16;
       p.g_npairs = p.g_ks * (p.g_ks + 1) / 2;
       p.g_tiles_p = p4v_cdiv(p.g_npairs * d->n_H, GRAM_PT); p.g_ldH = p.g_tiles_p * GRAM_PT;   // all column blocks side by side
-      p.g_nmblk = p4v_gram_update_splits(p.O, p.M);
+      p.g_nmblk = p4v_gram_update_splits(p.O, p.chunk_rows);
       const size_t KBg = 2 * (size_t)term;
       p.o_E = take((size_t)p.M * p.O * 4);
       p.o_XqT = take((size_t)p.K * p.g_Mp);
@@ -369,7 +379,7 @@ int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search) {
       p.g_osplit = std::max(1, p4v_cdiv(p.crb_rows, 2)); p.g_opb = p4v_cdiv(p.crb_rows, p.g_osplit);
       p.o_dprev = take((size_t)d->n_V * 4);
       p.o_D = take((size_t)p.O * 64 * 4);
-      p.o_segsG = take(2 * sizeof(P4VSeg));
+      p.o_segsG = take((p.chunked ? 4 : 2) * sizeof(P4VSeg));   // chunked: a full chunk and the last one
     }
   }
   p.total = o;
@@ -388,8 +398,14 @@ int upload_tables(const LinPlan& p, void* ws, cudaStream_t st) {
   if (!p.commits.empty())
     P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_commits), p.commits.data(), p.commits.size() * sizeof(CommitSeg), cudaMemcpyHostToDevice, st));
   if (p.gram) {
-    P4VSeg sg[2] = {{0, p.M, 0, 0, 0.f, 0.f, 0.f, 0, 0.f, 1, 1}, {0, p.M, (int)(p.g_term_bytes * P4V_TILE), 0, 0.f, 0.f, 0.f, 0, 0.f, 2, 1}};
-    P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segsG), sg, sizeof(sg), cudaMemcpyHostToDevice, st));
+    const int n_last = p.M - (p4v_cdiv(p.M, p.chunk_rows) - 1) * p.chunk_rows;
+    const int nr[2] = {p.chunk_rows, n_last};
+    P4VSeg sg[4];
+    for (int i = 0; i < 2; ++i) {
+      sg[2 * i] = P4VSeg{0, nr[i], 0, 0, 0.f, 0.f, 0.f, 0, 0.f, 1, 1};
+      sg[2 * i + 1] = P4VSeg{0, nr[i], (int)(gram_term(nr[i]) * P4V_TILE), 0, 0.f, 0.f, 0.f, 0, 0.f, 2, 1};
+    }
+    P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segsG), sg, (p.chunked ? 4 : 2) * sizeof(P4VSeg), cudaMemcpyHostToDevice, st));
   }
   return 0;
 }
@@ -407,28 +423,33 @@ int quant_W(const LinPlan& p, void* ws, const float* W, const float* delta, bool
   return p4v_quant_image(q, st);
 }
 
-int quant_X(const LinPlan& p, void* ws, const float* x, const float* delta, bool cand, cudaStream_t st) {
+// rows [r0, r0 + n) of the layer: one chunk (or all rows)
+struct Rows { int r0, n; };
+Rows all_rows(const LinPlan& p) { return Rows{0, p.M}; }
+
+int quant_X(const LinPlan& p, void* ws, const float* x, const float* delta, bool cand, Rows r, cudaStream_t st) {
   QuantImageArgs q{};
-  q.src = x; q.ld = p.K; q.prob_stride = 0; q.src_transposed = 0;
-  q.P = 1; q.rows = p.M; q.tiles = p.tiles_m;
+  q.src = x + (size_t)r.r0 * p.K; q.ld = p.K; q.prob_stride = 0; q.src_transposed = 0;
+  q.P = 1; q.rows = r.n; q.tiles = p4v_cdiv(r.n, P4V_TILE);
   q.dst = at<uint8_t>(ws, cand ? p.o_Xcand : p.o_Xcur);
-  q.tile_bytes = (unsigned long long)P4V_TILE * (cand ? p.KB_Xc : p.KB_X); q.plane_stride = q.tile_bytes * p.tiles_m;
+  q.tile_bytes = (unsigned long long)P4V_TILE * (cand ? p.KB_Xc : p.KB_X); q.plane_stride = q.tile_bytes * q.tiles;
   q.n_planes = cand ? p.d.eq_n : 1;
   q.factors = cand ? at<float>(ws, p.o_factors) : nullptr;
-  q.delta = delta; q.rows_per_block = p.M + P4V_TILE; q.d_stride = 0; q.d_mod = 1;   // single row block
+  q.delta = delta; q.rows_per_block = p.M + P4V_TILE; q.d_stride = 0; q.d_mod = 1;   // single row block: any row range
   q.segs = at<P4VSeg>(ws, cand ? p.o_segsXc : p.o_segsX); q.nseg = (int)(cand ? p.segsXc.size() : p.segsX.size());
   q.is_int8 = p.i8;
   return p4v_quant_image(q, st);
 }
 
-void fill_sweep(const LinPlan& p, void* ws, const Step& s, SweepParams& sp) {
+void fill_sweep(const LinPlan& p, void* ws, const Step& s, SweepParams& sp, Rows r) {
+  const int tiles_m = p4v_cdiv(r.n, P4V_TILE);
   sp = SweepParams{};
   sp.R_cur = at<uint8_t>(ws, p.o_Xcur); sp.R_cand = at<uint8_t>(ws, p.o_Xcand);
   sp.C_cur = at<uint8_t>(ws, p.o_Wcur); sp.C_cand = at<uint8_t>(ws, p.o_Wcand);
   sp.R_tile_bytes = (unsigned long long)P4V_TILE * p.KB_X; sp.C_tile_bytes = (unsigned long long)P4V_TILE * p.KB_W;
   sp.R_cand_tile_bytes = (unsigned long long)P4V_TILE * p.KB_Xc; sp.C_cand_tile_bytes = sp.C_tile_bytes;
-  sp.R_cand_stride = sp.R_cand_tile_bytes * p.tiles_m; sp.C_cand_stride = sp.C_cand_tile_bytes * p.tiles_o;
-  sp.P = 1; sp.M = p.M; sp.N = p.O; sp.tiles_m = p.tiles_m; sp.tiles_n = p.tiles_o;
+  sp.R_cand_stride = sp.R_cand_tile_bytes * tiles_m; sp.C_cand_stride = sp.C_cand_tile_bytes * p.tiles_o;
+  sp.P = 1; sp.M = r.n; sp.N = p.O; sp.tiles_m = tiles_m; sp.tiles_n = p.tiles_o;
   sp.ld = p.O; sp.prob_stride = 0;
   sp.gscale = at<float>(ws, p.o_gscale);
   sp.jobs = at<P4VJob>(ws, p.o_jobs) + s.job_off;
@@ -439,6 +460,7 @@ void fill_sweep(const LinPlan& p, void* ws, const Step& s, SweepParams& sp) {
   sp.partial = at<float>(ws, p.o_partial);
   sp.is_int8 = p.i8;
 }
+void fill_sweep(const LinPlan& p, void* ws, const Step& s, SweepParams& sp) { fill_sweep(p, ws, s, sp, all_rows(p)); }
 
 int run_sweep(const LinPlan& p, const Step& s, const SweepParams& sp, cudaStream_t st) {
   return p4v_run_sweep(sp, p.jobs.data() + s.job_off, p.d.kernel, st);
@@ -464,23 +486,33 @@ int tables_for(const LinPlan& p, void* ws, const Step& s, int kind, int target, 
 struct StepRef { bool is_w; int idx; };
 
 // One search step: [scale tables] -> sweep -> reduce -> select (+ tables of the next step) -> commit.
-int search_step(const LinPlan& p, void* ws, StepRef cur, const StepRef* next, bool tables_ready, const float* bias,
-                const float* y, const float* g, float* score_log, cudaStream_t st) {
+// Chunked: per chunk of rows, the chunk's X images (current; X step: candidates) -> sweep -> reduce into the fp64 table;
+// select after the last chunk; only the weight image is committed (the X images are rebuilt from the step sizes).
+int search_step(const LinPlan& p, void* ws, StepRef cur, const StepRef* next, bool tables_ready, const float* x,
+                const float* bias, const float* y, const float* g, float* score_log, cudaStream_t st) {
   const bool is_w = cur.is_w; const int idx = cur.idx;
   const Step& s = is_w ? p.wsteps[idx] : p.xsteps[idx];
   int rc;
   if (!tables_ready && (rc = tables_for(p, ws, s, is_w ? 0 : 1, idx, st))) return rc;
-  SweepParams sp; fill_sweep(p, ws, s, sp);
-  sp.Y = y; sp.Gr = g; sp.bias = p.d.has_bias ? bias : nullptr;
-  sp.order = is_w ? 0 : 1;
-  if ((rc = run_sweep(p, s, sp, st))) return rc;
+  SweepParams sp;
+  for (int r0 = 0; r0 < p.M; r0 += p.chunk_rows) {
+    const Rows r{r0, std::min(p.chunk_rows, p.M - r0)};
+    if (p.chunked) {
+      if ((rc = quant_X(p, ws, x, at<float>(ws, p.o_dX), false, r, st))) return rc;
+      if (!is_w && (rc = quant_X(p, ws, x, at<float>(ws, p.o_dX0), true, r, st))) return rc;
+    }
+    fill_sweep(p, ws, s, sp, r);
+    sp.Y = y + (size_t)r0 * p.O; sp.Gr = g + (size_t)r0 * p.O; sp.bias = p.d.has_bias ? bias : nullptr;
+    sp.order = is_w ? 0 : 1;
+    if ((rc = run_sweep(p, s, sp, st))) return rc;
+    ReduceArgs ra{};
+    ra.partial = sp.partial; ra.n_cand = p.d.eq_n; ra.P = 1; ra.tiles_m = sp.tiles_m; ra.tiles_n = p.tiles_o; ra.order = sp.order;
+    ra.mode = P4V_SG_COLUMN; ra.n_keys = p.nsg; ra.sums = at<double>(ws, p.o_scores); ra.accumulate = r0 > 0;
+    if ((rc = p4v_reduce_scores(ra, st))) return rc;
+  }
   const int n_groups = is_w ? p.d.n_V : 1;
-  ReduceArgs r{};
-  r.partial = sp.partial; r.n_cand = p.d.eq_n; r.P = 1; r.tiles_m = p.tiles_m; r.tiles_n = p.tiles_o; r.order = sp.order;
-  r.mode = P4V_SG_COLUMN; r.n_keys = p.nsg; r.sums = at<double>(ws, p.o_scores);
-  if ((rc = p4v_reduce_scores(r, st))) return rc;
   SelectArgs f{};
-  f.sums = r.sums; f.n_cand = p.d.eq_n; f.n_keys = p.nsg; f.n_groups = n_groups;
+  f.sums = at<double>(ws, p.o_scores); f.n_cand = p.d.eq_n; f.n_keys = p.nsg; f.n_groups = n_groups;
   f.keys_per_group = (is_w && p.d.n_V > 1) ? p.crb_rows / P4V_CG : p.nsg;
   f.inv_count = 1.0 / ((double)p.d.tokens * (double)(is_w ? p.crb_rows : p.O));
   f.gscale = at<float>(ws, p.o_gscale); f.factors = at<float>(ws, p.o_factors);
@@ -490,6 +522,7 @@ int search_step(const LinPlan& p, void* ws, StepRef cur, const StepRef* next, bo
   f.has_next = next != nullptr;
   if (next) f.next = tables_args(p, ws, next->is_w ? p.wsteps[next->idx] : p.xsteps[next->idx], next->is_w ? 0 : 1, next->idx);
   if ((rc = p4v_select_step(f, st))) return rc;
+  if (p.chunked && !is_w) return 0;
   CommitArgs c{};
   c.best = f.best; c.n_groups = n_groups;
   c.cand = at<uint8_t>(ws, is_w ? p.o_Wcand : p.o_Xcand);
@@ -503,49 +536,75 @@ int search_step(const LinPlan& p, void* ws, StepRef cur, const StepRef* next, bo
   return p4v_commit_step(c, st);
 }
 
+// (gs*g)^2 image of the rows r: rows = output channels, K = the chunk's tokens, two exact bf16 terms (transposed read)
+int gram_g2_image(const LinPlan& p, void* ws, const float* g, Rows r, cudaStream_t st) {
+  const unsigned term = gram_term(r.n);
+  QuantImageArgs q{};
+  q.src = g + (size_t)r.r0 * p.O; q.ld = p.O; q.prob_stride = 0; q.src_transposed = 1;
+  q.P = 1; q.rows = p.O; q.tiles = p.tiles_o;
+  q.dst = at<uint8_t>(ws, p.o_G2T); q.tile_bytes = (unsigned long long)P4V_TILE * 2 * term; q.plane_stride = 0;
+  q.n_planes = 1; q.factors = nullptr; q.delta = at<float>(ws, p.o_dW0); q.rows_per_block = p.O + P4V_TILE; q.d_stride = 0; q.d_mod = 1;
+  q.segs = at<P4VSeg>(ws, p.o_segsG) + (r.n == p.chunk_rows ? 0 : 2); q.nseg = 2; q.is_int8 = 0; q.presc = at<float>(ws, p.o_gscale);
+  return p4v_quant_image(q, st);
+}
+
 // Whole W search of one round in normal-equation form (gram.cu): residual once, then per column block
 // (pair image + Gram GEMM for every column block, once) and per column block update pass -> candidate evaluation -> select -> commit.
+// Chunked: the residual sweep, the (gs*g)^2 and pair images, the Gram GEMM (seeded from the stored H) and the update pass
+// (U, sum (g e)^2 added over the chunks) run per chunk of rows; evaluation, select and commit once per column block.
 int gram_wsearch(const LinPlan& p, void* ws, const float* x, const float* W, const float* bias, const float* y, const float* g,
                  int h_begin, int h_end, float* score_log, cudaStream_t st) {
   int rc;
   const float w_lo = (float)-p.w_qmax, w_hi = (float)(p.w_qmax - 1);
+  std::vector<Rows> chunks;
+  for (int r0 = 0; r0 < p.M; r0 += p.chunk_rows) chunks.push_back(Rows{r0, std::min(p.chunk_rows, p.M - r0)});
   // e = y - yhat(current step sizes), exact integer products (every segment as a fixed group)
   if ((rc = tables_for(p, ws, p.fwd, -1, 0, st))) return rc;
-  {
-    SweepParams sp; fill_sweep(p, ws, p.fwd, sp);
-    sp.Y = y; sp.Gr = g; sp.bias = p.d.has_bias ? bias : nullptr;
-    sp.out = at<float>(ws, p.o_E); sp.out_residual = 1; sp.n_cand = 1; sp.order = 0; sp.R_cand = nullptr; sp.C_cand = nullptr;
+  for (const Rows& r : chunks) {
+    if (p.chunked && (rc = quant_X(p, ws, x, at<float>(ws, p.o_dX), false, r, st))) return rc;
+    SweepParams sp; fill_sweep(p, ws, p.fwd, sp, r);
+    sp.Y = y + (size_t)r.r0 * p.O; sp.Gr = g + (size_t)r.r0 * p.O; sp.bias = p.d.has_bias ? bias : nullptr;
+    sp.out = at<float>(ws, p.o_E) + (size_t)r.r0 * p.O; sp.out_residual = 1; sp.n_cand = 1; sp.order = 0;
+    sp.R_cand = nullptr; sp.C_cand = nullptr;
     if ((rc = run_sweep(p, p.fwd, sp, st))) return rc;
   }
   if ((rc = p4v_xq_transpose(x, p.M, p.K, p.g_Mp, at<float>(ws, p.o_dX), p.crb_acts, (float)-p.a_qmax, (float)(p.a_qmax - 1),
                              at<int8_t>(ws, p.o_XqT), st))) return rc;
-  // H for every column block of the range: one pair image + one tensor-core GEMM (the activations do not change
-  // during the weight steps of a round)
+  // H for every column block of the range: one pair image + one tensor-core GEMM per chunk of rows (the activations do
+  // not change during the weight steps of a round)
   {
     const int nblk = h_end - h_begin;
-    const unsigned long long z_tile = (unsigned long long)GRAM_PT * 2 * p.g_term_bytes;
     const int tiles_p = p4v_cdiv(p.g_npairs * nblk, GRAM_PT);
-    if ((rc = p4v_pair_image(at<int8_t>(ws, p.o_XqT), p.g_Mp, p.M, h_begin * p.g_ks, p.g_ks, p.g_npairs, nblk, tiles_p, z_tile,
-                             p.g_term_bytes, at<uint8_t>(ws, p.o_Z), st))) return rc;
-    GramGemmArgs gg{};
-    gg.R = at<uint8_t>(ws, p.o_G2T); gg.R_tile_bytes = (unsigned long long)P4V_TILE * 2 * p.g_term_bytes;
-    gg.C = at<uint8_t>(ws, p.o_Z); gg.C_tile_bytes = z_tile; gg.term_bytes = p.g_term_bytes;
-    gg.tiles_o = p.tiles_o; gg.tiles_p = tiles_p; gg.O = p.O; gg.H = at<float>(ws, p.o_H); gg.ldH = p.g_ldH;
-    if ((rc = p4v_gram_gemm(gg, st))) return rc;
+    for (const Rows& r : chunks) {
+      const unsigned term = gram_term(r.n);
+      const unsigned long long z_tile = (unsigned long long)GRAM_PT * 2 * term;
+      if (p.chunked && (rc = gram_g2_image(p, ws, g, r, st))) return rc;
+      if ((rc = p4v_pair_image(at<int8_t>(ws, p.o_XqT) + r.r0, p.g_Mp, r.n, h_begin * p.g_ks, p.g_ks, p.g_npairs, nblk, tiles_p,
+                               z_tile, term, at<uint8_t>(ws, p.o_Z), st))) return rc;
+      GramGemmArgs gg{};
+      gg.R = at<uint8_t>(ws, p.o_G2T); gg.R_tile_bytes = (unsigned long long)P4V_TILE * 2 * term;
+      gg.C = at<uint8_t>(ws, p.o_Z); gg.C_tile_bytes = z_tile; gg.term_bytes = term;
+      gg.tiles_o = p.tiles_o; gg.tiles_p = tiles_p; gg.O = p.O; gg.H = at<float>(ws, p.o_H); gg.ldH = p.g_ldH;
+      gg.accumulate = r.r0 > 0;
+      if ((rc = p4v_gram_gemm(gg, st))) return rc;
+    }
   }
   for (int h = h_begin; h < h_end; ++h) {
-    GramUpdateArgs u{};
-    u.E = at<float>(ws, p.o_E); u.G = g; u.gscale = at<float>(ws, p.o_gscale);
-    u.W = W; u.M = p.M; u.O = p.O; u.K = p.K; u.XqT = at<int8_t>(ws, p.o_XqT); u.Mp = p.g_Mp;
-    u.dX = at<float>(ws, p.o_dX); u.crb_acts = p.crb_acts;
-    u.dW = at<float>(ws, p.o_dW); u.dW_prev = at<float>(ws, p.o_dprev); u.n_V = p.d.n_V; u.n_H = p.d.n_H; u.crb_rows = p.crb_rows;
-    u.h_prev = h > h_begin ? h - 1 : -1; u.k_prev = (h - 1) * p.g_ks; u.k_next = h * p.g_ks; u.ks = p.g_ks;
-    u.w_lo = w_lo; u.w_hi = w_hi; u.Upart = at<float>(ws, p.o_Upart); u.E2part = at<float>(ws, p.o_E2part);
-    u.D = at<float>(ws, p.o_D); u.n_split = p.g_nmblk;
-    if ((rc = p4v_gram_update(u, st))) return rc;
+    for (const Rows& r : chunks) {
+      GramUpdateArgs u{};
+      u.E = at<float>(ws, p.o_E) + (size_t)r.r0 * p.O; u.G = g + (size_t)r.r0 * p.O; u.gscale = at<float>(ws, p.o_gscale);
+      u.W = W; u.M = r.n; u.O = p.O; u.K = p.K; u.XqT = at<int8_t>(ws, p.o_XqT) + r.r0; u.Mp = p.g_Mp;
+      u.dX = at<float>(ws, p.o_dX); u.crb_acts = p.crb_acts;
+      u.dW = at<float>(ws, p.o_dW); u.dW_prev = at<float>(ws, p.o_dprev); u.n_V = p.d.n_V; u.n_H = p.d.n_H; u.crb_rows = p.crb_rows;
+      u.h_prev = h > h_begin ? h - 1 : -1; u.k_prev = (h - 1) * p.g_ks; u.k_next = h * p.g_ks; u.ks = p.g_ks;
+      u.w_lo = w_lo; u.w_hi = w_hi; u.Upart = at<float>(ws, p.o_Upart); u.E2part = at<float>(ws, p.o_E2part);
+      u.D = at<float>(ws, p.o_D); u.n_split = p.g_nmblk;
+      if ((rc = p4v_gram_update(u, st))) return rc;
+      if ((rc = p4v_gram_reduce(u.Upart, u.E2part, p.g_nmblk, p.O, p.g_ks, at<float>(ws, p.o_U), at<float>(ws, p.o_E2),
+                                r.r0 > 0, st))) return rc;
+    }
     GramEvalArgs ev{};
     ev.H = at<float>(ws, p.o_H) + (size_t)(h - h_begin) * p.g_npairs; ev.ldH = p.g_ldH; ev.npairs = p.g_npairs;
-    if ((rc = p4v_gram_reduce(u.Upart, u.E2part, p.g_nmblk, p.O, p.g_ks, at<float>(ws, p.o_U), at<float>(ws, p.o_E2), st))) return rc;
     ev.U = at<float>(ws, p.o_U); ev.E2 = at<float>(ws, p.o_E2);
     ev.W = W; ev.O = p.O; ev.K = p.K; ev.k_first = h * p.g_ks; ev.ks = p.g_ks;
     ev.dW = at<float>(ws, p.o_dW); ev.dW0 = at<float>(ws, p.o_dW0); ev.n_H = p.d.n_H; ev.h = h;
@@ -593,19 +652,13 @@ int begin_impl(const LinPlan& p, const float* x, const float* W, const float* g,
   if ((rc = p4v_keys_to_delta(keys, nW, (float)p.w_qmax - 0.5f, at<float>(ws, p.o_dW0), at<float>(ws, p.o_dW), st))) return rc;
   if ((rc = p4v_keys_to_delta(keys + nW, p.d.n_a, (float)p.a_qmax - 0.5f, at<float>(ws, p.o_dX0), at<float>(ws, p.o_dX), st))) return rc;
   if ((rc = p4v_make_gscale(keys + nW + p.d.n_a, at<float>(ws, p.o_gscale), st))) return rc;
-  if (p.gram) {          // (gs*g)^2 as two exact bf16 terms, transposed: rows = output channels, K = tokens
-    QuantImageArgs q{};
-    q.src = g; q.ld = p.O; q.prob_stride = 0; q.src_transposed = 1;
-    q.P = 1; q.rows = p.O; q.tiles = p.tiles_o;
-    q.dst = at<uint8_t>(ws, p.o_G2T); q.tile_bytes = (unsigned long long)P4V_TILE * 2 * p.g_term_bytes; q.plane_stride = 0;
-    q.n_planes = 1; q.factors = nullptr; q.delta = at<float>(ws, p.o_dW0); q.rows_per_block = p.O + P4V_TILE; q.d_stride = 0; q.d_mod = 1;
-    q.segs = at<P4VSeg>(ws, p.o_segsG); q.nseg = 2; q.is_int8 = 0; q.presc = at<float>(ws, p.o_gscale);
-    if ((rc = p4v_quant_image(q, st))) return rc;
-  }
+  // (gs*g)^2 of all rows, built once; a chunked search builds it per chunk
+  if (p.gram && !p.chunked && (rc = gram_g2_image(p, ws, g, all_rows(p), st))) return rc;
   if ((rc = quant_W(p, ws, W, at<float>(ws, p.o_dW0), false, st))) return rc;
   if ((rc = quant_W(p, ws, W, at<float>(ws, p.o_dW0), true, st))) return rc;
-  if ((rc = quant_X(p, ws, x, at<float>(ws, p.o_dX0), false, st))) return rc;
-  if ((rc = quant_X(p, ws, x, at<float>(ws, p.o_dX0), true, st))) return rc;
+  if (p.chunked) return 0;         // every step builds its chunks' activation images
+  if ((rc = quant_X(p, ws, x, at<float>(ws, p.o_dX0), false, all_rows(p), st))) return rc;
+  if ((rc = quant_X(p, ws, x, at<float>(ws, p.o_dX0), true, all_rows(p), st))) return rc;
   return 0;
 }
 
@@ -631,6 +684,7 @@ extern "C" int p4v_linear_begin(const p4v_linear_desc* d, const float* x, const 
   LinPlan p; int rc = build_plan(d, p, true);
   if (rc) return rc;
   P4V_REQUIRE(x && weight && raw_grad && workspace, "linear_begin: null pointer");
+  P4V_REQUIRE(!p.chunked, "linear_begin: the step-wise surface searches whole layers (rows_per_chunk must be 0)");
   P4V_REQUIRE(workspace_bytes >= p.total, "linear_begin: workspace too small (%zu < %zu)", workspace_bytes, p.total);
   return begin_impl(p, x, weight, raw_grad, workspace, (cudaStream_t)stream);
 }
@@ -640,10 +694,11 @@ extern "C" int p4v_linear_search_w(const p4v_linear_desc* d, const float* bias, 
   LinPlan p; int rc = build_plan(d, p, true);
   if (rc) return rc;
   P4V_REQUIRE(raw_out && raw_grad && workspace, "linear_search_w: null pointer");
+  P4V_REQUIRE(!p.chunked, "linear_search_w: the step-wise surface searches whole layers (rows_per_chunk must be 0)");
   P4V_REQUIRE(0 <= h_begin && h_begin <= h_end && h_end <= d->n_H, "linear_search_w: bad block range");
   for (int h = h_begin; h < h_end; ++h) {
     StepRef nx{true, h + 1};
-    if ((rc = search_step(p, workspace, StepRef{true, h}, h + 1 < h_end ? &nx : nullptr, h > h_begin, bias, raw_out, raw_grad,
+    if ((rc = search_step(p, workspace, StepRef{true, h}, h + 1 < h_end ? &nx : nullptr, h > h_begin, nullptr, bias, raw_out, raw_grad,
                           score_log, (cudaStream_t)stream))) return rc;
     if (score_log) score_log += (size_t)d->eq_n * d->n_V;
   }
@@ -655,10 +710,11 @@ extern "C" int p4v_linear_search_a(const p4v_linear_desc* d, const float* bias, 
   LinPlan p; int rc = build_plan(d, p, true);
   if (rc) return rc;
   P4V_REQUIRE(raw_out && raw_grad && workspace, "linear_search_a: null pointer");
+  P4V_REQUIRE(!p.chunked, "linear_search_a: the step-wise surface searches whole layers (rows_per_chunk must be 0)");
   P4V_REQUIRE(0 <= a_begin && a_begin <= a_end && a_end <= d->n_a, "linear_search_a: bad chunk range");
   for (int a = a_begin; a < a_end; ++a) {
     StepRef nx{false, a + 1};
-    if ((rc = search_step(p, workspace, StepRef{false, a}, a + 1 < a_end ? &nx : nullptr, a > a_begin, bias, raw_out, raw_grad,
+    if ((rc = search_step(p, workspace, StepRef{false, a}, a + 1 < a_end ? &nx : nullptr, a > a_begin, nullptr, bias, raw_out, raw_grad,
                           score_log, (cudaStream_t)stream))) return rc;
     if (score_log) score_log += d->eq_n;
   }
@@ -690,7 +746,7 @@ extern "C" int p4v_linear_calibrate(const p4v_linear_desc* d, const float* x, co
       if (score_log) score_log += (size_t)d->n_H * d->eq_n * d->n_V;
       for (int a = 0; a < d->n_a; ++a) {
         StepRef nx{false, a + 1};
-        if ((rc = search_step(p, workspace, StepRef{false, a}, a + 1 < d->n_a ? &nx : nullptr, a > 0, bias, raw_out, raw_grad,
+        if ((rc = search_step(p, workspace, StepRef{false, a}, a + 1 < d->n_a ? &nx : nullptr, a > 0, x, bias, raw_out, raw_grad,
                               score_log, st))) return rc;
         if (score_log) score_log += d->eq_n;
       }
@@ -702,7 +758,7 @@ extern "C" int p4v_linear_calibrate(const p4v_linear_desc* d, const float* x, co
       for (int a = 0; a < d->n_a; ++a) seq.push_back(StepRef{false, a});
     }
     for (size_t i = 0; i < seq.size(); ++i) {
-      if ((rc = search_step(p, workspace, seq[i], i + 1 < seq.size() ? &seq[i + 1] : nullptr, i > 0, bias, raw_out, raw_grad,
+      if ((rc = search_step(p, workspace, seq[i], i + 1 < seq.size() ? &seq[i + 1] : nullptr, i > 0, x, bias, raw_out, raw_grad,
                             score_log, st))) return rc;
       if (score_log) score_log += seq[i].is_w ? (size_t)d->eq_n * d->n_V : (size_t)d->eq_n;
     }
@@ -732,7 +788,7 @@ extern "C" int p4v_linear_quant_forward(const p4v_linear_desc* d, const float* x
   P4V_CUDA_OK(cudaMemcpyAsync(at<float>(workspace, p.o_dW), w_interval, (size_t)d->n_V * d->n_H * 4, cudaMemcpyDeviceToDevice, st));
   P4V_CUDA_OK(cudaMemcpyAsync(at<float>(workspace, p.o_dX), a_interval, (size_t)d->n_a * 4, cudaMemcpyDeviceToDevice, st));
   if ((rc = quant_W(p, workspace, weight, at<float>(workspace, p.o_dW), false, st))) return rc;
-  if ((rc = quant_X(p, workspace, x, at<float>(workspace, p.o_dX), false, st))) return rc;
+  if ((rc = quant_X(p, workspace, x, at<float>(workspace, p.o_dX), false, all_rows(p), st))) return rc;
   if ((rc = tables_for(p, workspace, p.fwd, -1, 0, st))) return rc;
   SweepParams sp; fill_sweep(p, workspace, p.fwd, sp);
   sp.bias = d->has_bias ? bias : nullptr;

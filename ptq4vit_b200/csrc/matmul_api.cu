@@ -21,6 +21,8 @@ struct MMPlan {
   p4v_matmul_desc d;
   bool i8, sos;
   int ew, P, H, S1, S2, S3, tiles_m, tiles_n, A_qmax, B_qmax;
+  int ipc;       // images per chunk (0: whole layer); the operand images hold Pc = ipc * heads problems
+  int Pc;
   int kb;        // padded K bytes of one part in the search operand type
   int kb16;      // padded K bytes in bf16 (split-search images)
   int KB_A, KB_B;            // row bytes of Acur / Bcur  (sos: Acur = [hi|lo])
@@ -52,8 +54,12 @@ int build_plan(const p4v_matmul_desc* d, MMPlan& p, bool with_search) {
   P4V_REQUIRE(d->batch > 0 && d->heads > 0 && d->S1 > 0 && d->S2 > 0 && d->S3 > 0, "matmul: empty shape");
   P4V_REQUIRE(d->A_bit >= 2 && d->A_bit <= 8 && d->B_bit >= 2 && d->B_bit <= 8, "matmul: bit widths must be in [2,8]");
   P4V_REQUIRE(d->eq_n >= 1 && d->eq_n <= P4V_MAX_CAND, "matmul: eq_n must be in [1,%d]", P4V_MAX_CAND);
+  P4V_REQUIRE(d->images_per_chunk >= 0 && d->images_per_chunk <= d->batch,
+              "matmul: images_per_chunk must be in [0, batch=%d] (got %d; 0 = whole layer)", d->batch, d->images_per_chunk);
   p.sos = d->sos != 0;
-  p.H = d->heads; p.P = d->batch * d->heads; p.S1 = d->S1; p.S2 = d->S2; p.S3 = d->S3;
+  p.H = d->heads; p.P = d->batch * d->heads;
+  p.ipc = with_search ? d->images_per_chunk : 0;
+  p.Pc = p.ipc > 0 ? p.ipc * d->heads : p.P; p.S1 = d->S1; p.S2 = d->S2; p.S3 = d->S3;
   p.A_qmax = 1 << (d->A_bit - 1); p.B_qmax = 1 << (d->B_bit - 1);
   p.tiles_m = p4v_cdiv(p.S1, P4V_TILE); p.tiles_n = p4v_cdiv(p.S3, P4V_TILE);
   if (d->operand == P4V_OPERAND_INT8) p.i8 = true;
@@ -144,7 +150,7 @@ int build_plan(const p4v_matmul_desc* d, MMPlan& p, bool with_search) {
   p.o_segA = take(p.segA.size() * sizeof(P4VSeg)); p.o_segB = take(p.segB.size() * sizeof(P4VSeg));
   p.o_segAs = take(std::max<size_t>(1, p.segAs.size()) * sizeof(P4VSeg));
   p.o_segBs = take(std::max<size_t>(1, p.segBs.size()) * sizeof(P4VSeg));
-  const size_t tilesA = (size_t)p.P * p.tiles_m, tilesB = (size_t)p.P * p.tiles_n;
+  const size_t tilesA = (size_t)p.Pc * p.tiles_m, tilesB = (size_t)p.Pc * p.tiles_n;   // one chunk of problems
   p.o_partial = take(with_search ? tilesA * p.tiles_n * n_c * 32 * 4 : 4);
   p.o_Acur = take(tilesA * P4V_TILE * p.KB_A);
   p.o_Bcur = take(tilesB * P4V_TILE * p.KB_B);
@@ -170,11 +176,20 @@ int upload(const MMPlan& p, void* ws, cudaStream_t st) {
   return 0;
 }
 
-// which: 0 Acur, 1 Acand, 2 Bcur, 3 Bcand, 4 A split-search candidates (bf16), 5 B exact split (bf16)
-int quant(const MMPlan& p, void* ws, int which, const float* src, cudaStream_t st) {
+// problems [p0, p0 + n) of the layer: one chunk of whole images (or the whole layer)
+struct Chunk { int p0, n; };
+std::vector<Chunk> chunks(const MMPlan& p) {
+  std::vector<Chunk> cs;
+  for (int p0 = 0; p0 < p.P; p0 += p.Pc) cs.push_back(Chunk{p0, std::min(p.Pc, p.P - p0)});
+  return cs;
+}
+
+// which: 0 Acur, 1 Acand, 2 Bcur, 3 Bcand, 4 A split-search candidates (bf16), 5 B exact split (bf16); of the problems of c
+int quant(const MMPlan& p, void* ws, int which, const float* src, Chunk c, cudaStream_t st) {
   QuantImageArgs q{};
   const bool isA = which == 0 || which == 1 || which == 4;
-  q.src = src; q.P = p.P; q.prob_stride = isA ? (long long)p.S1 * p.S2 : (long long)p.S2 * p.S3;
+  q.P = c.n; q.prob_stride = isA ? (long long)p.S1 * p.S2 : (long long)p.S2 * p.S3;
+  q.src = src + (size_t)c.p0 * q.prob_stride;     // chunks start at an image: problem p of the chunk is head p % heads
   q.src_transposed = isA ? 0 : 1; q.ld = isA ? p.S2 : p.S3;
   q.rows = isA ? p.S1 : p.S3; q.tiles = isA ? p.tiles_m : p.tiles_n;
   q.rows_per_block = 0; q.d_mod = p.H; q.d_stride = 1;
@@ -192,18 +207,19 @@ int quant(const MMPlan& p, void* ws, int which, const float* src, cudaStream_t s
     default: q.dst = at<uint8_t>(ws, p.o_Bsplit); KB = p.KB_Bs; q.delta = at<float>(ws, p.o_dB0); q.segs = at<P4VSeg>(ws, p.o_segBs); q.nseg = 3; q.is_int8 = 0; break;
   }
   q.tile_bytes = (unsigned long long)P4V_TILE * KB;
-  q.plane_stride = q.tile_bytes * q.tiles * p.P;
+  q.plane_stride = q.tile_bytes * q.tiles * c.n;
   return p4v_quant_image(q, st);
 }
+int quant(const MMPlan& p, void* ws, int which, const float* src, cudaStream_t st) { return quant(p, ws, which, src, Chunk{0, p.P}, st); }
 
-void fill_sweep(const MMPlan& p, void* ws, const MStep& s, SweepParams& sp) {
+void fill_sweep(const MMPlan& p, void* ws, const MStep& s, SweepParams& sp, Chunk c) {
   sp = SweepParams{};
   sp.R_cur = at<uint8_t>(ws, p.o_Acur); sp.C_cur = at<uint8_t>(ws, p.o_Bcur);
   sp.R_cand = at<uint8_t>(ws, p.o_Acand); sp.C_cand = at<uint8_t>(ws, p.o_Bcand);
   sp.R_tile_bytes = sp.R_cand_tile_bytes = (unsigned long long)P4V_TILE * p.KB_A;
   sp.C_tile_bytes = sp.C_cand_tile_bytes = (unsigned long long)P4V_TILE * p.KB_B;
-  sp.R_cand_stride = sp.R_cand_tile_bytes * p.tiles_m * p.P; sp.C_cand_stride = sp.C_cand_tile_bytes * p.tiles_n * p.P;
-  sp.P = p.P; sp.M = p.S1; sp.N = p.S3; sp.tiles_m = p.tiles_m; sp.tiles_n = p.tiles_n;
+  sp.R_cand_stride = sp.R_cand_tile_bytes * p.tiles_m * c.n; sp.C_cand_stride = sp.C_cand_tile_bytes * p.tiles_n * c.n;
+  sp.P = c.n; sp.M = p.S1; sp.N = p.S3; sp.tiles_m = p.tiles_m; sp.tiles_n = p.tiles_n;
   sp.ld = p.S3; sp.prob_stride = (long long)p.S1 * p.S3;
   sp.gscale = at<float>(ws, p.o_gscale);
   sp.jobs = at<P4VJob>(ws, p.o_jobs) + s.job_off;
@@ -212,6 +228,7 @@ void fill_sweep(const MMPlan& p, void* ws, const MStep& s, SweepParams& sp) {
   sp.nsg = p.H; sp.sg_mode = P4V_SG_PROBLEM;
   sp.n_cand = p.d.eq_n; sp.partial = at<float>(ws, p.o_partial); sp.is_int8 = p.i8;
 }
+void fill_sweep(const MMPlan& p, void* ws, const MStep& s, SweepParams& sp) { fill_sweep(p, ws, s, sp, Chunk{0, p.P}); }
 
 int run_sweep(const MMPlan& p, const MStep& s, const SweepParams& sp, cudaStream_t st) {
   return p4v_run_sweep(sp, p.jobs.data() + s.job_off, p.d.kernel, st);
@@ -239,63 +256,85 @@ __global__ void sos_aux_kernel(const float* split, float qm1, float* aux, float*
 }
 __global__ void set_scalar_kernel(float* p, float v) { p[0] = v; }
 
-int reduce_finish(const MMPlan& p, void* ws, const SweepParams& sp, int n_cand, int n_groups, double inv_count,
-                  const float* factors, const float* d0, float* d, float* score_log, cudaStream_t st) {
+// scores of chunk c: the first chunk writes the fp64 table, later chunks add to it (fixed chunk order)
+int reduce(const MMPlan& p, void* ws, const SweepParams& sp, int n_cand, bool accumulate, cudaStream_t st) {
   ReduceArgs r{};
-  r.partial = sp.partial; r.n_cand = n_cand; r.P = p.P; r.tiles_m = p.tiles_m; r.tiles_n = p.tiles_n; r.order = sp.order;
-  r.mode = P4V_SG_PROBLEM; r.n_keys = p.H; r.sums = at<double>(ws, p.o_scores);
-  int rc = p4v_reduce_scores(r, st);
-  if (rc) return rc;
+  r.partial = sp.partial; r.n_cand = n_cand; r.P = sp.P; r.tiles_m = p.tiles_m; r.tiles_n = p.tiles_n; r.order = sp.order;
+  r.mode = P4V_SG_PROBLEM; r.n_keys = p.H; r.sums = at<double>(ws, p.o_scores); r.accumulate = accumulate ? 1 : 0;
+  return p4v_reduce_scores(r, st);
+}
+
+int finish(const MMPlan& p, void* ws, int n_cand, int n_groups, double inv_count, const float* factors, const float* d0,
+           float* d, float* score_log, cudaStream_t st) {
   SelectArgs f{};     // no image commit: the current image is re-quantised from the fp32 source with the chosen step size
-  f.sums = r.sums; f.n_cand = n_cand; f.n_keys = p.H; f.n_groups = n_groups; f.keys_per_group = n_groups == 1 ? p.H : 1;
+  f.sums = at<double>(ws, p.o_scores); f.n_cand = n_cand; f.n_keys = p.H; f.n_groups = n_groups; f.keys_per_group = n_groups == 1 ? p.H : 1;
   f.inv_count = inv_count; f.gscale = at<float>(ws, p.o_gscale); f.factors = factors;
   f.d0 = d0; f.d = d; f.d_stride = 1; f.d_col = 0; f.best = at<int>(ws, p.o_best); f.score_log = score_log;
   f.has_next = 0;
   return p4v_select_step(f, st);
 }
 
-int search_A(const MMPlan& p, void* ws, const float* A, const float* Y, const float* G, float* log, cudaStream_t st) {
+// One search step over every chunk: [chunk images] -> sweep -> reduce (into the table).  Unchunked, the images are
+// those begin() built and the previous step re-quantised.
+template <class Images, class Setup>
+int sweep_chunks(const MMPlan& p, void* ws, const MStep& s, const float* Y, const float* G, int n_cand, Images images,
+                 Setup setup, cudaStream_t st) {
+  int rc;
+  const std::vector<Chunk> cs = chunks(p);
+  for (size_t i = 0; i < cs.size(); ++i) {
+    if (p.ipc && (rc = images(cs[i]))) return rc;
+    const size_t off = (size_t)cs[i].p0 * p.S1 * p.S3;
+    SweepParams sp; fill_sweep(p, ws, s, sp, cs[i]);
+    sp.Y = Y + off; sp.Gr = G + off;
+    setup(sp, cs[i]);
+    if ((rc = run_sweep(p, s, sp, st))) return rc;
+    if ((rc = reduce(p, ws, sp, n_cand, i > 0, st))) return rc;
+  }
+  return 0;
+}
+
+int search_A(const MMPlan& p, void* ws, const float* A, const float* B, const float* Y, const float* G, float* log, cudaStream_t st) {
   int rc;
   if ((rc = tables(p, ws, p.stepA, 2, at<float>(ws, p.o_dA0), at<float>(ws, p.o_dA), at<float>(ws, p.o_dB),
                    at<float>(ws, p.o_factors), p.d.eq_n, st))) return rc;
-  SweepParams sp; fill_sweep(p, ws, p.stepA, sp);
-  sp.Y = Y; sp.Gr = G; sp.order = 1;
-  if ((rc = run_sweep(p, p.stepA, sp, st))) return rc;
-  if ((rc = reduce_finish(p, ws, sp, p.d.eq_n, p.H, 1.0 / ((double)p.S1 * p.S3), at<float>(ws, p.o_factors),
-                          at<float>(ws, p.o_dA0), at<float>(ws, p.o_dA), log, st))) return rc;
-  return quant(p, ws, 0, A, st);
+  auto images = [&](Chunk c) { int r = quant(p, ws, 1, A, c, st); return r ? r : quant(p, ws, 2, B, c, st); };
+  if ((rc = sweep_chunks(p, ws, p.stepA, Y, G, p.d.eq_n, images, [](SweepParams& sp, Chunk) { sp.order = 1; }, st))) return rc;
+  if ((rc = finish(p, ws, p.d.eq_n, p.H, 1.0 / ((double)p.S1 * p.S3), at<float>(ws, p.o_factors),
+                   at<float>(ws, p.o_dA0), at<float>(ws, p.o_dA), log, st))) return rc;
+  return p.ipc ? 0 : quant(p, ws, 0, A, st);
 }
 
-int search_B(const MMPlan& p, void* ws, const float* B, const float* Y, const float* G, float* log, cudaStream_t st) {
+int search_B(const MMPlan& p, void* ws, const float* A, const float* B, const float* Y, const float* G, float* log, cudaStream_t st) {
   int rc;
   if ((rc = tables(p, ws, p.stepB, p.sos ? 3 : 2, at<float>(ws, p.o_dB0), at<float>(ws, p.o_dB),
                    p.sos ? at<float>(ws, p.o_aux) : at<float>(ws, p.o_dA), at<float>(ws, p.o_factors), p.d.eq_n, st))) return rc;
-  SweepParams sp; fill_sweep(p, ws, p.stepB, sp);
-  sp.Y = Y; sp.Gr = G; sp.order = 0;
-  if ((rc = run_sweep(p, p.stepB, sp, st))) return rc;
-  if ((rc = reduce_finish(p, ws, sp, p.d.eq_n, p.H, 1.0 / ((double)p.S1 * p.S3), at<float>(ws, p.o_factors),
-                          at<float>(ws, p.o_dB0), at<float>(ws, p.o_dB), log, st))) return rc;
-  return quant(p, ws, 2, B, st);
+  auto images = [&](Chunk c) { int r = quant(p, ws, 0, A, c, st); return r ? r : quant(p, ws, 3, B, c, st); };
+  if ((rc = sweep_chunks(p, ws, p.stepB, Y, G, p.d.eq_n, images, [](SweepParams& sp, Chunk) { sp.order = 0; }, st))) return rc;
+  if ((rc = finish(p, ws, p.d.eq_n, p.H, 1.0 / ((double)p.S1 * p.S3), at<float>(ws, p.o_factors),
+                   at<float>(ws, p.o_dB0), at<float>(ws, p.o_dB), log, st))) return rc;
+  return p.ipc ? 0 : quant(p, ws, 2, B, st);
 }
 
-int search_split(const MMPlan& p, void* ws, const float* A, const float* Y, const float* G, float* log, cudaStream_t st) {
+int search_split(const MMPlan& p, void* ws, const float* A, const float* B, const float* Y, const float* G, float* log, cudaStream_t st) {
   int rc;
   // candA[c][head] = split_c * 1, candB[g][head] = aux[0] = 1/(qmax-1); the high part ignores candA
   if ((rc = tables(p, ws, p.stepS, 3, at<float>(ws, p.o_ones), at<float>(ws, p.o_ones), at<float>(ws, p.o_aux),
                    at<float>(ws, p.o_sfactors), p.n_split, st))) return rc;
-  SweepParams sp; fill_sweep(p, ws, p.stepS, sp);
-  sp.Y = Y; sp.Gr = G; sp.order = 1; sp.n_cand = p.n_split; sp.is_int8 = 0; sp.cand_noA_mask = 1ull;
-  sp.R_cand = at<uint8_t>(ws, p.o_Ascand); sp.R_cand_tile_bytes = (unsigned long long)P4V_TILE * p.KB_As;
-  sp.R_cand_stride = sp.R_cand_tile_bytes * p.tiles_m * p.P;
-  sp.C_cur = at<uint8_t>(ws, p.o_Bsplit); sp.C_tile_bytes = (unsigned long long)P4V_TILE * p.KB_Bs;
-  if ((rc = run_sweep(p, p.stepS, sp, st))) return rc;
+  auto images = [&](Chunk c) { int r = quant(p, ws, 4, A, c, st); return r ? r : quant(p, ws, 5, B, c, st); };
+  auto setup = [&](SweepParams& sp, Chunk c) {
+    sp.order = 1; sp.n_cand = p.n_split; sp.is_int8 = 0; sp.cand_noA_mask = 1ull;
+    sp.R_cand = at<uint8_t>(ws, p.o_Ascand); sp.R_cand_tile_bytes = (unsigned long long)P4V_TILE * p.KB_As;
+    sp.R_cand_stride = sp.R_cand_tile_bytes * p.tiles_m * c.n;
+    sp.C_cur = at<uint8_t>(ws, p.o_Bsplit); sp.C_tile_bytes = (unsigned long long)P4V_TILE * p.KB_Bs;
+  };
+  if ((rc = sweep_chunks(p, ws, p.stepS, Y, G, p.n_split, images, setup, st))) return rc;
   // global score: mean over heads and rows (matmul.py:620-621)
-  if ((rc = reduce_finish(p, ws, sp, p.n_split, 1, 1.0 / ((double)p.H * p.S1 * p.S3), at<float>(ws, p.o_sfactors),
-                          at<float>(ws, p.o_ones), at<float>(ws, p.o_split), log, st))) return rc;
+  if ((rc = finish(p, ws, p.n_split, 1, 1.0 / ((double)p.H * p.S1 * p.S3), at<float>(ws, p.o_sfactors),
+                   at<float>(ws, p.o_ones), at<float>(ws, p.o_split), log, st))) return rc;
   sos_aux_kernel<<<1, 1, 0, st>>>(at<float>(ws, p.o_split), (float)(p.A_qmax - 1), at<float>(ws, p.o_aux), nullptr);
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
-  return quant(p, ws, 0, A, st);
+  return p.ipc ? 0 : quant(p, ws, 0, A, st);
 }
 
 int begin(const MMPlan& p, void* ws, const float* A, const float* B, const float* G, cudaStream_t st) {
@@ -317,6 +356,9 @@ int begin(const MMPlan& p, void* ws, const float* A, const float* B, const float
     set_scalar_kernel<<<1, 1, 0, st>>>(at<float>(ws, p.o_split), 0.01f);       // matmul.py:354-355 (dead: overwritten by the first search)
     sos_aux_kernel<<<1, 1, 0, st>>>(at<float>(ws, p.o_split), (float)(p.A_qmax - 1), at<float>(ws, p.o_aux), nullptr);
     P4V_CUDA_OK(cudaGetLastError());
+  }
+  if (p.ipc) return 0;            // chunked: every step builds its chunks' images
+  if (p.sos) {
     if ((rc = quant(p, ws, 4, A, st))) return rc;
     if ((rc = quant(p, ws, 5, B, st))) return rc;
   } else {
@@ -356,13 +398,13 @@ extern "C" int p4v_matmul_calibrate(const p4v_matmul_desc* d, const float* A, co
   if ((rc = begin(p, workspace, A, B, raw_grad, st))) return rc;
   for (int e = 0; e < d->search_round; ++e) {
     if (p.sos) {
-      if ((rc = search_split(p, workspace, A, raw_out, raw_grad, score_log, st))) return rc;
+      if ((rc = search_split(p, workspace, A, B, raw_out, raw_grad, score_log, st))) return rc;
       if (score_log) score_log += p.n_split;
     } else {
-      if ((rc = search_A(p, workspace, A, raw_out, raw_grad, score_log, st))) return rc;
+      if ((rc = search_A(p, workspace, A, B, raw_out, raw_grad, score_log, st))) return rc;
       if (score_log) score_log += (size_t)d->eq_n * p.H;
     }
-    if ((rc = search_B(p, workspace, B, raw_out, raw_grad, score_log, st))) return rc;
+    if ((rc = search_B(p, workspace, A, B, raw_out, raw_grad, score_log, st))) return rc;
     if (score_log) score_log += (size_t)d->eq_n * p.H;
   }
   if (p.sos) {

@@ -262,13 +262,19 @@ __global__ void reduce_scores_kernel(const ReduceArgs a) {
       }
     acc += __shfl_xor_sync(0xffffffffu, acc, 8);
     acc += __shfl_xor_sync(0xffffffffu, acc, 16);
-    if (lane < 8) a.sums[(size_t)c * a.n_keys + key * P4V_TILE_CG + lane] = acc;
+    if (lane < 8) {
+      double* s = a.sums + (size_t)c * a.n_keys + key * P4V_TILE_CG + lane;
+      *s = a.accumulate ? *s + acc : acc;
+    }
   } else {                                // key = p % n_keys ; all 32 entries belong to the key
     for (int p = key; p < a.P; p += a.n_keys)
       for (int t = 0; t < per_p; ++t)
         acc += (double)a.partial[(((size_t)p * per_p + t) * a.n_cand + c) * 32 + lane];
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if (lane == 0) a.sums[(size_t)c * a.n_keys + key] = acc;
+    if (lane == 0) {
+      double* s = a.sums + (size_t)c * a.n_keys + key;
+      *s = a.accumulate ? *s + acc : acc;
+    }
   }
 }
 

@@ -68,6 +68,7 @@ struct ReduceArgs {
   int mode;                  // P4V_SG_COLUMN: key = global 16-column group (tn*8+i) ; P4V_SG_PROBLEM: key = p % n_keys
   int n_keys;
   double* sums;              // [n_cand][n_keys]  fixed-order fp64 sums of the sweep partials
+  int accumulate;            // 1: add to sums (later chunks of a chunked search) instead of overwriting them
 };
 int p4v_reduce_scores(const ReduceArgs& a, cudaStream_t st);
 

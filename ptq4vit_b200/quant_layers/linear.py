@@ -12,6 +12,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _lib
+from ._chunking import choose_chunks, workspace_budget
 from ._metric import metric_weight
 
 GELU_MIN_NEG = 0.16997124254703522  # reference: quant_layers/linear.py:574
@@ -199,7 +200,7 @@ class PTQSLQuantLinear(MinMaxQuantLinear):
         self.crb_rows = out_features // n_V
         self.crb_cols = in_features // n_H  # ignore remnent != 0 situations
         self.crb_acts = in_features // n_a
-        self.parallel_eq_n = parallel_eq_n   # kept for signature parity; the CUDA path holds a whole layer in HBM
+        self.parallel_eq_n = parallel_eq_n   # kept for signature parity; the CUDA path sizes its chunks by device memory
         self.init_layerwise = init_layerwise
         self.raw_grad = None
         self.last_scores = None              # optional per-step score tables (set P4V_SCORE_LOG=1 or keep_scores=True)
@@ -220,7 +221,18 @@ class PTQSLQuantLinear(MinMaxQuantLinear):
         d = self._desc(x2.shape[0], tokens, self.search_round, (self.eq_alpha, self.eq_beta, self.eq_n))
         lib = _lib.lib()
         nbytes, nlog = ctypes.c_size_t(), ctypes.c_size_t()
-        _lib.check(lib.p4v_linear_workspace_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "p4v_linear_workspace_bytes")
+
+        def ws_bytes(rows_per_chunk):
+            d.rows_per_chunk = rows_per_chunk
+            _lib.check(lib.p4v_linear_workspace_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "p4v_linear_workspace_bytes")
+            return nbytes.value
+        # rows per chunk: a multiple of the 128-row tile; 0 (the whole layer) whenever it fits
+        rows_per_chunk, n_chunks = choose_chunks(d.rows, 128, ws_bytes, workspace_budget(dev))
+        ws_bytes(rows_per_chunk)
+        if n_chunks > 1:         # the reference's batching attributes: images per chunk (a chunk may end inside an image)
+            self.calib_need_batching = True
+            self.calib_batch_size = -(-rows_per_chunk // tokens)
+        self.calib_chunks = n_chunks
         _lib.check(lib.p4v_linear_score_log_floats(ctypes.byref(d), ctypes.byref(nlog)), "p4v_linear_score_log_floats")
         ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
         w = self.weight.detach().contiguous().float()
@@ -273,7 +285,8 @@ class PTQSLBatchingQuantLinear(PTQSLQuantLinear):
         self.calib_need_batching = False
 
     def _initialize_calib_parameters(self):
-        """reference: linear.py:365-378.  80 GB of HBM hold a whole layer: no batching."""
+        """reference: linear.py:365-378.  The search batches only when its workspace does not fit in the free device
+        memory; _native_calibrate then sets calib_need_batching and calib_batch_size (images per chunk of rows)."""
         self.calib_size = int(self.raw_input.shape[0])
         self.calib_batch_size = int(self.raw_input.shape[0])
         self.calib_need_batching = False

@@ -10,6 +10,7 @@ import torch
 from torch import nn
 
 from .. import _lib
+from ._chunking import choose_chunks, workspace_budget
 from ._metric import metric_weight
 
 
@@ -191,7 +192,17 @@ class PTQSLQuantMatMul(MinMaxQuantMatMul):
         H = d.heads
         lib = _lib.lib()
         nbytes, nlog = ctypes.c_size_t(), ctypes.c_size_t()
-        _lib.check(lib.p4v_matmul_workspace_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "p4v_matmul_workspace_bytes")
+
+        def ws_bytes(images_per_chunk):
+            d.images_per_chunk = images_per_chunk
+            _lib.check(lib.p4v_matmul_workspace_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "p4v_matmul_workspace_bytes")
+            return nbytes.value
+        images_per_chunk, n_chunks = choose_chunks(d.batch, 1, ws_bytes, workspace_budget(dev))
+        ws_bytes(images_per_chunk)
+        if n_chunks > 1:         # the reference's batching attributes (matmul.py:396-409)
+            self.calib_need_batching = True
+            self.calib_batch_size = max(1, images_per_chunk // (d.batch // int(A.shape[0])))   # heads folded into the batch
+        self.calib_chunks = n_chunks
         _lib.check(lib.p4v_matmul_score_log_floats(ctypes.byref(d), ctypes.byref(nlog)), "p4v_matmul_score_log_floats")
         ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
         a_int = torch.empty(H, dtype=torch.float32, device=dev)
@@ -243,7 +254,8 @@ class PTQSLBatchingQuantMatMul(PTQSLQuantMatMul):
     _force_headwise = True
 
     def _initialize_calib_parameters(self):
-        """reference: matmul.py:396-409; a whole layer fits in HBM, no batching."""
+        """reference: matmul.py:396-409.  The search batches only when its workspace does not fit in the free device
+        memory; _native_calibrate then sets calib_need_batching and calib_batch_size (images per chunk)."""
         self.calib_size = int(self.raw_input[0].shape[0])
         self.calib_batch_size = int(self.raw_input[0].shape[0])
         self.calib_need_batching = False

@@ -8,20 +8,26 @@
   (quant_calib.py:369-372), so the captured (input, output, grad) tensors do not depend on the
   order -- ONE forward+backward sweep over the calibration images with hooks on all modules
   replaces the reference's one-sweep-per-module loop (quant_calib.py:317-356), and the tensors
-  stay in HBM instead of bouncing through host memory (quant_calib.py:173-201).  When the
-  tensors do not fit (`capture="per_module"`) or sequential=True the reference's loop is used.
+  stay in HBM instead of bouncing through host memory (quant_calib.py:173-201).  With
+  capture="auto" the captures of this rank are estimated from the shapes seen in the first batch of
+  the target pass: when they cannot fit in free device memory (or `capture_budget` bytes) next to the
+  largest of the smallest search workspaces, or with `capture="per_module"` or sequential=True, the
+  reference's loop is used.
 * search: `module.calibration_step2()` runs the CUDA search.
 * multi-GPU: modules are independent => static LPT sharding over ranks, every rank captures,
   searches its share, and one all_gather of the chosen step sizes ends the job.
 """
+import ctypes
 import time
 
 import torch
 import torch.nn.functional as F
 
+from .. import _lib
+from ..quant_layers._chunking import device_free_bytes
 from ..quant_layers.conv import MinMaxQuantConv2d
-from ..quant_layers.linear import MinMaxQuantLinear, PTQSLBatchingQuantLinear
-from ..quant_layers.matmul import MinMaxQuantMatMul, PTQSLBatchingQuantMatMul
+from ..quant_layers.linear import MinMaxQuantLinear, PTQSLBatchingQuantLinear, PTQSLQuantLinear
+from ..quant_layers.matmul import MinMaxQuantMatMul, PTQSLBatchingQuantMatMul, PTQSLQuantMatMul
 
 
 # ---------------------------------------------------------------- hooks (device resident)
@@ -122,6 +128,61 @@ def module_cost(module, n_img, shapes=None, tokens_hint=197):
             lead, H, S1, S2, S3 = 1, 12, tokens_hint, 64, tokens_hint
         return rounds * (_ROUND_OVERHEAD_S + 2 * eq_n * 2.0 * n_img * lead * H * S1 * S2 * S3 / _MATMUL_RATE)
     return 0.0
+
+
+def _prod(shape):
+    n = 1
+    for s in shape:
+        n *= int(s)
+    return n
+
+
+def capture_bytes(module, n_img, shapes):
+    """Bytes of the tensors the single-pass capture keeps for one module until its search: fp32 input(s), output and
+    output gradient, from the per-image shapes seen in the target pass (see HessianQuantCalibrator._record_shapes)."""
+    if shapes is None:
+        return 0
+    if "x" in shapes:
+        rows = n_img * _prod(shapes["x"][:-1])
+        return 4 * rows * (int(shapes["x"][-1]) + 2 * module.out_features)
+    if "A" in shapes:
+        lead, H, S1, S2 = _prod(shapes["A"][:-3]), *[int(s) for s in shapes["A"][-3:]]
+        S3 = int(shapes["B"][-1])
+        return 4 * n_img * lead * H * (S1 * S2 + S2 * S3 + 2 * S1 * S3)
+    return 4 * n_img * (shapes.get("x_elems", 0) + 2 * shapes.get("y_elems", 0))
+
+
+def min_search_workspace_bytes(module, n_img, shapes):
+    """Device memory the module's search needs at least: its workspace split into the smallest chunks the library takes
+    (128 rows of a Linear, one image of a MatMul); the conv search (not chunked) with its im2col matrix; 0 for modules
+    without a native search."""
+    if shapes is None:
+        return 0
+    lib = _lib.lib()
+    n = ctypes.c_size_t()
+    eq = (module.eq_alpha, module.eq_beta, module.eq_n) if hasattr(module, "eq_n") else None
+    if isinstance(module, PTQSLQuantLinear) and "x" in shapes:
+        rows = n_img * _prod(shapes["x"][:-1])
+        d = module._desc(rows, _prod(shapes["x"][1:-1]), module.search_round, eq)
+        d.rows_per_chunk = 128 if rows > 128 else 0
+        _lib.check(lib.p4v_linear_workspace_bytes(ctypes.byref(d), ctypes.byref(n)), "p4v_linear_workspace_bytes")
+        return n.value
+    if isinstance(module, PTQSLQuantMatMul) and "A" in shapes:
+        batch = n_img * _prod(shapes["A"][:-3])
+        A = torch.empty((batch,) + tuple(shapes["A"][-3:]), device="meta")
+        B = torch.empty((batch,) + tuple(shapes["B"][-3:]), device="meta")
+        d = module._desc(A, B, module.search_round, eq)
+        d.images_per_chunk = 1
+        _lib.check(lib.p4v_matmul_workspace_bytes(ctypes.byref(d), ctypes.byref(n)), "p4v_matmul_workspace_bytes")
+        return n.value
+    if isinstance(module, MinMaxQuantConv2d) and hasattr(module, "eq_n") and "positions" in shapes:
+        d = _lib.ConvDesc()
+        d.images, d.out_channels, d.K, d.positions = n_img, module.out_channels, shapes["conv_K"], shapes["positions"]
+        d.w_bit, d.eq_n, d.eq_alpha, d.eq_beta = int(module.w_bit), int(module.eq_n), float(module.eq_alpha), float(module.eq_beta)
+        d.has_bias = 0 if module.bias is None else 1
+        _lib.check(lib.p4v_conv_workspace_bytes(ctypes.byref(d), ctypes.byref(n)), "p4v_conv_workspace_bytes")
+        return n.value + 4 * n_img * shapes["positions"] * shapes["conv_K"]
+    return 0
 
 
 def shard_modules(names, costs, world_size):
@@ -359,7 +420,7 @@ class HessianQuantCalibrator(QuantCalibrator):
     """reference: utils/quant_calib.py:203-378"""
 
     def __init__(self, net, wrapped_modules, calib_loader, sequential=False, batch_size=1, capture="auto",
-                 distributed=None, target_noise=0.0):
+                 distributed=None, target_noise=0.0, capture_budget=None):
         super().__init__(net, wrapped_modules, calib_loader, sequential=sequential)
         self.batch_size = batch_size
         self.capture = capture
@@ -367,14 +428,22 @@ class HessianQuantCalibrator(QuantCalibrator):
         self.target_noise = target_noise     # synthetic benches: perturb the KL target so that gradients are not ~0
         self.timings = {}
         self.keep_captured = None            # tests: a dict to receive {name: captured tensors} before they are consumed
+        self.capture_budget = capture_budget  # capture="auto": bytes for captures + search (None: the free device memory)
 
     # -- target distribution (quant_calib.py:228-232 / :308-313)
-    def _raw_pred_softmax(self):
+    def _raw_pred_softmax(self, shapes=None):
+        """The net's softmax over every calibration image; with a dict `shapes`, also the per-image input shapes of every
+        wrapped module (see _record_shapes), taken from the first batch."""
         dev = self._device()
         preds = []
+        hooks = self._record_shapes(shapes) if shapes is not None else []
         with torch.no_grad():
             for inp in self._loader_batches():
+                self._batch_images = int(inp.shape[0])
                 preds.append(F.softmax(self.net(inp.to(dev)), dim=-1).detach())
+                for h in hooks:
+                    h.remove()
+                hooks = []
         raw = torch.cat(preds, dim=0)
         if self.target_noise > 0:
             gen = torch.Generator(device=raw.device).manual_seed(1234)
@@ -398,47 +467,63 @@ class HessianQuantCalibrator(QuantCalibrator):
         want = hasattr(module, "metric") and (module.metric == "hessian" or not hessian_only)
         return self._forward_hooks_for(module, want_grad=want)
 
-    # -- layer-wise sharding (only meaningful when sequential=False)
-    def _probe_shapes(self):
-        """Per-image input shapes of every wrapped module (one forward of one image, no grad)."""
-        shapes, hooks = {}, []
-
+    # -- layer-wise sharding (only meaningful when sequential=False) and the capture plan
+    def _record_shapes(self, shapes):
+        """Forward hooks filling `shapes` with the per-image input shapes of every wrapped module, as the first forward
+        they see (of self._batch_images images) has them; window attention folds windows into the batch dimension:
+        lead = windows per image.  Returns the hooks."""
         def rec(name):
             def f(mod, inp, out):
+                if name in shapes:
+                    return
+                lead = max(1, int(inp[0].shape[0]) // self._batch_images)
                 if isinstance(mod, MinMaxQuantMatMul):
-                    shapes[name] = {"A": tuple(inp[0].shape[1:]), "B": tuple(inp[1].shape[1:]), "lead": int(inp[0].shape[0])}
+                    shapes[name] = {"A": (lead,) + tuple(inp[0].shape[1:]), "B": tuple(inp[1].shape[1:])}
                 elif isinstance(mod, MinMaxQuantConv2d):
                     k = mod.kernel_size
-                    shapes[name] = {"conv_macs": float(out.shape[1] * out.shape[2] * out.shape[3] * mod.in_channels * k[0] * k[1])}
+                    shapes[name] = {"conv_macs": float(out.shape[1] * out.shape[2] * out.shape[3] * mod.in_channels * k[0] * k[1]),
+                                    "x_elems": inp[0][0].numel(), "y_elems": out[0].numel(),
+                                    "positions": int(out.shape[2] * out.shape[3]), "conv_K": int(mod.in_channels * k[0] * k[1])}
                 else:
-                    shapes[name] = {"x": tuple(inp[0].shape[1:]), "lead": int(inp[0].shape[0])}
+                    shapes[name] = {"x": (lead,) + tuple(inp[0].shape[1:])}
             return f
-        for n, m in self.wrapped_modules.items():
-            hooks.append(m.register_forward_hook(rec(n)))
+        return [m.register_forward_hook(rec(n)) for n, m in self.wrapped_modules.items()]
+
+    def _probe_shapes(self):
+        """Per-image input shapes of every wrapped module from one forward of one image (no grad)."""
+        shapes = {}
+        hooks = self._record_shapes(shapes)
         first = next(iter(self._loader_batches()))
+        self._batch_images = 1
         with torch.no_grad():
             self.net(first[:1].to(self._device()))
         for h in hooks:
             h.remove()
-        # window attention folds windows into the batch dimension: lead = windows per image
-        for n, s in shapes.items():
-            lead = s.pop("lead", 1)
-            if "x" in s:
-                s["x"] = (lead,) + s["x"]
-            if "A" in s:
-                s["A"] = (lead,) + s["A"]
         return shapes
 
-    def _my_modules(self):
+    def _my_modules(self, shapes=None):
+        """This rank's modules and the owner of every module (None on one rank).  `shapes`: as _record_shapes fills
+        them; probed with one forward when not given."""
         names = list(self.wrapped_modules.keys())
         dist = self.distributed
         if dist is None or not dist.is_initialized() or dist.get_world_size() == 1 or self.sequential:
             return names, None
         n_img = sum(inp.shape[0] for inp in self._loader_batches())
-        shapes = self._probe_shapes()
+        shapes = shapes if shapes is not None else self._probe_shapes()
         costs = [module_cost(self.wrapped_modules[n], n_img, shapes.get(n)) for n in names]
         owner = shard_modules(names, costs, dist.get_world_size())
         return [n for n in names if owner[n] == dist.get_rank()], owner
+
+    def _capture_plan(self, my_names, shapes):
+        """capture="auto": one capture pass for all of this rank's modules when their captured tensors fit in the free
+        device memory (or `capture_budget`) next to the largest memory one of their searches needs at least, else the
+        per-module loop.  Returns (single_pass, estimated capture bytes, that search memory, budget)."""
+        n_img = sum(inp.shape[0] for inp in self._loader_batches())
+        mods = [(self.wrapped_modules[n], shapes.get(n)) for n in my_names]
+        est = sum(capture_bytes(m, n_img, s) for m, s in mods)
+        ws = max([min_search_workspace_bytes(m, n_img, s) for m, s in mods] + [0])
+        budget = self.capture_budget if self.capture_budget is not None else device_free_bytes(self._device())
+        return est + ws <= budget, est, ws, budget
 
     def _gather(self, owner):
         dist = self.distributed
@@ -478,9 +563,17 @@ class HessianQuantCalibrator(QuantCalibrator):
     def batching_quant_calib(self):
         """reference: quant_calib.py:300-378"""
         t0 = self._clock()
-        raw_pred_softmax = self._raw_pred_softmax()
-        my_names, owner = self._my_modules()
-        single_pass = (not self.sequential) and self.capture in ("auto", "single_pass")
+        auto = (not self.sequential) and self.capture == "auto"
+        shapes = {}
+        raw_pred_softmax = self._raw_pred_softmax(shapes)
+        my_names, owner = self._my_modules(shapes)
+        plan = {}
+        if auto:
+            fits, est, ws, budget = self._capture_plan(my_names, shapes)
+            single_pass = fits
+            plan = {"capture_bytes_est": est, "min_workspace_bytes": ws, "memory_budget_bytes": budget}
+        else:
+            single_pass = (not self.sequential) and self.capture == "single_pass"
         t_capture = t_search = 0.0
         if single_pass:
             hooks = []
@@ -523,7 +616,8 @@ class HessianQuantCalibrator(QuantCalibrator):
         self.calibrated = True
         t3 = self._clock()
         self.timings = {"capture_s": t_capture, "search_s": t_search, "gather_s": t3 - t2, "total_s": t3 - t0,
-                        "modules_searched": len(my_names), "single_pass": bool(single_pass)}
+                        "modules_searched": len(my_names), "single_pass": bool(single_pass),
+                        "capture_mode": "single_pass" if single_pass else "per_module", **plan}
 
     def quant_calib(self):
         """reference: quant_calib.py:216-298 -- the non-batching driver: per module one forward+backward sweep, then
