@@ -175,6 +175,44 @@ __device__ __forceinline__ void wgmma_stage(AccT (&d)[64], uint32_t nk, uint64_t
   wg_commit();
 }
 
+// Pair steps: one column half at a time.  D[64 rows][64 cols] (+)= A[64][32 bytes of K] * B[64][32 bytes of K]^T.
+#define P4V_WG_D32                                                                                                 \
+  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29," \
+  "%30,%31}"
+#define P4V_WG_OP32(C) P4V_WG_OP8(C, 0), P4V_WG_OP8(C, 8), P4V_WG_OP8(C, 16), P4V_WG_OP8(C, 24)
+__device__ __forceinline__ void wgmma_n64_k32(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " P4V_WG_D32 ", %32, %33, p, 1, 1, 0, 0;\n\t}"
+               : P4V_WG_OP32(P4V_F) : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_n64_k32(uint32_t (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 " P4V_WG_D32 ", %32, %33, p;\n\t}"
+               : P4V_WG_OP32(P4V_R) : "l"(da), "l"(db), "r"(accumulate));
+}
+// One stage of a pair step: the same nk k32 steps of the shared column slab against both row parts (d0: part 0, d1:
+// part 1), one committed straight-line batch per count as in wgmma_stage.
+template <int N, typename AccT>
+__device__ __forceinline__ void wgmma_pair_seq(AccT (&d0)[32], AccT (&d1)[32], uint64_t da0, uint64_t da1, uint64_t db,
+                                               uint32_t accumulate) {
+#pragma unroll
+  for (int k = 0; k < N; ++k) wgmma_n64_k32(d0, da0 + 256 * k, db + 256 * k, k ? 1u : accumulate);
+#pragma unroll
+  for (int k = 0; k < N; ++k) wgmma_n64_k32(d1, da1 + 256 * k, db + 256 * k, k ? 1u : accumulate);
+}
+template <typename AccT>
+__device__ __forceinline__ void wgmma_pair_stage(AccT (&d0)[32], AccT (&d1)[32], uint32_t nk, uint64_t da0, uint64_t da1,
+                                                 uint64_t db, uint32_t accumulate) {
+  wg_fence();
+  switch (nk) {
+    case 1: wgmma_pair_seq<1>(d0, d1, da0, da1, db, accumulate); break;
+    case 2: wgmma_pair_seq<2>(d0, d1, da0, da1, db, accumulate); break;
+    case 3: wgmma_pair_seq<3>(d0, d1, da0, da1, db, accumulate); break;
+    default: wgmma_pair_seq<4>(d0, d1, da0, da1, db, accumulate); break;
+  }
+  wg_commit();
+}
+
 // Register reallocation between the warpgroups (all four warps of a warpgroup execute it): the producer warpgroup
 // gives registers back, the consumer warpgroups take them.  128 * 56 + 256 * 224 = 384 * 168, the launch budget.
 // ptxas -v: no spills in any instantiation (40 / 232 leaves the producer spilling 12-20 bytes).
@@ -243,9 +281,19 @@ __device__ __forceinline__ float reduce8_over_warp(float (&p)[8], int lane) {
   return t;
 }
 
-template <bool kInt8, bool kSingle>
+// Consumer modes, chosen per launch by p4v_launch_sweep_tc:
+//   kModeSingle: one candidate group; r stays in registers, g is parked.
+//   kModeMulti:  several candidate groups, evaluated one job at a time; the residual is parked and restored per
+//                candidate, g is read from global memory per candidate.
+//   kModePair:   two candidate groups over the same candidate column slabs with different resident row parts (twin
+//                activations of post-GELU weight steps, hi/lo parts of split-of-softmax B steps): one ring stage per
+//                job pair, both parts multiplied per 64-column half, r stays in registers, g is parked.
+enum { kModeMulti = 0, kModeSingle = 1, kModePair = 2 };
+
+template <bool kInt8, int kMode>
 __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_constant__ SweepParams P) {
   using AccT = typename std::conditional<kInt8, uint32_t, float>::type;
+  constexpr bool kPair = kMode == kModePair, kMulti = kMode == kModeMulti;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
   // carve: [ring R stages][ring C stages][resident R x bufs][resident C][control][score reduction][gradient tile]
@@ -317,8 +365,9 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
       for (int j = 0; j < P.n_fixed_jobs; ++j) issue(S.jobs[j], r_cur, c_cur);
       const uint8_t* r_cand = P.R_cand + rt * P.R_cand_tile_bytes + (size_t)f.c0 * P.R_cand_stride;
       const uint8_t* c_cand = P.C_cand + ct * P.C_cand_tile_bytes + (size_t)f.c0 * P.C_cand_stride;
+      const int stage_jobs = kPair ? P.n_cand_jobs / 2 : P.n_cand_jobs;   // pair: job i + n/2 shares job i's column slab
       for (int c = f.c0; c < f.c1; ++c) {
-        for (int jj = 0; jj < P.n_cand_jobs; ++jj) {
+        for (int jj = 0; jj < stage_jobs; ++jj) {
           const P4VJob j = S.jobs[P.n_fixed_jobs + jj];
           issue(j, (j.flags & P4V_JOB_RCAND) ? r_cand : r_cur, (j.flags & P4V_JOB_CCAND) ? c_cand : c_cur);
         }
@@ -330,8 +379,8 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
 
   // ======================= consumers (2 warpgroups x 64 rows of the tile) =======================
   // Registers hold the residual r and the accumulator fragment.  This thread's slice of shared memory ([fragment value
-  // pair][consumer thread] float2) parks g in single-segment steps and, in multi-segment steps, the residual every
-  // candidate starts from (g is then read from global memory once per candidate).
+  // pair][consumer thread] float2) parks g in single-segment and pair steps and, in multi-segment steps, the residual
+  // every candidate starts from (g is then read from global memory once per candidate).
   regs_inc();
   const int et = threadIdx.x - 128;                  // 0..255
   const int wg = et >> 7;                            // row half of the tile
@@ -374,6 +423,10 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
   };
 
   while (next_frag(P, sched, f)) {
+    if constexpr (kPair) {   // acc must not stay live into the candidates, whose column halves use a0/a1 (see there)
+#pragma unroll
+      for (int v = 0; v < 64; ++v) acc[v] = 0;
+    }
     asm volatile("bar.sync 1, %0;" ::"n"(kConsumers));   // previous fragment done with the tables
     {
       const int sg0 = (P.sg_mode == P4V_SG_COLUMN) ? f.tn * P4V_TILE_CG : (f.p % P.nsg);
@@ -417,7 +470,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
           }
         }
         r[v] = y0 - b0; r[v + 1] = y1 - b1;
-        if (kSingle && want_g) park[(v >> 1) * kConsumers] = make_float2(g0 * gs, g1 * gs);
+        if (!kMulti && want_g) park[(v >> 1) * kConsumers] = make_float2(g0 * gs, g1 * gs);
       }
     }
     asm volatile("bar.sync 1, %0;" ::"n"(kConsumers));   // tables visible
@@ -442,16 +495,16 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
       }
       continue;
     }
-    if constexpr (!kSingle) {
+    if constexpr (kMulti) {
 #pragma unroll
       for (int v = 0; v < 64; v += 2) park[(v >> 1) * kConsumers] = make_float2(r[v], r[v + 1]);
     }
-    // g of values (v, v + 1): parked (single-segment steps) or from global memory
+    // g of values (v, v + 1): parked (single-segment and pair steps) or from global memory
     const bool gvec = ((P.ld | P.prob_stride) & 1) == 0 && (f.tn + 1) * P4V_TILE <= P.N &&
                       (reinterpret_cast<uintptr_t>(P.Gr) & 7) == 0;
     const float* const grow = P.Gr + pbase + (size_t)gm * P.ld + gc;
     auto gpair = [&](const int v) -> float2 {
-      if constexpr (kSingle) {
+      if constexpr (!kMulti) {
         return park[(v >> 1) * kConsumers];
       } else {
         const int h = (v >> 1) & 1, dc = 8 * (v >> 2);
@@ -468,50 +521,105 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
       mbar_wait(&S.res_full[rbuf], rphase);
       res16 = ((resR + rbuf * resB) & 0x3FFFF) >> 4;
     }
+    // Pair steps: the two column-half accumulators.  Defined here, and acc above at the start of the fragment, so that
+    // ptxas sees neither live across the other's use (a wgmma reads its accumulators: an undefined one stays live
+    // around the loops, which spills).
+    AccT a0[32], a1[32];
+    if constexpr (kPair) {
+#pragma unroll
+      for (int v = 0; v < 32; ++v) { a0[v] = 0; a1[v] = 0; }
+    }
     for (int c = f.c0; c < f.c1; ++c) {
-      if constexpr (!kSingle) {
+      if constexpr (kMulti) {
         if (c > f.c0) {
 #pragma unroll
           for (int v = 0; v < 64; v += 2) { const float2 x = park[(v >> 1) * kConsumers]; r[v] = x.x; r[v + 1] = x.y; }
         }
       }
       float ph[P4V_TILE_CG][2];                    // sum of (g * e)^2 per column group and fragment row
-      int gi = 0;
-      for (int jj = 0; jj < P.n_cand_jobs; ++jj) {
-        const P4VJob jb = S.jobs[P.n_fixed_jobs + jj];
-        run(jb, res16 + (jb.res_off >> 4) + wg * 64, [&] {
-          const bool noA = (P.cand_noA_mask >> gi) & 1ull;
-          if (gi + 1 < P.n_cand_groups) {
-            if constexpr (!kSingle) {
+      float p[P4V_TILE_CG];                        // ... and per column group (this thread's two rows)
+      if constexpr (kPair) {
+        // The candidate's np stages (job i: part 0 = job i, part 1 = job i + np, same column slab).  A column half's two
+        // accumulators run over all of them before its epilogue, so all np stages are held until the second half is
+        // done (the launcher guarantees np + 1 ring stages).  Same fp32 operations in the same order as the
+        // multi-segment path: t = r - s0 * acc0, then (g * (t - s1 * acc1))^2.
+        const int np = P.n_cand_jobs >> 1;
+        const bool noA0 = P.cand_noA_mask & 1ull, noA1 = (P.cand_noA_mask >> 1) & 1ull;
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          uint32_t s = stage, sp = phase;
+          for (int i = 0; i < np; ++i) {
+            if (half == 0) mbar_wait_addr(full0 + s * 8, sp);
+            const P4VJob j0 = S.jobs[P.n_fixed_jobs + i], j1 = S.jobs[P.n_fixed_jobs + np + i];
+            const uint64_t da0 = dconst | (uint64_t)(res16 + (j0.res_off >> 4) + wg * 64);
+            const uint64_t da1 = dconst | (uint64_t)(res16 + (j1.res_off >> 4) + wg * 64);
+            const uint64_t db = dconst | (uint64_t)(ringC16 + s * sC16 + half * 64);   // +64 rows x 16 B
+            const uint32_t nk = __shfl_sync(0xffffffffu, (uint32_t)j0.kb >> 5, 0);   // warp-uniform, see run()
+            wgmma_pair_stage(a0, a1, nk, da0, da1, db, (j0.flags & P4V_JOB_FIRST) ? 0u : 1u);
+            if (++s == nst) { s = 0; sp ^= 1; }
+          }
+          wg_wait0();
+          // a0[v] / a1[v] of this half = fragment value 32 * half + v of the m64n128 layout (column groups 4 * half ..)
+#pragma unroll
+          for (int k = 0; k < P4V_TILE_CG / 2; ++k) {
+            const int kk = (P4V_TILE_CG / 2) * half + k;
+            const float s0 = noA0 ? S.candB[0][kk] : S.candA[c][kk] * S.candB[0][kk];
+            const float s1 = noA1 ? S.candB[1][kk] : S.candA[c][kk] * S.candB[1][kk];
+            float q[2] = {0.f, 0.f};
+#pragma unroll
+            for (int e = 0; e < 8; e += 2) {
+              const int v = 8 * k + e, V = 32 * half + v;
+              const float2 gv = gpair(V);
+              const float w0 = gv.x * fmaf(-s1, acc_to_float(a1[v]), fmaf(-s0, acc_to_float(a0[v]), r[V]));
+              const float w1 = gv.y * fmaf(-s1, acc_to_float(a1[v + 1]), fmaf(-s0, acc_to_float(a0[v + 1]), r[V + 1]));
+              q[(e >> 1) & 1] = fmaf(w0, w0, q[(e >> 1) & 1]);
+              q[(e >> 1) & 1] = fmaf(w1, w1, q[(e >> 1) & 1]);
+            }
+            p[kk] = q[0] + q[1];                   // added at once: half 0 keeps 4 values live, not 8
+          }
+        }
+        for (int i = 0; i < np; ++i) {
+          warp_arrive(&S.empty[stage], lane);
+          if (++stage == nst) { stage = 0; phase ^= 1; }
+        }
+      } else {
+        int gi = 0;
+        for (int jj = 0; jj < P.n_cand_jobs; ++jj) {
+          const P4VJob jb = S.jobs[P.n_fixed_jobs + jj];
+          run(jb, res16 + (jb.res_off >> 4) + wg * 64, [&] {
+            const bool noA = (P.cand_noA_mask >> gi) & 1ull;
+            if (gi + 1 < P.n_cand_groups) {
+              if constexpr (kMulti) {
+#pragma unroll
+                for (int k = 0; k < P4V_TILE_CG; ++k) {
+                  const float s = noA ? S.candB[gi][k] : S.candA[c][k] * S.candB[gi][k];
+#pragma unroll
+                  for (int e = 0; e < 8; ++e) r[8 * k + e] = fmaf(-s, acc_to_float(acc[8 * k + e]), r[8 * k + e]);
+                }
+              }
+            } else {
+              // final segment: (g * (r - s*acc))^2; r itself is not modified
 #pragma unroll
               for (int k = 0; k < P4V_TILE_CG; ++k) {
                 const float s = noA ? S.candB[gi][k] : S.candA[c][k] * S.candB[gi][k];
+                float q[2] = {0.f, 0.f};
 #pragma unroll
-                for (int e = 0; e < 8; ++e) r[8 * k + e] = fmaf(-s, acc_to_float(acc[8 * k + e]), r[8 * k + e]);
+                for (int e = 0; e < 8; e += 2) {
+                  const int v = 8 * k + e;
+                  const float2 gv = gpair(v);
+                  const float w0 = gv.x * fmaf(-s, acc_to_float(acc[v]), r[v]);
+                  const float w1 = gv.y * fmaf(-s, acc_to_float(acc[v + 1]), r[v + 1]);
+                  q[(e >> 1) & 1] = fmaf(w0, w0, q[(e >> 1) & 1]);
+                  q[(e >> 1) & 1] = fmaf(w1, w1, q[(e >> 1) & 1]);
+                }
+                ph[k][0] = q[0]; ph[k][1] = q[1];
               }
             }
-          } else {
-            // final segment: (g * (r - s*acc))^2; r itself is not modified
-#pragma unroll
-            for (int k = 0; k < P4V_TILE_CG; ++k) {
-              const float s = noA ? S.candB[gi][k] : S.candA[c][k] * S.candB[gi][k];
-              float q[2] = {0.f, 0.f};
-#pragma unroll
-              for (int e = 0; e < 8; e += 2) {
-                const int v = 8 * k + e;
-                const float2 gv = gpair(v);
-                const float w0 = gv.x * fmaf(-s, acc_to_float(acc[v]), r[v]);
-                const float w1 = gv.y * fmaf(-s, acc_to_float(acc[v + 1]), r[v + 1]);
-                q[(e >> 1) & 1] = fmaf(w0, w0, q[(e >> 1) & 1]);
-                q[(e >> 1) & 1] = fmaf(w1, w1, q[(e >> 1) & 1]);
-              }
-              ph[k][0] = q[0]; ph[k][1] = q[1];
-            }
-          }
-          ++gi;
-        });
+            ++gi;
+          });
+        }
       }
-      if (P.row_keys) {
+      if (!kPair && P.row_keys) {
         // one score per ROW (channel-wise conv search): [tile][candidate][column half][128 rows].  The quad of lanes
         // holding rows (frow, frow + 8) reduces its four (row, column half) totals and scatters them over its lanes.
         float k4[4] = {0.f, 0.f, 0.f, 0.f};
@@ -525,9 +633,10 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
         continue;
       }
       // per warp: totals of its 16 rows per column group; the two warps of a quarter add theirs every kRedBatch candidates
-      float p[P4V_TILE_CG];
+      if constexpr (!kPair) {
 #pragma unroll
-      for (int k = 0; k < P4V_TILE_CG; ++k) p[k] = ph[k][0] + ph[k][1];
+        for (int k = 0; k < P4V_TILE_CG; ++k) p[k] = ph[k][0] + ph[k][1];
+      }
       const float tot = reduce8_over_warp(p, lane);
       float* const rbase = red + (size_t)(rb * 4 + quarter) * kRedBatch * 2 * P4V_TILE_CG;
       if ((lane & 3) == 0) rbase[(nb * 2 + (cw & 1)) * P4V_TILE_CG + (lane >> 2)] = tot;
@@ -590,13 +699,39 @@ int p4v_launch_sweep_tc(const SweepParams& p_in, const P4VJob* host_jobs, int nu
   p.n_stages = nst;
   const size_t smem = (size_t)nst * per_stage + (size_t)p.resident_bufs * res_bytes + p.cres_bytes + ((sizeof(SmemCtl) + 127) & ~size_t(127)) + (size_t)red_bytes + 256;
   P4V_REQUIRE(smem <= 227 * 1024, "sweep: shared-memory plan too large (%zu bytes)", smem);
-#define P4V_LAUNCH(I8, SG)                                                                             \
+  // Pair step: two candidate groups whose jobs i and i + n/2 multiply the same candidate column slab (same offsets and
+  // flags, one accumulator each) with two resident row parts, each half one accumulator chain.  The pair consumer holds
+  // a candidate's n/2 stages at once, so the ring must have one more.  P4V_NO_PAIR=1 keeps such steps on the
+  // multi-segment path (A/B comparison).
+  bool pair = false;
+  if (!single && p.out == nullptr && p.n_cand_groups == 2 && p.n_cand_jobs % 2 == 0 && p.n_cand_jobs / 2 + 1 <= nst &&
+      getenv("P4V_NO_PAIR") == nullptr) {
+    const int np = p.n_cand_jobs / 2;
+    const P4VJob* cj = host_jobs + p.n_fixed_jobs;
+    pair = true;
+    for (int i = 0; i < np; ++i) {
+      const P4VJob &a = cj[i], &b = cj[np + i];
+      const uint32_t need = P4V_JOB_CCAND | P4V_JOB_RRES;
+      pair = pair && a.c_off == b.c_off && a.kb == b.kb && p4v_job_nsub(a) == 1 && p4v_job_nsub(b) == 1 &&
+             a.flags == b.flags && (a.flags & (need | P4V_JOB_RCAND | P4V_JOB_CRES)) == need &&
+             ((a.flags & P4V_JOB_FIRST) != 0) == (i == 0) && ((a.flags & P4V_JOB_LAST) != 0) == (i + 1 == np);
+    }
+  }
+  const int mode = single ? kModeSingle : pair ? kModePair : kModeMulti;
+#define P4V_LAUNCH(I8, MODE)                                                                           \
   do {                                                                                                 \
-    P4V_CUDA_OK(cudaFuncSetAttribute(sweep_tc_kernel<I8, SG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    sweep_tc_kernel<I8, SG><<<grid, kThreads, smem, st>>>(p);                                          \
+    P4V_CUDA_OK(cudaFuncSetAttribute(sweep_tc_kernel<I8, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    sweep_tc_kernel<I8, MODE><<<grid, kThreads, smem, st>>>(p);                                        \
   } while (0)
-  if (p.is_int8) { if (single) P4V_LAUNCH(true, true); else P4V_LAUNCH(true, false); }
-  else           { if (single) P4V_LAUNCH(false, true); else P4V_LAUNCH(false, false); }
+#define P4V_LAUNCH_MODE(I8)                                                                            \
+  do {                                                                                                 \
+    if (mode == kModeSingle) P4V_LAUNCH(I8, kModeSingle);                                              \
+    else if (mode == kModePair) P4V_LAUNCH(I8, kModePair);                                             \
+    else P4V_LAUNCH(I8, kModeMulti);                                                                   \
+  } while (0)
+  if (p.is_int8) P4V_LAUNCH_MODE(true);
+  else           P4V_LAUNCH_MODE(false);
+#undef P4V_LAUNCH_MODE
 #undef P4V_LAUNCH
   P4V_CUDA_OK(cudaGetLastError());
   return 0;
