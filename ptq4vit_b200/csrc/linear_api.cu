@@ -136,9 +136,15 @@ struct LinPlan {
   // workspace offsets
   size_t o_factors, o_keys, o_dW0, o_dW, o_dX0, o_dX, o_gscale, o_scores, o_best, o_fix, o_candA, o_candB, o_jobs,
       o_metas, o_segsW, o_segsX, o_segsXc, o_commits, o_partial, o_Wcur, o_Xcur, o_Wcand, o_Xcand, total;
+  // int8 activation step of a bf16 layer (build_plan): K bytes of its images, its jobs and segment tables, the step (same
+  // groups and scale tables as xsteps[0], jobs in jobs8) and its buffers inside the bf16 candidate activation region
+  bool x8; int KB8;
+  std::vector<P4VJob> jobs8; std::vector<P4VSeg> segsW8, segsXc8;
+  Step xstep8;
+  size_t o_Xcand8, o_Wcur8, o_jobs8, o_segsW8, o_segsXc8;
 };
 
-void add_group(LinPlan& p, int r_off_bytes, int c_off_bytes, int kb, uint8_t src_flags, int group_idx, int& njobs) {
+void add_group(std::vector<P4VJob>& jobs, int r_off_bytes, int c_off_bytes, int kb, uint8_t src_flags, int group_idx, int& njobs) {
   for (int b = 0; b < kb; b += P4V_JOB_KB) {
     P4VJob j{};
     const int len = std::min(P4V_JOB_KB, kb - b);
@@ -147,7 +153,7 @@ void add_group(LinPlan& p, int r_off_bytes, int c_off_bytes, int kb, uint8_t src
     j.kb = (uint8_t)len;
     j.flags = src_flags | (b == 0 ? P4V_JOB_FIRST : 0) | (b + len >= kb ? P4V_JOB_LAST : 0);
     j.group = (uint8_t)group_idx;
-    p.jobs.push_back(j);
+    jobs.push_back(j);
     ++njobs;
   }
 }
@@ -167,10 +173,10 @@ void mark_resident(LinPlan& p, const Step& st) {
 
 // Merge runs of single-job accumulator groups whose K slabs are adjacent in BOTH operand images into one
 // stage load with several sub-accumulators (one bulk copy / one stage handshake for up to 128 bytes of K).
-void batch_jobs(LinPlan& p, int first, int& count) {
+void batch_jobs(std::vector<P4VJob>& jobs, int first, int& count) {
   std::vector<P4VJob> out;
   for (int j = 0; j < count; ++j) {
-    const P4VJob jb = p.jobs[first + j];
+    const P4VJob jb = jobs[first + j];
     const bool single = (jb.flags & P4V_JOB_FIRST) && (jb.flags & P4V_JOB_LAST) && !(jb.flags & (P4V_JOB_RRES | P4V_JOB_CCAND));
     if (single && !out.empty()) {
       P4VJob& prev = out.back();
@@ -185,12 +191,14 @@ void batch_jobs(LinPlan& p, int first, int& count) {
     }
     out.push_back(jb);
   }
-  std::copy(out.begin(), out.end(), p.jobs.begin() + first);
-  p.jobs.erase(p.jobs.begin() + first + out.size(), p.jobs.begin() + first + count);
+  std::copy(out.begin(), out.end(), jobs.begin() + first);
+  jobs.erase(jobs.begin() + first + out.size(), jobs.begin() + first + count);
   count = (int)out.size();
 }
 
-int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search) {
+// x8_ok: the caller passes the activations to every activation step (p4v_linear_calibrate), which the int8 activation
+// step needs to rebuild the bf16 current activation image after its pick.
+int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search, bool x8_ok = false) {
   P4V_REQUIRE(d != nullptr, "null desc");
   p.d = *d;
   p.M = d->rows; p.K = d->in_features; p.O = d->out_features;
@@ -224,7 +232,9 @@ int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search) {
   for (size_t i = 0; i + 1 < cuts.size(); ++i) min_len = std::min(min_len, cuts[i + 1] - cuts[i]);
   if (d->operand == P4V_OPERAND_INT8) p.i8 = true;
   else if (d->operand == P4V_OPERAND_BF16) p.i8 = false;
-  else p.i8 = min_len >= 64;     // short slabs are epilogue bound: integer-valued bf16 saves the int->float converts (measured)
+  // Automatic choice: short K segments (< 64 elements) take integer-valued bf16 for the weight steps, the residual and the
+  // quantised forward.  The activation step of such a layer may still run on int8 images (x8 below).
+  else p.i8 = min_len >= 64;
   p.ew = p.i8 ? 1 : 2;
   p.segs.clear();
   int off = 0;
@@ -267,7 +277,7 @@ int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search) {
   p.max_groups = 1;
   auto begin_step = [&](Step& st) { st = Step{}; st.job_off = (int)p.jobs.size(); st.commit_off = (int)p.commits.size(); };
   auto fixed_group = [&](Step& st, const BSeg& s, bool neg) {
-    add_group(p, neg ? s.xoff_n : s.xoff_p, s.woff, s.kb, 0, st.nfg, st.nfj);
+    add_group(p.jobs, neg ? s.xoff_n : s.xoff_p, s.woff, s.kb, 0, st.nfg, st.nfj);
     p.metas.push_back(GroupMeta{(short)s.h, (short)s.a, (short)(neg ? 1 : 0), 0});
     ++st.nfg;
   };
@@ -278,17 +288,17 @@ int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search) {
       for (auto& s : p.segs) if (s.h != h) { fixed_group(st, s, false); if (p.twin) fixed_group(st, s, true); }
       st.meta_cand = (int)p.metas.size();
       for (auto& s : p.segs) if (s.h == h) {
-        add_group(p, s.xoff_p, s.woff, s.kb, P4V_JOB_CCAND, st.ncg, st.ncj);
+        add_group(p.jobs, s.xoff_p, s.woff, s.kb, P4V_JOB_CCAND, st.ncg, st.ncj);
         p.metas.push_back(GroupMeta{(short)s.h, (short)s.a, 0, 0}); ++st.ncg;
         if (p.twin) {
-          add_group(p, s.xoff_n, s.woff, s.kb, P4V_JOB_CCAND, st.ncg, st.ncj);
+          add_group(p.jobs, s.xoff_n, s.woff, s.kb, P4V_JOB_CCAND, st.ncg, st.ncj);
           p.metas.push_back(GroupMeta{(short)s.h, (short)s.a, 1, 0}); ++st.ncg;
         }
         p.commits.push_back(CommitSeg{s.woff * P4V_TILE, s.woff * P4V_TILE, s.kb});
         st.commit_chunks += s.kb / 16; ++st.ncommit;
       }
       mark_resident(p, st);
-      batch_jobs(p, st.job_off, st.nfj);
+      batch_jobs(p.jobs, st.job_off, st.nfj);
       p.wsteps.push_back(st);
     }
     for (int a = 0; a < d->n_a; ++a) {
@@ -297,14 +307,14 @@ int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search) {
       for (auto& s : p.segs) { if (s.a != a) fixed_group(st, s, false); if (p.twin) fixed_group(st, s, true); }
       st.meta_cand = (int)p.metas.size();
       for (auto& s : p.segs) if (s.a == a) {
-        add_group(p, s.xcoff, s.woff, s.kb, P4V_JOB_RCAND, st.ncg, st.ncj);
+        add_group(p.jobs, s.xcoff, s.woff, s.kb, P4V_JOB_RCAND, st.ncg, st.ncj);
         p.metas.push_back(GroupMeta{(short)s.h, (short)s.a, 0, 0}); ++st.ncg;
         p.commits.push_back(CommitSeg{s.xcoff * P4V_TILE, s.xoff_p * P4V_TILE, s.kb});
         st.commit_chunks += s.kb / 16; ++st.ncommit;
       }
       {   // candidates change the row operand only: keep the tile's weight image resident when it fits
-        int ncj = st.ncj; batch_jobs(p, st.job_off + st.nfj, ncj); st.ncj = ncj;
-        batch_jobs(p, st.job_off, st.nfj);
+        int ncj = st.ncj; batch_jobs(p.jobs, st.job_off + st.nfj, ncj); st.ncj = ncj;
+        batch_jobs(p.jobs, st.job_off, st.nfj);
         if ((size_t)p.KB_W * P4V_TILE <= 100 * 1024 && getenv("P4V_NO_CRES") == nullptr)
           for (int j = 0; j < st.nfj + st.ncj; ++j) p.jobs[st.job_off + j].flags |= P4V_JOB_CRES;
       }
@@ -316,7 +326,7 @@ int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search) {
     st.meta_fix = (int)p.metas.size();
     for (auto& s : p.segs) { fixed_group(st, s, false); if (p.twin) fixed_group(st, s, true); }
     st.meta_cand = (int)p.metas.size();
-    batch_jobs(p, st.job_off, st.nfj);
+    batch_jobs(p.jobs, st.job_off, st.nfj);
     p.fwd = st;
   }
   auto check = [&](const Step& st) {
@@ -382,6 +392,42 @@ int build_plan(const p4v_linear_desc* d, LinPlan& p, bool with_search) {
       p.o_segsG = take((p.chunked ? 4 : 2) * sizeof(P4VSeg));   // chunked: a full chunk and the last one
     }
   }
+  // Activation step of a layer that chose bf16 automatically, when the step has no fixed groups (one activation chunk,
+  // not post-GELU): run it on int8 images.  The tile's int8 weight image (half the bf16 bytes) then stays resident in
+  // shared memory, only the candidate activation slab streams, and the tensor cores run at the int8 rate.  bf16 with
+  // fp32 accumulators and int8 with s32 accumulators form the same exact integer products (below 2^24), and the
+  // epilogue runs the same fp32 operations per group in the same order, so score tables and picks are bit-identical.
+  // The int8 candidate planes, an int8 copy of the current weight image and the step's job and segment tables take the
+  // place of the bf16 candidate activation planes, which only the activation steps read: the workspace does not grow.
+  // The weight steps, the residual sweep and the quantised forward keep the bf16 images.
+  p.x8 = false;
+  if (x8_ok && d->operand == P4V_OPERAND_AUTO && !p.i8 && d->kernel == P4V_KERNEL_TCGEN05 && p.xsteps.size() == 1 &&
+      p.xsteps[0].nfg == 0 && getenv("P4V_NO_CRES") == nullptr) {
+    p.jobs8.clear(); p.segsW8.clear(); p.segsXc8.clear();
+    Step& st = p.xstep8;
+    st = p.xsteps[0]; st.job_off = 0; st.nfj = 0; st.ncj = 0;
+    int off8 = 0;
+    for (size_t i = 0; i < p.segs.size(); ++i) {   // one candidate group per segment, in the order of the bf16 step
+      const int kb = (int)align_up((size_t)p.segs[i].klen, 32);
+      P4VSeg w = p.segsW[i], x = p.segsXc[i];
+      w.dst_off = x.dst_off = off8 * P4V_TILE;
+      p.segsW8.push_back(w); p.segsXc8.push_back(x);
+      add_group(p.jobs8, off8, off8, kb, P4V_JOB_RCAND, (int)i, st.ncj);
+      off8 += kb;
+    }
+    p.KB8 = off8;
+    batch_jobs(p.jobs8, 0, st.ncj);
+    for (auto& j : p.jobs8) j.flags |= P4V_JOB_CRES;
+    size_t o8 = p.o_Xcand;
+    auto take8 = [&](size_t bytes) { size_t r = o8; o8 = align_up(o8 + bytes, 256); return r; };
+    p.o_Xcand8 = take8((size_t)n_c * p.tiles_mc * P4V_TILE * p.KB8);
+    p.o_Wcur8 = take8((size_t)p.tiles_o * P4V_TILE * p.KB8);
+    p.o_jobs8 = take8(p.jobs8.size() * sizeof(P4VJob));
+    p.o_segsW8 = take8(p.segsW8.size() * sizeof(P4VSeg));
+    p.o_segsXc8 = take8(p.segsXc8.size() * sizeof(P4VSeg));
+    const size_t region_end = align_up(p.o_Xcand + (size_t)n_c * p.tiles_mc * P4V_TILE * p.KB_Xc, 256);
+    p.x8 = (size_t)p.KB8 * P4V_TILE <= 100 * 1024 && o8 <= region_end && st.ncj <= P4V_MAX_JOBS;
+  }
   p.total = o;
   return 0;
 }
@@ -397,6 +443,11 @@ int upload_tables(const LinPlan& p, void* ws, cudaStream_t st) {
   P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segsXc), p.segsXc.data(), p.segsXc.size() * sizeof(P4VSeg), cudaMemcpyHostToDevice, st));
   if (!p.commits.empty())
     P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_commits), p.commits.data(), p.commits.size() * sizeof(CommitSeg), cudaMemcpyHostToDevice, st));
+  if (p.x8) {
+    P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_jobs8), p.jobs8.data(), p.jobs8.size() * sizeof(P4VJob), cudaMemcpyHostToDevice, st));
+    P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segsW8), p.segsW8.data(), p.segsW8.size() * sizeof(P4VSeg), cudaMemcpyHostToDevice, st));
+    P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segsXc8), p.segsXc8.data(), p.segsXc8.size() * sizeof(P4VSeg), cudaMemcpyHostToDevice, st));
+  }
   if (p.gram) {
     const int n_last = p.M - (p4v_cdiv(p.M, p.chunk_rows) - 1) * p.chunk_rows;
     const int nr[2] = {p.chunk_rows, n_last};
@@ -410,16 +461,17 @@ int upload_tables(const LinPlan& p, void* ws, cudaStream_t st) {
   return 0;
 }
 
-int quant_W(const LinPlan& p, void* ws, const float* W, const float* delta, bool cand, cudaStream_t st) {
+// x8: the int8 current weight image of the int8 activation step (cand must be false)
+int quant_W(const LinPlan& p, void* ws, const float* W, const float* delta, bool cand, cudaStream_t st, bool x8 = false) {
   QuantImageArgs q{};
   q.src = W; q.ld = p.K; q.prob_stride = 0; q.src_transposed = 0;
   q.P = 1; q.rows = p.O; q.tiles = p.tiles_o;
-  q.dst = at<uint8_t>(ws, cand ? p.o_Wcand : p.o_Wcur);
-  q.tile_bytes = (unsigned long long)P4V_TILE * p.KB_W; q.plane_stride = q.tile_bytes * p.tiles_o;
+  q.dst = at<uint8_t>(ws, x8 ? p.o_Wcur8 : cand ? p.o_Wcand : p.o_Wcur);
+  q.tile_bytes = (unsigned long long)P4V_TILE * (x8 ? p.KB8 : p.KB_W); q.plane_stride = q.tile_bytes * p.tiles_o;
   q.n_planes = cand ? p.d.eq_n : 1;
   q.factors = cand ? at<float>(ws, p.o_factors) : nullptr;
   q.delta = delta; q.rows_per_block = p.crb_rows; q.d_stride = p.d.n_H; q.d_mod = 1;
-  q.segs = at<P4VSeg>(ws, p.o_segsW); q.nseg = (int)p.segsW.size(); q.is_int8 = p.i8;
+  q.segs = at<P4VSeg>(ws, x8 ? p.o_segsW8 : p.o_segsW); q.nseg = (int)p.segsW.size(); q.is_int8 = x8 || p.i8;
   return p4v_quant_image(q, st);
 }
 
@@ -427,17 +479,19 @@ int quant_W(const LinPlan& p, void* ws, const float* W, const float* delta, bool
 struct Rows { int r0, n; };
 Rows all_rows(const LinPlan& p) { return Rows{0, p.M}; }
 
+// The candidate planes are int8 when the activation step runs on int8 images (p.x8)
 int quant_X(const LinPlan& p, void* ws, const float* x, const float* delta, bool cand, Rows r, cudaStream_t st) {
+  const bool x8 = cand && p.x8;
   QuantImageArgs q{};
   q.src = x + (size_t)r.r0 * p.K; q.ld = p.K; q.prob_stride = 0; q.src_transposed = 0;
   q.P = 1; q.rows = r.n; q.tiles = p4v_cdiv(r.n, P4V_TILE);
-  q.dst = at<uint8_t>(ws, cand ? p.o_Xcand : p.o_Xcur);
-  q.tile_bytes = (unsigned long long)P4V_TILE * (cand ? p.KB_Xc : p.KB_X); q.plane_stride = q.tile_bytes * q.tiles;
+  q.dst = at<uint8_t>(ws, x8 ? p.o_Xcand8 : cand ? p.o_Xcand : p.o_Xcur);
+  q.tile_bytes = (unsigned long long)P4V_TILE * (x8 ? p.KB8 : cand ? p.KB_Xc : p.KB_X); q.plane_stride = q.tile_bytes * q.tiles;
   q.n_planes = cand ? p.d.eq_n : 1;
   q.factors = cand ? at<float>(ws, p.o_factors) : nullptr;
   q.delta = delta; q.rows_per_block = p.M + P4V_TILE; q.d_stride = 0; q.d_mod = 1;   // single row block: any row range
-  q.segs = at<P4VSeg>(ws, cand ? p.o_segsXc : p.o_segsX); q.nseg = (int)(cand ? p.segsXc.size() : p.segsX.size());
-  q.is_int8 = p.i8;
+  q.segs = at<P4VSeg>(ws, x8 ? p.o_segsXc8 : cand ? p.o_segsXc : p.o_segsX); q.nseg = (int)(cand ? p.segsXc.size() : p.segsX.size());
+  q.is_int8 = x8 || p.i8;
   return p4v_quant_image(q, st);
 }
 
@@ -461,6 +515,16 @@ void fill_sweep(const LinPlan& p, void* ws, const Step& s, SweepParams& sp, Rows
   sp.is_int8 = p.i8;
 }
 void fill_sweep(const LinPlan& p, void* ws, const Step& s, SweepParams& sp) { fill_sweep(p, ws, s, sp, all_rows(p)); }
+
+// The int8 activation step: int8 candidate activation planes against the resident int8 current weight image
+void fill_sweep_x8(const LinPlan& p, void* ws, SweepParams& sp, Rows r) {
+  fill_sweep(p, ws, p.xstep8, sp, r);
+  sp.R_cand = at<uint8_t>(ws, p.o_Xcand8); sp.C_cur = at<uint8_t>(ws, p.o_Wcur8);
+  sp.R_cand_tile_bytes = sp.C_tile_bytes = (unsigned long long)P4V_TILE * p.KB8;
+  sp.R_cand_stride = sp.R_cand_tile_bytes * sp.tiles_m;
+  sp.jobs = at<P4VJob>(ws, p.o_jobs8);
+  sp.is_int8 = 1;
+}
 
 int run_sweep(const LinPlan& p, const Step& s, const SweepParams& sp, cudaStream_t st) {
   return p4v_run_sweep(sp, p.jobs.data() + s.job_off, p.d.kernel, st);
@@ -488,12 +552,16 @@ struct StepRef { bool is_w; int idx; };
 // One search step: [scale tables] -> sweep -> reduce -> select (+ tables of the next step) -> commit.
 // Chunked: per chunk of rows, the chunk's X images (current; X step: candidates) -> sweep -> reduce into the fp64 table;
 // select after the last chunk; only the weight image is committed (the X images are rebuilt from the step sizes).
-int search_step(const LinPlan& p, void* ws, StepRef cur, const StepRef* next, bool tables_ready, const float* x,
+// An int8 activation step (p.x8) first quantises the current weights to int8 and, unchunked, rebuilds the bf16 current
+// activation image from the chosen step size instead of committing a candidate slab.
+int search_step(const LinPlan& p, void* ws, StepRef cur, const StepRef* next, bool tables_ready, const float* x, const float* W,
                 const float* bias, const float* y, const float* g, float* score_log, cudaStream_t st) {
   const bool is_w = cur.is_w; const int idx = cur.idx;
+  const bool x8 = !is_w && p.x8;
   const Step& s = is_w ? p.wsteps[idx] : p.xsteps[idx];
   int rc;
   if (!tables_ready && (rc = tables_for(p, ws, s, is_w ? 0 : 1, idx, st))) return rc;
+  if (x8 && (rc = quant_W(p, ws, W, at<float>(ws, p.o_dW), false, st, true))) return rc;
   SweepParams sp;
   for (int r0 = 0; r0 < p.M; r0 += p.chunk_rows) {
     const Rows r{r0, std::min(p.chunk_rows, p.M - r0)};
@@ -501,10 +569,11 @@ int search_step(const LinPlan& p, void* ws, StepRef cur, const StepRef* next, bo
       if ((rc = quant_X(p, ws, x, at<float>(ws, p.o_dX), false, r, st))) return rc;
       if (!is_w && (rc = quant_X(p, ws, x, at<float>(ws, p.o_dX0), true, r, st))) return rc;
     }
-    fill_sweep(p, ws, s, sp, r);
+    if (x8) fill_sweep_x8(p, ws, sp, r);
+    else fill_sweep(p, ws, s, sp, r);
     sp.Y = y + (size_t)r0 * p.O; sp.Gr = g + (size_t)r0 * p.O; sp.bias = p.d.has_bias ? bias : nullptr;
     sp.order = is_w ? 0 : 1;
-    if ((rc = run_sweep(p, s, sp, st))) return rc;
+    if ((rc = x8 ? p4v_run_sweep(sp, p.jobs8.data(), p.d.kernel, st) : run_sweep(p, s, sp, st))) return rc;
     ReduceArgs ra{};
     ra.partial = sp.partial; ra.n_cand = p.d.eq_n; ra.P = 1; ra.tiles_m = sp.tiles_m; ra.tiles_n = p.tiles_o; ra.order = sp.order;
     ra.mode = P4V_SG_COLUMN; ra.n_keys = p.nsg; ra.sums = at<double>(ws, p.o_scores); ra.accumulate = r0 > 0;
@@ -523,6 +592,7 @@ int search_step(const LinPlan& p, void* ws, StepRef cur, const StepRef* next, bo
   if (next) f.next = tables_args(p, ws, next->is_w ? p.wsteps[next->idx] : p.xsteps[next->idx], next->is_w ? 0 : 1, next->idx);
   if ((rc = p4v_select_step(f, st))) return rc;
   if (p.chunked && !is_w) return 0;
+  if (x8) return quant_X(p, ws, x, at<float>(ws, p.o_dX), false, all_rows(p), st);
   CommitArgs c{};
   c.best = f.best; c.n_groups = n_groups;
   c.cand = at<uint8_t>(ws, is_w ? p.o_Wcand : p.o_Xcand);
@@ -698,7 +768,7 @@ extern "C" int p4v_linear_search_w(const p4v_linear_desc* d, const float* bias, 
   P4V_REQUIRE(0 <= h_begin && h_begin <= h_end && h_end <= d->n_H, "linear_search_w: bad block range");
   for (int h = h_begin; h < h_end; ++h) {
     StepRef nx{true, h + 1};
-    if ((rc = search_step(p, workspace, StepRef{true, h}, h + 1 < h_end ? &nx : nullptr, h > h_begin, nullptr, bias, raw_out, raw_grad,
+    if ((rc = search_step(p, workspace, StepRef{true, h}, h + 1 < h_end ? &nx : nullptr, h > h_begin, nullptr, nullptr, bias, raw_out, raw_grad,
                           score_log, (cudaStream_t)stream))) return rc;
     if (score_log) score_log += (size_t)d->eq_n * d->n_V;
   }
@@ -714,7 +784,7 @@ extern "C" int p4v_linear_search_a(const p4v_linear_desc* d, const float* bias, 
   P4V_REQUIRE(0 <= a_begin && a_begin <= a_end && a_end <= d->n_a, "linear_search_a: bad chunk range");
   for (int a = a_begin; a < a_end; ++a) {
     StepRef nx{false, a + 1};
-    if ((rc = search_step(p, workspace, StepRef{false, a}, a + 1 < a_end ? &nx : nullptr, a > a_begin, nullptr, bias, raw_out, raw_grad,
+    if ((rc = search_step(p, workspace, StepRef{false, a}, a + 1 < a_end ? &nx : nullptr, a > a_begin, nullptr, nullptr, bias, raw_out, raw_grad,
                           score_log, (cudaStream_t)stream))) return rc;
     if (score_log) score_log += d->eq_n;
   }
@@ -733,7 +803,7 @@ extern "C" int p4v_linear_intervals(const p4v_linear_desc* d, void* workspace, f
 extern "C" int p4v_linear_calibrate(const p4v_linear_desc* d, const float* x, const float* weight, const float* bias,
                                     const float* raw_out, const float* raw_grad, void* workspace, size_t workspace_bytes,
                                     float* w_interval, float* a_interval, float* score_log, void* stream) {
-  LinPlan p; int rc = build_plan(d, p, true);
+  LinPlan p; int rc = build_plan(d, p, true, true);
   if (rc) return rc;
   P4V_REQUIRE(x && weight && raw_out && raw_grad && workspace && w_interval && a_interval, "linear_calibrate: null pointer");
   P4V_REQUIRE(!d->has_bias || bias, "linear_calibrate: has_bias set but bias is null");
@@ -746,7 +816,7 @@ extern "C" int p4v_linear_calibrate(const p4v_linear_desc* d, const float* x, co
       if (score_log) score_log += (size_t)d->n_H * d->eq_n * d->n_V;
       for (int a = 0; a < d->n_a; ++a) {
         StepRef nx{false, a + 1};
-        if ((rc = search_step(p, workspace, StepRef{false, a}, a + 1 < d->n_a ? &nx : nullptr, a > 0, x, bias, raw_out, raw_grad,
+        if ((rc = search_step(p, workspace, StepRef{false, a}, a + 1 < d->n_a ? &nx : nullptr, a > 0, x, weight, bias, raw_out, raw_grad,
                               score_log, st))) return rc;
         if (score_log) score_log += d->eq_n;
       }
@@ -758,7 +828,7 @@ extern "C" int p4v_linear_calibrate(const p4v_linear_desc* d, const float* x, co
       for (int a = 0; a < d->n_a; ++a) seq.push_back(StepRef{false, a});
     }
     for (size_t i = 0; i < seq.size(); ++i) {
-      if ((rc = search_step(p, workspace, seq[i], i + 1 < seq.size() ? &seq[i + 1] : nullptr, i > 0, x, bias, raw_out, raw_grad,
+      if ((rc = search_step(p, workspace, seq[i], i + 1 < seq.size() ? &seq[i + 1] : nullptr, i > 0, x, weight, bias, raw_out, raw_grad,
                             score_log, st))) return rc;
       if (score_log) score_log += seq[i].is_w ? (size_t)d->eq_n * d->n_V : (size_t)d->eq_n;
     }
