@@ -117,3 +117,12 @@ extern "C" void p4v_set_error(const char* fmt, ...);
 // ---- kernel launchers shared between translation units ----------------------
 int p4v_launch_sweep_tc(const SweepParams& p, const P4VJob* host_jobs, int num_sms, cudaStream_t st);
 int p4v_launch_sweep_simt(const SweepParams& p, cudaStream_t st);
+
+// ---- library runtime (runtime.cu) -------------------------------------------
+void p4v_count_launch();                   // every kernel launch, for p4v_launch_count
+int p4v_num_sms();
+bool p4v_prof_on();                        // live kernel timing of the tensor-core launches (p4v_profile_enable)
+void p4v_prof_begin(cudaStream_t st, cudaEvent_t* e0);
+void p4v_prof_end(cudaStream_t st, cudaEvent_t e0, int kind, double ops);
+// one slab sweep on the kernel `kernel` selects (P4V_KERNEL_*): counted and, while timing is on, timed
+int p4v_run_sweep(const SweepParams& sp, const P4VJob* host_jobs, int kernel, cudaStream_t st);

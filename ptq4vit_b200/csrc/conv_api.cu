@@ -10,26 +10,17 @@
 // per-ROW scale; the sweep's scales are per column group, so delta0[o] is folded into the targets once:
 //     (g * (y - b - f*d0*D))^2 = (g*d0 * ((y - b)/d0 - f*D))^2
 // and the candidate scale is the plain factor f_c.  Scores are kept per row (SweepParams::row_keys).
-#include <algorithm>
-#include <vector>
-
 #include "../../include/ptq4vit_b200.h"
-#include "prep.cuh"
-
-void p4v_count_launch();
-int p4v_run_sweep(const SweepParams& sp, const P4VJob* host_jobs, int kernel, cudaStream_t st);
+#include "plan.cuh"
 
 namespace {
-
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-template <class T> T* at(void* ws, size_t off) { return reinterpret_cast<T*>(static_cast<uint8_t*>(ws) + off); }
 
 struct ConvPlan {
   p4v_conv_desc d;
   int P, O, K, L, tiles_o, tiles_l, kb, w_qmax;
-  std::vector<P4VJob> jobs; std::vector<P4VSeg> segW, segC; std::vector<float> factors;
-  size_t o_factors, o_keys, o_d0, o_d, o_gscale, o_ones, o_scores, o_best, o_candA, o_candB, o_fix, o_jobs, o_segW, o_segC,
-      o_partial, o_Wcand, o_Cimg, o_Y, o_G, total;
+  Table<P4VJob> jobs; Table<P4VSeg> segW, segC; Table<float> factors;
+  Image Wcand, Cimg;   // candidate planes of the integer kernel; the three-term split of the im2col matrix
+  size_t o_keys, o_d0, o_d, o_gscale, o_ones, o_scores, o_best, o_candA, o_candB, o_fix, o_partial, o_Y, o_G, total;
 };
 
 int build_plan(const p4v_conv_desc* d, ConvPlan& p) {
@@ -44,34 +35,24 @@ int build_plan(const p4v_conv_desc* d, ConvPlan& p) {
   p.tiles_o = p4v_cdiv(p.O, P4V_TILE); p.tiles_l = p4v_cdiv(p.L, P4V_TILE);
   p.kb = (int)align_up((size_t)p.K * 2, 32);                    // bf16 row bytes of one term
   P4V_REQUIRE(3 * (p.kb / 32) <= P4V_MAX_JOBS * 4 && 3 * p4v_cdiv(p.kb, P4V_JOB_KB) <= P4V_MAX_JOBS, "conv: kernel volume too large");
-  p.segW = {P4VSeg{0, p.K, 0, 0, 0.f, (float)-p.w_qmax, (float)(p.w_qmax - 1), 0, 0.f, 0, 0}};
-  p.segC.clear();
-  for (int t = 0; t < 3; ++t) p.segC.push_back(P4VSeg{0, p.K, t * p.kb * P4V_TILE, 0, 0.f, 0.f, 0.f, 0, 0.f, t + 1, 0});
-  p.factors.resize(d->eq_n + 1);
-  for (int i = 0; i <= d->eq_n; ++i) p.factors[i] = (float)(d->eq_alpha + i * (d->eq_beta - d->eq_alpha) / d->eq_n);
-  p.jobs.clear();
-  for (int t = 0; t < 3; ++t)
-    for (int b = 0; b < p.kb; b += P4V_JOB_KB) {
-      P4VJob j{};
-      const int len = std::min(P4V_JOB_KB, p.kb - b);
-      j.r_off = (uint32_t)b * P4V_TILE; j.c_off = (uint32_t)(t * p.kb + b) * P4V_TILE; j.kb = (uint8_t)len;
-      j.flags = P4V_JOB_RCAND | ((t == 0 && b == 0) ? P4V_JOB_FIRST : 0) | ((t == 2 && b + len >= p.kb) ? P4V_JOB_LAST : 0);
-      j.group = 0;
-      p.jobs.push_back(j);
-    }
-  size_t o = 0;
-  auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+  p.segW.host = {P4VSeg{0, p.K, 0, 0, 0.f, (float)-p.w_qmax, (float)(p.w_qmax - 1), 0, 0.f, 0, 0}};
+  for (int t = 0; t < 3; ++t) p.segC.host.push_back(P4VSeg{0, p.K, t * p.kb * P4V_TILE, 0, 0.f, 0.f, 0.f, 0, 0.f, t + 1, 0});
+  p.factors.host = cand_factors(d->eq_n, d->eq_alpha, d->eq_beta);
+  int n_jobs = 0;   // one accumulator: the three term products chained
+  for (int t = 0; t < 3; ++t) add_group(p.jobs.host, 0, t * p.kb, p.kb, P4V_JOB_RCAND, 0, t == 0, t == 2, n_jobs);
+  p.Wcand = Image{0, p.kb, p.tiles_o, 1, d->eq_n, false}; p.Cimg = Image{0, 3 * p.kb, p.tiles_l, p.P, 1, false};
+  Carver c{0};
   const int n_c = d->eq_n;
-  p.o_factors = take((n_c + 1) * 4); p.o_keys = take((p.O + 1) * 4);
-  p.o_d0 = take(p.O * 4); p.o_d = take(p.O * 4); p.o_gscale = take(4); p.o_ones = take(4);
-  p.o_scores = take((size_t)n_c * p.O * 8); p.o_best = take(p.O * 4);
-  p.o_candA = take((size_t)n_c * 4); p.o_candB = take(4); p.o_fix = take(4);
-  p.o_jobs = take(p.jobs.size() * sizeof(P4VJob)); p.o_segW = take(sizeof(P4VSeg)); p.o_segC = take(3 * sizeof(P4VSeg));
-  p.o_partial = take((size_t)p.P * p.tiles_o * p.tiles_l * n_c * 256 * 4);
-  p.o_Wcand = take((size_t)n_c * p.tiles_o * P4V_TILE * p.kb);
-  p.o_Cimg = take((size_t)p.P * p.tiles_l * P4V_TILE * 3 * p.kb);
-  p.o_Y = take((size_t)p.P * p.O * p.L * 4); p.o_G = take((size_t)p.P * p.O * p.L * 4);
-  p.total = o;
+  p.factors.off = c.take(p.factors.bytes()); p.o_keys = c.take((p.O + 1) * 4);
+  p.o_d0 = c.take(p.O * 4); p.o_d = c.take(p.O * 4); p.o_gscale = c.take(4); p.o_ones = c.take(4);
+  p.o_scores = c.take((size_t)n_c * p.O * 8); p.o_best = c.take(p.O * 4);
+  p.o_candA = c.take((size_t)n_c * 4); p.o_candB = c.take(4); p.o_fix = c.take(4);
+  p.jobs.off = c.take(p.jobs.bytes()); p.segW.off = c.take(p.segW.bytes()); p.segC.off = c.take(p.segC.bytes());
+  p.o_partial = c.take((size_t)p.P * p.tiles_o * p.tiles_l * n_c * 256 * 4);
+  p.Wcand.off = c.take(p.Wcand.bytes());
+  p.Cimg.off = c.take(p.Cimg.bytes());
+  p.o_Y = c.take((size_t)p.P * p.O * p.L * 4); p.o_G = c.take((size_t)p.P * p.O * p.L * 4);
+  p.total = c.end;
   return 0;
 }
 
@@ -128,10 +109,8 @@ extern "C" int p4v_conv_calibrate(const p4v_conv_desc* d, const float* cols, con
   P4V_REQUIRE(!d->has_bias || bias, "conv_calibrate: has_bias set but bias is null");
   P4V_REQUIRE(workspace_bytes >= p.total, "conv_calibrate: workspace too small (%zu < %zu)", workspace_bytes, p.total);
   cudaStream_t st = (cudaStream_t)stream;
-  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_factors), p.factors.data(), p.factors.size() * 4, cudaMemcpyHostToDevice, st));
-  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_jobs), p.jobs.data(), p.jobs.size() * sizeof(P4VJob), cudaMemcpyHostToDevice, st));
-  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segW), p.segW.data(), sizeof(P4VSeg), cudaMemcpyHostToDevice, st));
-  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segC), p.segC.data(), 3 * sizeof(P4VSeg), cudaMemcpyHostToDevice, st));
+  if ((rc = p.factors.upload(ws, st)) || (rc = p.jobs.upload(ws, st)) || (rc = p.segW.upload(ws, st)) ||
+      (rc = p.segC.upload(ws, st))) return rc;
   // min-max step size per output channel (conv.py:487) and the gradient scale
   int* keys = at<int>(ws, p.o_keys);
   if ((rc = p4v_keys_reset(keys, p.O + 1, st))) return rc;
@@ -139,7 +118,7 @@ extern "C" int p4v_conv_calibrate(const p4v_conv_desc* d, const float* cols, con
   if ((rc = p4v_group_absmax(raw_grad, (long long)p.P * p.O * p.L, 1, 1, keys + p.O, st))) return rc;
   if ((rc = p4v_keys_to_delta(keys, p.O, (float)p.w_qmax - 0.5f, at<float>(ws, p.o_d0), at<float>(ws, p.o_d), st))) return rc;
   if ((rc = p4v_make_gscale(keys + p.O, at<float>(ws, p.o_gscale), st))) return rc;
-  conv_fill_kernel<<<p4v_cdiv(d->eq_n, 128), 128, 0, st>>>(at<float>(ws, p.o_candA), at<float>(ws, p.o_factors), d->eq_n, at<float>(ws, p.o_candB));
+  conv_fill_kernel<<<p4v_cdiv(d->eq_n, 128), 128, 0, st>>>(at<float>(ws, p.o_candA), p.factors.dev(ws), d->eq_n, at<float>(ws, p.o_candB));
   p4v_count_launch();
   const long long n = (long long)p.P * p.O * p.L;
   conv_prescale_kernel<<<132 * 8, 256, 0, st>>>(raw_out, raw_grad, d->has_bias ? bias : nullptr, at<float>(ws, p.o_d0), p.O, p.L, n,
@@ -148,44 +127,41 @@ extern "C" int p4v_conv_calibrate(const p4v_conv_desc* d, const float* cols, con
   P4V_CUDA_OK(cudaGetLastError());
   {   // candidate planes of the integer kernel: rows = channels, one step size per row
     QuantImageArgs q{};
-    q.src = weight; q.ld = p.K; q.prob_stride = 0; q.src_transposed = 0; q.P = 1; q.rows = p.O; q.tiles = p.tiles_o;
-    q.dst = at<uint8_t>(ws, p.o_Wcand); q.tile_bytes = (unsigned long long)P4V_TILE * p.kb; q.plane_stride = q.tile_bytes * p.tiles_o;
-    q.n_planes = d->eq_n; q.factors = at<float>(ws, p.o_factors); q.delta = at<float>(ws, p.o_d0);
-    q.rows_per_block = 1; q.d_stride = 1; q.d_mod = 1; q.segs = at<P4VSeg>(ws, p.o_segW); q.nseg = 1; q.is_int8 = 0;
+    p.Wcand.fill(q, ws);
+    q.src = weight; q.ld = p.K; q.prob_stride = 0; q.src_transposed = 0; q.rows = p.O;
+    q.factors = p.factors.dev(ws); q.delta = at<float>(ws, p.o_d0);
+    q.rows_per_block = 1; q.d_stride = 1; q.d_mod = 1; q.segs = p.segW.dev(ws); q.nseg = 1;
     if ((rc = p4v_quant_image(q, st))) return rc;
   }
   {   // exact three-term bf16 split of the FP32 im2col matrix: rows = output positions
     QuantImageArgs q{};
-    q.src = cols; q.ld = p.K; q.prob_stride = (long long)p.L * p.K; q.src_transposed = 0; q.P = p.P; q.rows = p.L; q.tiles = p.tiles_l;
-    q.dst = at<uint8_t>(ws, p.o_Cimg); q.tile_bytes = (unsigned long long)P4V_TILE * 3 * p.kb; q.plane_stride = 0;
-    q.n_planes = 1; q.factors = nullptr; q.delta = at<float>(ws, p.o_d0); q.rows_per_block = 0; q.d_stride = 0; q.d_mod = 1;
-    q.segs = at<P4VSeg>(ws, p.o_segC); q.nseg = 3; q.is_int8 = 0;
+    p.Cimg.fill(q, ws);
+    q.src = cols; q.ld = p.K; q.prob_stride = (long long)p.L * p.K; q.src_transposed = 0; q.rows = p.L;
+    q.factors = nullptr; q.delta = at<float>(ws, p.o_d0); q.rows_per_block = 0; q.d_stride = 0; q.d_mod = 1;
+    q.segs = p.segC.dev(ws); q.nseg = 3;
     if ((rc = p4v_quant_image(q, st))) return rc;
   }
   SweepParams sp{};
-  sp.R_cur = sp.R_cand = at<uint8_t>(ws, p.o_Wcand); sp.C_cur = sp.C_cand = at<uint8_t>(ws, p.o_Cimg);
-  sp.R_tile_bytes = sp.R_cand_tile_bytes = (unsigned long long)P4V_TILE * p.kb;
-  sp.C_tile_bytes = sp.C_cand_tile_bytes = (unsigned long long)P4V_TILE * 3 * p.kb;
-  sp.R_cand_stride = sp.R_cand_tile_bytes * p.tiles_o; sp.C_cand_stride = 0;
+  fill_images(sp, ws, p.Wcand, p.Wcand, p.Cimg, p.Cimg);
   sp.R_shared = 1;                                          // the kernel planes do not depend on the image
   sp.P = p.P; sp.M = p.O; sp.N = p.L; sp.tiles_m = p.tiles_o; sp.tiles_n = p.tiles_l;
   sp.Y = at<float>(ws, p.o_Y); sp.Gr = at<float>(ws, p.o_G); sp.bias = nullptr;
   sp.ld = p.L; sp.prob_stride = (long long)p.O * p.L;
   sp.gscale = at<float>(ws, p.o_gscale);
-  sp.jobs = at<P4VJob>(ws, p.o_jobs);
-  sp.n_fixed_jobs = 0; sp.n_cand_jobs = (int)p.jobs.size(); sp.n_fixed_groups = 0; sp.n_cand_groups = 1;
+  sp.jobs = p.jobs.dev(ws);
+  sp.n_fixed_jobs = 0; sp.n_cand_jobs = (int)p.jobs.host.size(); sp.n_fixed_groups = 0; sp.n_cand_groups = 1;
   sp.fix_scale = at<float>(ws, p.o_fix); sp.candA = at<float>(ws, p.o_candA); sp.candB = at<float>(ws, p.o_candB);
   sp.nsg = 1; sp.sg_mode = P4V_SG_PROBLEM;                  // one scale group: the candidate factor
-  sp.n_cand = d->eq_n; sp.partial = at<float>(ws, p.o_partial); sp.is_int8 = 0; sp.order = 0;
+  sp.n_cand = d->eq_n; sp.partial = at<float>(ws, p.o_partial); sp.order = 0;
   sp.row_keys = 1;
-  if ((rc = p4v_run_sweep(sp, p.jobs.data(), d->kernel, st))) return rc;
+  if ((rc = p4v_run_sweep(sp, p.jobs.host.data(), d->kernel, st))) return rc;
   conv_reduce_kernel<<<p4v_cdiv(d->eq_n * p.O, 256), 256, 0, st>>>(sp.partial, p.P, p.tiles_o, p.tiles_l, d->eq_n, p.O, at<double>(ws, p.o_scores));
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   SelectArgs f{};
   f.sums = at<double>(ws, p.o_scores); f.n_cand = d->eq_n; f.n_keys = p.O; f.n_groups = p.O; f.keys_per_group = 1;
   f.inv_count = 1.0 / (double)p.L;                          // mean over the output positions, sum over the images (conv.py:548-549)
-  f.gscale = at<float>(ws, p.o_gscale); f.factors = at<float>(ws, p.o_factors);
+  f.gscale = at<float>(ws, p.o_gscale); f.factors = p.factors.dev(ws);
   f.d0 = at<float>(ws, p.o_d0); f.d = at<float>(ws, p.o_d); f.d_stride = 1; f.d_col = 0;
   f.best = at<int>(ws, p.o_best); f.score_log = score_log; f.has_next = 0;
   if ((rc = p4v_select_step(f, st))) return rc;

@@ -15,12 +15,6 @@
 #include "gram.cuh"
 #include <cstdio>
 
-void p4v_count_launch();
-int p4v_num_sms();
-bool p4v_prof_on();
-void p4v_prof_begin(cudaStream_t st, cudaEvent_t* e0);
-void p4v_prof_end(cudaStream_t st, cudaEvent_t e0, int kind, double ops);
-
 namespace {
 
 constexpr int kThreads = 128 + 256;

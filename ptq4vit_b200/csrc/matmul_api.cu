@@ -1,23 +1,24 @@
 // C-ABI for the head-wise MatMul scale-factor search (PTQSLBatchingQuantMatMul and the
 // split-of-softmax variant).  Problem p = image * heads + head; the row operand is A[p]
 // (S1 x S2), the column operand is B[p]^T (S3 x S2); one K segment (n_V = n_H = 1).
-#include <algorithm>
-#include <vector>
-
 #include "../../include/ptq4vit_b200.h"
-#include "prep.cuh"
-
-void p4v_count_launch();
-int p4v_run_sweep(const SweepParams& sp, const P4VJob* host_jobs, int kernel, cudaStream_t st);
+#include "plan.cuh"
 
 namespace {
 
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-template <class T> T* at(void* ws, size_t off) { return reinterpret_cast<T*>(static_cast<uint8_t*>(ws) + off); }
+// An operand image and how it is built: from A (rows S1) or from B (rows S3, read transposed), with the current step
+// sizes (cur) or the initial ones, the candidate factors (none: one plane of the step sizes) and its segment table
+struct Operand { Image im; bool B, cur; const Table<float>* factors; const Table<P4VSeg>* segs; };
 
-struct MStep { int job_off, nfj, ncj, nfg, ncg, meta_fix, meta_cand; };
+struct MStep {
+  int job_off, nfj, ncj, nfg, ncg, meta_fix, meta_cand;
+  int order, n_cand; unsigned long long noA_mask;   // sweep order, candidates, candidate groups that ignore candA
+  const Image *Rcur, *Rcand, *Ccur, *Ccand;         // the images the sweep reads: rows = A, columns = B^T
+};
 
 struct MMPlan {
+  MMPlan() = default;
+  MMPlan(const MMPlan&) = delete;                   // the steps and operands point at the plan's images and tables
   p4v_matmul_desc d;
   bool i8, sos;
   int ew, P, H, S1, S2, S3, tiles_m, tiles_n, A_qmax, B_qmax;
@@ -25,28 +26,16 @@ struct MMPlan {
   int Pc;
   int kb;        // padded K bytes of one part in the search operand type
   int kb16;      // padded K bytes in bf16 (split-search images)
-  int KB_A, KB_B;            // row bytes of Acur / Bcur  (sos: Acur = [hi|lo])
-  int KB_As, KB_Bs;          // split search: Acand = [hi|lo] bf16, Bsplit = [b1|b2|b3] bf16
-  std::vector<P4VJob> jobs; std::vector<GroupMeta> metas;
-  std::vector<P4VSeg> segA, segB, segAs, segBs;
+  Table<P4VJob> jobs; Table<GroupMeta> metas;
+  Table<P4VSeg> segA, segB, segAs, segBs;
+  Table<float> factors, split_factors;
+  // Acur = [hi|lo] for sos; split search: Ascand = [hi|lo] bf16 candidates, Bsplit = [b1|b2|b3] exact bf16 split of B
+  Operand Acur, Acand, Bcur, Bcand, Ascand, Bsplit;
   MStep stepA, stepB, stepS, fwd;
-  std::vector<float> factors, split_factors;
   int n_split;
-  size_t o_factors, o_sfactors, o_keys, o_dA0, o_dA, o_dB0, o_dB, o_ones, o_aux, o_split, o_gscale, o_scores, o_best,
-      o_fix, o_candA, o_candB, o_jobs, o_metas, o_segA, o_segB, o_segAs, o_segBs, o_partial, o_Acur, o_Bcur, o_Acand,
-      o_Bcand, o_Ascand, o_Bsplit, total;
+  size_t o_keys, o_dA0, o_dA, o_dB0, o_dB, o_ones, o_aux, o_split, o_gscale, o_scores, o_best, o_fix, o_candA, o_candB,
+      o_partial, total;
 };
-
-void push_jobs(MMPlan& p, int r_off, int c_off, int kb, uint8_t src, int group, bool first, bool last, int& n) {
-  for (int b = 0; b < kb; b += P4V_JOB_KB) {
-    P4VJob j{};
-    const int len = std::min(P4V_JOB_KB, kb - b);
-    j.r_off = (uint32_t)(r_off + b) * P4V_TILE; j.c_off = (uint32_t)(c_off + b) * P4V_TILE; j.kb = (uint8_t)len;
-    j.flags = src | ((first && b == 0) ? P4V_JOB_FIRST : 0) | ((last && b + len >= kb) ? P4V_JOB_LAST : 0);
-    j.group = (uint8_t)group;
-    p.jobs.push_back(j); ++n;
-  }
-}
 
 int build_plan(const p4v_matmul_desc* d, MMPlan& p, bool with_search) {
   P4V_REQUIRE(d != nullptr, "null desc");
@@ -68,109 +57,105 @@ int build_plan(const p4v_matmul_desc* d, MMPlan& p, bool with_search) {
   p.ew = p.i8 ? 1 : 2;
   p.kb = (int)align_up((size_t)p.S2 * p.ew, 32);
   p.kb16 = (int)align_up((size_t)p.S2 * 2, 32);
-  p.KB_A = p.sos ? 2 * p.kb : p.kb; p.KB_B = p.kb;
-  p.KB_As = 2 * p.kb16; p.KB_Bs = 3 * p.kb16;
   const float qa1 = (float)(p.A_qmax - 1);
 
-  p.segA.clear(); p.segB.clear(); p.segAs.clear(); p.segBs.clear();
   if (p.sos) {
-    p.segA.push_back(P4VSeg{0, p.S2, 0, 0, 0.f, 0.f, qa1, 1, qa1, 0, 0});
-    p.segA.push_back(P4VSeg{0, p.S2, p.kb * P4V_TILE, 0, 0.f, 0.f, qa1, 2, qa1, 0, 0});
-    p.segAs.push_back(P4VSeg{0, p.S2, 0, 0, 0.f, 0.f, qa1, 1, qa1, 0, 0});
-    p.segAs.push_back(P4VSeg{0, p.S2, p.kb16 * P4V_TILE, 0, 0.f, 0.f, qa1, 2, qa1, 0, 0});
-    for (int t = 0; t < 3; ++t) p.segBs.push_back(P4VSeg{0, p.S2, t * p.kb16 * P4V_TILE, 0, 0.f, 0.f, 0.f, 0, 0.f, t + 1, 0});
+    p.segA.host.push_back(P4VSeg{0, p.S2, 0, 0, 0.f, 0.f, qa1, 1, qa1, 0, 0});
+    p.segA.host.push_back(P4VSeg{0, p.S2, p.kb * P4V_TILE, 0, 0.f, 0.f, qa1, 2, qa1, 0, 0});
+    p.segAs.host.push_back(P4VSeg{0, p.S2, 0, 0, 0.f, 0.f, qa1, 1, qa1, 0, 0});
+    p.segAs.host.push_back(P4VSeg{0, p.S2, p.kb16 * P4V_TILE, 0, 0.f, 0.f, qa1, 2, qa1, 0, 0});
+    for (int t = 0; t < 3; ++t) p.segBs.host.push_back(P4VSeg{0, p.S2, t * p.kb16 * P4V_TILE, 0, 0.f, 0.f, 0.f, 0, 0.f, t + 1, 0});
   } else {
-    p.segA.push_back(P4VSeg{0, p.S2, 0, 0, 0.f, (float)-p.A_qmax, (float)(p.A_qmax - 1), 0, 0.f, 0, 0});
+    p.segA.host.push_back(P4VSeg{0, p.S2, 0, 0, 0.f, (float)-p.A_qmax, (float)(p.A_qmax - 1), 0, 0.f, 0, 0});
   }
-  p.segB.push_back(P4VSeg{0, p.S2, 0, 0, 0.f, (float)-p.B_qmax, (float)(p.B_qmax - 1), 0, 0.f, 0, 0});
+  p.segB.host.push_back(P4VSeg{0, p.S2, 0, 0, 0.f, (float)-p.B_qmax, (float)(p.B_qmax - 1), 0, 0.f, 0, 0});
 
-  p.factors.resize(d->eq_n + 1);
-  for (int i = 0; i <= d->eq_n; ++i) p.factors[i] = (float)(d->eq_alpha + i * (d->eq_beta - d->eq_alpha) / d->eq_n);
+  p.factors.host = cand_factors(d->eq_n, d->eq_alpha, d->eq_beta);
   p.n_split = 20;                                         // matmul.py:636
-  p.split_factors.resize(p.n_split);
-  for (int i = 0; i < p.n_split; ++i) p.split_factors[i] = (float)(1.0 / (double)(1u << i));
+  p.split_factors.host.resize(p.n_split);
+  for (int i = 0; i < p.n_split; ++i) p.split_factors.host[i] = (float)(1.0 / (double)(1u << i));
 
-  p.jobs.clear(); p.metas.clear();
+  const int KB_A = p.sos ? 2 * p.kb : p.kb;
+  p.Acur = Operand{Image{0, KB_A, p.tiles_m, p.Pc, 1, p.i8}, false, true, nullptr, &p.segA};
+  p.Acand = Operand{Image{0, KB_A, p.tiles_m, p.Pc, d->eq_n, p.i8}, false, false, &p.factors, &p.segA};
+  p.Bcur = Operand{Image{0, p.kb, p.tiles_n, p.Pc, 1, p.i8}, true, true, nullptr, &p.segB};
+  p.Bcand = Operand{Image{0, p.kb, p.tiles_n, p.Pc, d->eq_n, p.i8}, true, false, &p.factors, &p.segB};
+  p.Ascand = Operand{Image{0, 2 * p.kb16, p.tiles_m, p.Pc, p.n_split, false}, false, false, &p.split_factors, &p.segAs};
+  p.Bsplit = Operand{Image{0, 3 * p.kb16, p.tiles_n, p.Pc, 1, false}, true, false, nullptr, &p.segBs};
+
+  std::vector<P4VJob>& jobs = p.jobs.host;
+  std::vector<GroupMeta>& metas = p.metas.host;
   p.stepA = p.stepB = p.stepS = p.fwd = MStep{};
-  auto begin = [&](MStep& s) { s = MStep{}; s.job_off = (int)p.jobs.size(); s.meta_fix = (int)p.metas.size(); };
+  auto begin = [&](MStep& s, int order, int n_cand) {
+    s = MStep{};
+    s.job_off = (int)jobs.size(); s.meta_fix = (int)metas.size(); s.order = order; s.n_cand = n_cand;
+    s.Rcur = &p.Acur.im; s.Rcand = &p.Acand.im; s.Ccur = &p.Bcur.im; s.Ccand = &p.Bcand.im;
+  };
   if (with_search) {
     if (!p.sos) {   // A step: candidates on the row operand
-      begin(p.stepA); p.stepA.meta_cand = (int)p.metas.size();
-      push_jobs(p, 0, 0, p.kb, P4V_JOB_RCAND, 0, true, true, p.stepA.ncj);
-      p.metas.push_back(GroupMeta{0, 0, 0, 0}); p.stepA.ncg = 1;
-    } else {        // split search: (hi,lo)_c x exact 3-term bf16 split of the unquantised B
-      begin(p.stepS); p.stepS.meta_cand = (int)p.metas.size();
+      begin(p.stepA, 1, d->eq_n); p.stepA.meta_cand = (int)metas.size();
+      add_group(jobs, 0, 0, p.kb, P4V_JOB_RCAND, 0, true, true, p.stepA.ncj);
+      metas.push_back(GroupMeta{0, 0, 0, 0}); p.stepA.ncg = 1;
+    } else {        // split search: (hi,lo)_c x exact 3-term bf16 split of the unquantised B; the high part ignores candA
+      begin(p.stepS, 1, p.n_split); p.stepS.meta_cand = (int)metas.size();
+      p.stepS.noA_mask = 1ull; p.stepS.Rcand = &p.Ascand.im; p.stepS.Ccur = &p.Bsplit.im;
       for (int part = 0; part < 2; ++part) {
         for (int t = 0; t < 3; ++t)
-          push_jobs(p, part * p.kb16, t * p.kb16, p.kb16, P4V_JOB_RCAND, part, t == 0, t == 2, p.stepS.ncj);
-        p.metas.push_back(GroupMeta{0, 0, 0, 0});        // both parts use aux[0] = 1/(qmax-1); lo also the candidate split
+          add_group(jobs, part * p.kb16, t * p.kb16, p.kb16, P4V_JOB_RCAND, part, t == 0, t == 2, p.stepS.ncj);
+        metas.push_back(GroupMeta{0, 0, 0, 0});        // both parts use aux[0] = 1/(qmax-1); lo also the candidate split
         ++p.stepS.ncg;
       }
     }
-    begin(p.stepB); p.stepB.meta_cand = (int)p.metas.size();
+    begin(p.stepB, 0, d->eq_n); p.stepB.meta_cand = (int)metas.size();
     if (!p.sos) {
-      push_jobs(p, 0, 0, p.kb, P4V_JOB_CCAND, 0, true, true, p.stepB.ncj);
-      p.metas.push_back(GroupMeta{0, 0, 0, 0}); p.stepB.ncg = 1;
+      add_group(jobs, 0, 0, p.kb, P4V_JOB_CCAND, 0, true, true, p.stepB.ncj);
+      metas.push_back(GroupMeta{0, 0, 0, 0}); p.stepB.ncg = 1;
     } else {
       for (int part = 0; part < 2; ++part) {
-        push_jobs(p, part * p.kb, 0, p.kb, P4V_JOB_CCAND, part, true, true, p.stepB.ncj);
-        p.metas.push_back(GroupMeta{0, (short)part, 0, 0}); ++p.stepB.ncg;     // aux[0] = 1/(qmax-1), aux[1] = A_interval
+        add_group(jobs, part * p.kb, 0, p.kb, P4V_JOB_CCAND, part, true, true, p.stepB.ncj);
+        metas.push_back(GroupMeta{0, (short)part, 0, 0}); ++p.stepB.ncg;     // aux[0] = 1/(qmax-1), aux[1] = A_interval
       }
     }
-    {   // the row operand (A) of the B step is the same for every candidate: keep it resident when it is small
-      uint32_t total = 0, off = 0;
-      for (int j = 0; j < p.stepB.ncj; ++j) total += (uint32_t)p.jobs[p.stepB.job_off + j].kb * P4V_TILE;
-      if (total <= 60 * 1024)
-        for (int j = 0; j < p.stepB.ncj; ++j) {
-          P4VJob& jb = p.jobs[p.stepB.job_off + j];
-          jb.flags |= P4V_JOB_RRES; jb.res_off = off; off += (uint32_t)jb.kb * P4V_TILE;
-        }
-    }
+    mark_resident(jobs, p.stepB.job_off, p.stepB.ncj);   // the row operand (A) of the B step is the same for every candidate
   }
-  begin(p.fwd);
-  if (!p.sos) { push_jobs(p, 0, 0, p.kb, 0, 0, true, true, p.fwd.nfj); p.metas.push_back(GroupMeta{0, 0, 0, 0}); p.fwd.nfg = 1; }
+  begin(p.fwd, 0, 1);
+  if (!p.sos) { add_group(jobs, 0, 0, p.kb, 0, 0, true, true, p.fwd.nfj); metas.push_back(GroupMeta{0, 0, 0, 0}); p.fwd.nfg = 1; }
   else for (int part = 0; part < 2; ++part) {
-    push_jobs(p, part * p.kb, 0, p.kb, 0, part, true, true, p.fwd.nfj);
-    p.metas.push_back(GroupMeta{0, (short)part, 0, 0}); ++p.fwd.nfg;
+    add_group(jobs, part * p.kb, 0, p.kb, 0, part, true, true, p.fwd.nfj);
+    metas.push_back(GroupMeta{0, (short)part, 0, 0}); ++p.fwd.nfg;
   }
-  p.fwd.meta_cand = (int)p.metas.size();
-  P4V_REQUIRE((int)p.jobs.size() <= 4 * P4V_MAX_JOBS && p.stepS.ncj <= P4V_MAX_JOBS && p.stepB.ncj <= P4V_MAX_JOBS &&
+  p.fwd.meta_cand = (int)metas.size();
+  P4V_REQUIRE((int)jobs.size() <= 4 * P4V_MAX_JOBS && p.stepS.ncj <= P4V_MAX_JOBS && p.stepB.ncj <= P4V_MAX_JOBS &&
               p.stepA.ncj <= P4V_MAX_JOBS && p.fwd.nfj <= P4V_MAX_JOBS, "matmul: S2 too large");
 
-  size_t o = 0;
-  auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+  Carver c{0};
   const int n_c = std::max(d->eq_n, p.n_split);
-  p.o_factors = take((d->eq_n + 1) * 4); p.o_sfactors = take(p.n_split * 4);
-  p.o_keys = take((2 * p.H + 1) * 4);
-  p.o_dA0 = take(p.H * 4); p.o_dA = take(p.H * 4); p.o_dB0 = take(p.H * 4); p.o_dB = take(p.H * 4);
-  p.o_ones = take(p.H * 4); p.o_aux = take(2 * 4); p.o_split = take(4); p.o_gscale = take(4);
-  p.o_scores = take((size_t)n_c * p.H * 8); p.o_best = take(p.H * 4);
-  p.o_fix = take((size_t)2 * p.H * 4); p.o_candA = take((size_t)n_c * p.H * 4); p.o_candB = take((size_t)2 * p.H * 4);
-  p.o_jobs = take(p.jobs.size() * sizeof(P4VJob)); p.o_metas = take(p.metas.size() * sizeof(GroupMeta));
-  p.o_segA = take(p.segA.size() * sizeof(P4VSeg)); p.o_segB = take(p.segB.size() * sizeof(P4VSeg));
-  p.o_segAs = take(std::max<size_t>(1, p.segAs.size()) * sizeof(P4VSeg));
-  p.o_segBs = take(std::max<size_t>(1, p.segBs.size()) * sizeof(P4VSeg));
-  const size_t tilesA = (size_t)p.Pc * p.tiles_m, tilesB = (size_t)p.Pc * p.tiles_n;   // one chunk of problems
-  p.o_partial = take(with_search ? tilesA * p.tiles_n * n_c * 32 * 4 : 4);
-  p.o_Acur = take(tilesA * P4V_TILE * p.KB_A);
-  p.o_Bcur = take(tilesB * P4V_TILE * p.KB_B);
-  p.o_Acand = take(with_search && !p.sos ? (size_t)d->eq_n * tilesA * P4V_TILE * p.KB_A : 4);
-  p.o_Bcand = take(with_search ? (size_t)d->eq_n * tilesB * P4V_TILE * p.KB_B : 4);
-  p.o_Ascand = take(with_search && p.sos ? (size_t)p.n_split * tilesA * P4V_TILE * p.KB_As : 4);
-  p.o_Bsplit = take(with_search && p.sos ? tilesB * P4V_TILE * p.KB_Bs : 4);
-  p.total = o;
+  p.factors.off = c.take(p.factors.bytes()); p.split_factors.off = c.take(p.split_factors.bytes());
+  p.o_keys = c.take((2 * p.H + 1) * 4);
+  p.o_dA0 = c.take(p.H * 4); p.o_dA = c.take(p.H * 4); p.o_dB0 = c.take(p.H * 4); p.o_dB = c.take(p.H * 4);
+  p.o_ones = c.take(p.H * 4); p.o_aux = c.take(2 * 4); p.o_split = c.take(4); p.o_gscale = c.take(4);
+  p.o_scores = c.take((size_t)n_c * p.H * 8); p.o_best = c.take(p.H * 4);
+  p.o_fix = c.take((size_t)2 * p.H * 4); p.o_candA = c.take((size_t)n_c * p.H * 4); p.o_candB = c.take((size_t)2 * p.H * 4);
+  p.jobs.off = c.take(p.jobs.bytes()); p.metas.off = c.take(p.metas.bytes());
+  p.segA.off = c.take(p.segA.bytes()); p.segB.off = c.take(p.segB.bytes());
+  p.segAs.off = c.take(std::max(p.segAs.bytes(), sizeof(P4VSeg)));
+  p.segBs.off = c.take(std::max(p.segBs.bytes(), sizeof(P4VSeg)));
+  p.o_partial = c.take(with_search ? (size_t)p.Pc * p.tiles_m * p.tiles_n * n_c * 32 * 4 : 4);   // one chunk of problems
+  p.Acur.im.off = c.take(p.Acur.im.bytes());
+  p.Bcur.im.off = c.take(p.Bcur.im.bytes());
+  p.Acand.im.off = c.take(with_search && !p.sos ? p.Acand.im.bytes() : 4);
+  p.Bcand.im.off = c.take(with_search ? p.Bcand.im.bytes() : 4);
+  p.Ascand.im.off = c.take(with_search && p.sos ? p.Ascand.im.bytes() : 4);
+  p.Bsplit.im.off = c.take(with_search && p.sos ? p.Bsplit.im.bytes() : 4);
+  p.total = c.end;
   return 0;
 }
 
 int upload(const MMPlan& p, void* ws, cudaStream_t st) {
-  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_factors), p.factors.data(), p.factors.size() * 4, cudaMemcpyHostToDevice, st));
-  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_sfactors), p.split_factors.data(), p.split_factors.size() * 4, cudaMemcpyHostToDevice, st));
-  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_jobs), p.jobs.data(), p.jobs.size() * sizeof(P4VJob), cudaMemcpyHostToDevice, st));
-  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_metas), p.metas.data(), p.metas.size() * sizeof(GroupMeta), cudaMemcpyHostToDevice, st));
-  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segA), p.segA.data(), p.segA.size() * sizeof(P4VSeg), cudaMemcpyHostToDevice, st));
-  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segB), p.segB.data(), p.segB.size() * sizeof(P4VSeg), cudaMemcpyHostToDevice, st));
-  if (!p.segAs.empty()) P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segAs), p.segAs.data(), p.segAs.size() * sizeof(P4VSeg), cudaMemcpyHostToDevice, st));
-  if (!p.segBs.empty()) P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_segBs), p.segBs.data(), p.segBs.size() * sizeof(P4VSeg), cudaMemcpyHostToDevice, st));
+  int rc;
+  if ((rc = p.factors.upload(ws, st)) || (rc = p.split_factors.upload(ws, st)) || (rc = p.jobs.upload(ws, st)) ||
+      (rc = p.metas.upload(ws, st)) || (rc = p.segA.upload(ws, st)) || (rc = p.segB.upload(ws, st)) ||
+      (rc = p.segAs.upload(ws, st)) || (rc = p.segBs.upload(ws, st))) return rc;
   std::vector<float> ones(p.H, 1.f);
   P4V_CUDA_OK(cudaMemcpyAsync(at<void>(ws, p.o_ones), ones.data(), p.H * 4, cudaMemcpyHostToDevice, st));
   return 0;
@@ -184,54 +169,39 @@ std::vector<Chunk> chunks(const MMPlan& p) {
   return cs;
 }
 
-// which: 0 Acur, 1 Acand, 2 Bcur, 3 Bcand, 4 A split-search candidates (bf16), 5 B exact split (bf16); of the problems of c
-int quant(const MMPlan& p, void* ws, int which, const float* src, Chunk c, cudaStream_t st) {
+// Build operand image o of the problems of chunk c from its source A or B
+int quant(const MMPlan& p, void* ws, const Operand& o, const float* A, const float* B, Chunk c, cudaStream_t st) {
   QuantImageArgs q{};
-  const bool isA = which == 0 || which == 1 || which == 4;
-  q.P = c.n; q.prob_stride = isA ? (long long)p.S1 * p.S2 : (long long)p.S2 * p.S3;
-  q.src = src + (size_t)c.p0 * q.prob_stride;     // chunks start at an image: problem p of the chunk is head p % heads
-  q.src_transposed = isA ? 0 : 1; q.ld = isA ? p.S2 : p.S3;
-  q.rows = isA ? p.S1 : p.S3; q.tiles = isA ? p.tiles_m : p.tiles_n;
+  o.im.chunk(o.im.tiles, c.n).fill(q, ws);
+  q.prob_stride = o.B ? (long long)p.S2 * p.S3 : (long long)p.S1 * p.S2;
+  q.src = (o.B ? B : A) + (size_t)c.p0 * q.prob_stride;     // chunks start at an image: problem p of the chunk is head p % heads
+  q.src_transposed = o.B ? 1 : 0; q.ld = o.B ? p.S3 : p.S2; q.rows = o.B ? p.S3 : p.S1;
   q.rows_per_block = 0; q.d_mod = p.H; q.d_stride = 1;
-  q.is_int8 = p.i8; q.n_planes = 1; q.factors = nullptr; q.split = at<float>(ws, p.o_split);
-  int KB = 0;
-  switch (which) {
-    case 0: q.dst = at<uint8_t>(ws, p.o_Acur); KB = p.KB_A; q.delta = at<float>(ws, p.o_dA); q.segs = at<P4VSeg>(ws, p.o_segA); q.nseg = (int)p.segA.size(); break;
-    case 1: q.dst = at<uint8_t>(ws, p.o_Acand); KB = p.KB_A; q.delta = at<float>(ws, p.o_dA0); q.segs = at<P4VSeg>(ws, p.o_segA); q.nseg = (int)p.segA.size();
-            q.n_planes = p.d.eq_n; q.factors = at<float>(ws, p.o_factors); break;
-    case 2: q.dst = at<uint8_t>(ws, p.o_Bcur); KB = p.KB_B; q.delta = at<float>(ws, p.o_dB); q.segs = at<P4VSeg>(ws, p.o_segB); q.nseg = 1; break;
-    case 3: q.dst = at<uint8_t>(ws, p.o_Bcand); KB = p.KB_B; q.delta = at<float>(ws, p.o_dB0); q.segs = at<P4VSeg>(ws, p.o_segB); q.nseg = 1;
-            q.n_planes = p.d.eq_n; q.factors = at<float>(ws, p.o_factors); break;
-    case 4: q.dst = at<uint8_t>(ws, p.o_Ascand); KB = p.KB_As; q.delta = at<float>(ws, p.o_dA0); q.segs = at<P4VSeg>(ws, p.o_segAs); q.nseg = 2;
-            q.n_planes = p.n_split; q.factors = at<float>(ws, p.o_sfactors); q.is_int8 = 0; break;
-    default: q.dst = at<uint8_t>(ws, p.o_Bsplit); KB = p.KB_Bs; q.delta = at<float>(ws, p.o_dB0); q.segs = at<P4VSeg>(ws, p.o_segBs); q.nseg = 3; q.is_int8 = 0; break;
-  }
-  q.tile_bytes = (unsigned long long)P4V_TILE * KB;
-  q.plane_stride = q.tile_bytes * q.tiles * c.n;
+  q.factors = o.factors ? o.factors->dev(ws) : nullptr; q.split = at<float>(ws, p.o_split);
+  q.delta = at<float>(ws, o.B ? (o.cur ? p.o_dB : p.o_dB0) : (o.cur ? p.o_dA : p.o_dA0));
+  q.segs = o.segs->dev(ws); q.nseg = (int)o.segs->host.size();
   return p4v_quant_image(q, st);
 }
-int quant(const MMPlan& p, void* ws, int which, const float* src, cudaStream_t st) { return quant(p, ws, which, src, Chunk{0, p.P}, st); }
+int quant(const MMPlan& p, void* ws, const Operand& o, const float* A, const float* B, cudaStream_t st) {
+  return quant(p, ws, o, A, B, Chunk{0, p.P}, st);
+}
 
 void fill_sweep(const MMPlan& p, void* ws, const MStep& s, SweepParams& sp, Chunk c) {
   sp = SweepParams{};
-  sp.R_cur = at<uint8_t>(ws, p.o_Acur); sp.C_cur = at<uint8_t>(ws, p.o_Bcur);
-  sp.R_cand = at<uint8_t>(ws, p.o_Acand); sp.C_cand = at<uint8_t>(ws, p.o_Bcand);
-  sp.R_tile_bytes = sp.R_cand_tile_bytes = (unsigned long long)P4V_TILE * p.KB_A;
-  sp.C_tile_bytes = sp.C_cand_tile_bytes = (unsigned long long)P4V_TILE * p.KB_B;
-  sp.R_cand_stride = sp.R_cand_tile_bytes * p.tiles_m * c.n; sp.C_cand_stride = sp.C_cand_tile_bytes * p.tiles_n * c.n;
+  auto part = [&](const Image* im) { return im->chunk(im->tiles, c.n); };
+  fill_images(sp, ws, part(s.Rcur), part(s.Rcand), part(s.Ccur), part(s.Ccand));
   sp.P = c.n; sp.M = p.S1; sp.N = p.S3; sp.tiles_m = p.tiles_m; sp.tiles_n = p.tiles_n;
   sp.ld = p.S3; sp.prob_stride = (long long)p.S1 * p.S3;
   sp.gscale = at<float>(ws, p.o_gscale);
-  sp.jobs = at<P4VJob>(ws, p.o_jobs) + s.job_off;
+  sp.jobs = p.jobs.dev(ws) + s.job_off;
   sp.n_fixed_jobs = s.nfj; sp.n_cand_jobs = s.ncj; sp.n_fixed_groups = s.nfg; sp.n_cand_groups = s.ncg;
   sp.fix_scale = at<float>(ws, p.o_fix); sp.candA = at<float>(ws, p.o_candA); sp.candB = at<float>(ws, p.o_candB);
   sp.nsg = p.H; sp.sg_mode = P4V_SG_PROBLEM;
-  sp.n_cand = p.d.eq_n; sp.partial = at<float>(ws, p.o_partial); sp.is_int8 = p.i8;
+  sp.cand_noA_mask = s.noA_mask; sp.n_cand = s.n_cand; sp.order = s.order; sp.partial = at<float>(ws, p.o_partial);
 }
-void fill_sweep(const MMPlan& p, void* ws, const MStep& s, SweepParams& sp) { fill_sweep(p, ws, s, sp, Chunk{0, p.P}); }
 
 int run_sweep(const MMPlan& p, const MStep& s, const SweepParams& sp, cudaStream_t st) {
-  return p4v_run_sweep(sp, p.jobs.data() + s.job_off, p.d.kernel, st);
+  return p4v_run_sweep(sp, p.jobs.host.data() + s.job_off, p.d.kernel, st);
 }
 
 // kind 2: searched operand tables (d0, cur other) per head ; kind 3: other operand = aux[meta.a]
@@ -242,8 +212,8 @@ int tables(const MMPlan& p, void* ws, const MStep& s, int kind, const float* d_s
   t.dW = d_fixed_w; t.dW0 = d_search0; t.n_V = p.H; t.n_H = 1; t.crb_rows = P4V_CG;
   t.dX = d_other; t.dX0 = d_other; t.n_a = 1; t.d_neg = 0.f;
   t.factors = factors; t.n_cand = n_cand;
-  t.fixed_meta = at<GroupMeta>(ws, p.o_metas) + s.meta_fix; t.n_fixed_groups = s.nfg;
-  t.cand_meta = at<GroupMeta>(ws, p.o_metas) + s.meta_cand; t.n_cand_groups = s.ncg;
+  t.fixed_meta = p.metas.dev(ws) + s.meta_fix; t.n_fixed_groups = s.nfg;
+  t.cand_meta = p.metas.dev(ws) + s.meta_cand; t.n_cand_groups = s.ncg;
   t.nsg = p.H;
   t.fix_scale = at<float>(ws, p.o_fix); t.candA = at<float>(ws, p.o_candA); t.candB = at<float>(ws, p.o_candB);
   return p4v_step_tables(t, st);
@@ -257,9 +227,9 @@ __global__ void sos_aux_kernel(const float* split, float qm1, float* aux, float*
 __global__ void set_scalar_kernel(float* p, float v) { p[0] = v; }
 
 // scores of chunk c: the first chunk writes the fp64 table, later chunks add to it (fixed chunk order)
-int reduce(const MMPlan& p, void* ws, const SweepParams& sp, int n_cand, bool accumulate, cudaStream_t st) {
+int reduce(const MMPlan& p, void* ws, const SweepParams& sp, bool accumulate, cudaStream_t st) {
   ReduceArgs r{};
-  r.partial = sp.partial; r.n_cand = n_cand; r.P = sp.P; r.tiles_m = p.tiles_m; r.tiles_n = p.tiles_n; r.order = sp.order;
+  r.partial = sp.partial; r.n_cand = sp.n_cand; r.P = sp.P; r.tiles_m = p.tiles_m; r.tiles_n = p.tiles_n; r.order = sp.order;
   r.mode = P4V_SG_PROBLEM; r.n_keys = p.H; r.sums = at<double>(ws, p.o_scores); r.accumulate = accumulate ? 1 : 0;
   return p4v_reduce_scores(r, st);
 }
@@ -274,21 +244,19 @@ int finish(const MMPlan& p, void* ws, int n_cand, int n_groups, double inv_count
   return p4v_select_step(f, st);
 }
 
-// One search step over every chunk: [chunk images] -> sweep -> reduce (into the table).  Unchunked, the images are
-// those begin() built and the previous step re-quantised.
-template <class Images, class Setup>
-int sweep_chunks(const MMPlan& p, void* ws, const MStep& s, const float* Y, const float* G, int n_cand, Images images,
-                 Setup setup, cudaStream_t st) {
+// One search step over every chunk: [the chunk's images R and C] -> sweep -> reduce (into the table).  Unchunked, the
+// images are those begin() built and the previous step re-quantised.
+int sweep_chunks(const MMPlan& p, void* ws, const MStep& s, const Operand& R, const Operand& C, const float* A, const float* B,
+                 const float* Y, const float* G, cudaStream_t st) {
   int rc;
   const std::vector<Chunk> cs = chunks(p);
   for (size_t i = 0; i < cs.size(); ++i) {
-    if (p.ipc && (rc = images(cs[i]))) return rc;
+    if (p.ipc && ((rc = quant(p, ws, R, A, B, cs[i], st)) || (rc = quant(p, ws, C, A, B, cs[i], st)))) return rc;
     const size_t off = (size_t)cs[i].p0 * p.S1 * p.S3;
     SweepParams sp; fill_sweep(p, ws, s, sp, cs[i]);
     sp.Y = Y + off; sp.Gr = G + off;
-    setup(sp, cs[i]);
     if ((rc = run_sweep(p, s, sp, st))) return rc;
-    if ((rc = reduce(p, ws, sp, n_cand, i > 0, st))) return rc;
+    if ((rc = reduce(p, ws, sp, i > 0, st))) return rc;
   }
   return 0;
 }
@@ -296,45 +264,36 @@ int sweep_chunks(const MMPlan& p, void* ws, const MStep& s, const float* Y, cons
 int search_A(const MMPlan& p, void* ws, const float* A, const float* B, const float* Y, const float* G, float* log, cudaStream_t st) {
   int rc;
   if ((rc = tables(p, ws, p.stepA, 2, at<float>(ws, p.o_dA0), at<float>(ws, p.o_dA), at<float>(ws, p.o_dB),
-                   at<float>(ws, p.o_factors), p.d.eq_n, st))) return rc;
-  auto images = [&](Chunk c) { int r = quant(p, ws, 1, A, c, st); return r ? r : quant(p, ws, 2, B, c, st); };
-  if ((rc = sweep_chunks(p, ws, p.stepA, Y, G, p.d.eq_n, images, [](SweepParams& sp, Chunk) { sp.order = 1; }, st))) return rc;
-  if ((rc = finish(p, ws, p.d.eq_n, p.H, 1.0 / ((double)p.S1 * p.S3), at<float>(ws, p.o_factors),
+                   p.factors.dev(ws), p.d.eq_n, st))) return rc;
+  if ((rc = sweep_chunks(p, ws, p.stepA, p.Acand, p.Bcur, A, B, Y, G, st))) return rc;
+  if ((rc = finish(p, ws, p.d.eq_n, p.H, 1.0 / ((double)p.S1 * p.S3), p.factors.dev(ws),
                    at<float>(ws, p.o_dA0), at<float>(ws, p.o_dA), log, st))) return rc;
-  return p.ipc ? 0 : quant(p, ws, 0, A, st);
+  return p.ipc ? 0 : quant(p, ws, p.Acur, A, B, st);
 }
 
 int search_B(const MMPlan& p, void* ws, const float* A, const float* B, const float* Y, const float* G, float* log, cudaStream_t st) {
   int rc;
   if ((rc = tables(p, ws, p.stepB, p.sos ? 3 : 2, at<float>(ws, p.o_dB0), at<float>(ws, p.o_dB),
-                   p.sos ? at<float>(ws, p.o_aux) : at<float>(ws, p.o_dA), at<float>(ws, p.o_factors), p.d.eq_n, st))) return rc;
-  auto images = [&](Chunk c) { int r = quant(p, ws, 0, A, c, st); return r ? r : quant(p, ws, 3, B, c, st); };
-  if ((rc = sweep_chunks(p, ws, p.stepB, Y, G, p.d.eq_n, images, [](SweepParams& sp, Chunk) { sp.order = 0; }, st))) return rc;
-  if ((rc = finish(p, ws, p.d.eq_n, p.H, 1.0 / ((double)p.S1 * p.S3), at<float>(ws, p.o_factors),
+                   p.sos ? at<float>(ws, p.o_aux) : at<float>(ws, p.o_dA), p.factors.dev(ws), p.d.eq_n, st))) return rc;
+  if ((rc = sweep_chunks(p, ws, p.stepB, p.Acur, p.Bcand, A, B, Y, G, st))) return rc;
+  if ((rc = finish(p, ws, p.d.eq_n, p.H, 1.0 / ((double)p.S1 * p.S3), p.factors.dev(ws),
                    at<float>(ws, p.o_dB0), at<float>(ws, p.o_dB), log, st))) return rc;
-  return p.ipc ? 0 : quant(p, ws, 2, B, st);
+  return p.ipc ? 0 : quant(p, ws, p.Bcur, A, B, st);
 }
 
 int search_split(const MMPlan& p, void* ws, const float* A, const float* B, const float* Y, const float* G, float* log, cudaStream_t st) {
   int rc;
   // candA[c][head] = split_c * 1, candB[g][head] = aux[0] = 1/(qmax-1); the high part ignores candA
   if ((rc = tables(p, ws, p.stepS, 3, at<float>(ws, p.o_ones), at<float>(ws, p.o_ones), at<float>(ws, p.o_aux),
-                   at<float>(ws, p.o_sfactors), p.n_split, st))) return rc;
-  auto images = [&](Chunk c) { int r = quant(p, ws, 4, A, c, st); return r ? r : quant(p, ws, 5, B, c, st); };
-  auto setup = [&](SweepParams& sp, Chunk c) {
-    sp.order = 1; sp.n_cand = p.n_split; sp.is_int8 = 0; sp.cand_noA_mask = 1ull;
-    sp.R_cand = at<uint8_t>(ws, p.o_Ascand); sp.R_cand_tile_bytes = (unsigned long long)P4V_TILE * p.KB_As;
-    sp.R_cand_stride = sp.R_cand_tile_bytes * p.tiles_m * c.n;
-    sp.C_cur = at<uint8_t>(ws, p.o_Bsplit); sp.C_tile_bytes = (unsigned long long)P4V_TILE * p.KB_Bs;
-  };
-  if ((rc = sweep_chunks(p, ws, p.stepS, Y, G, p.n_split, images, setup, st))) return rc;
+                   p.split_factors.dev(ws), p.n_split, st))) return rc;
+  if ((rc = sweep_chunks(p, ws, p.stepS, p.Ascand, p.Bsplit, A, B, Y, G, st))) return rc;
   // global score: mean over heads and rows (matmul.py:620-621)
-  if ((rc = finish(p, ws, p.n_split, 1, 1.0 / ((double)p.H * p.S1 * p.S3), at<float>(ws, p.o_sfactors),
+  if ((rc = finish(p, ws, p.n_split, 1, 1.0 / ((double)p.H * p.S1 * p.S3), p.split_factors.dev(ws),
                    at<float>(ws, p.o_ones), at<float>(ws, p.o_split), log, st))) return rc;
   sos_aux_kernel<<<1, 1, 0, st>>>(at<float>(ws, p.o_split), (float)(p.A_qmax - 1), at<float>(ws, p.o_aux), nullptr);
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
-  return p.ipc ? 0 : quant(p, ws, 0, A, st);
+  return p.ipc ? 0 : quant(p, ws, p.Acur, A, B, st);
 }
 
 int begin(const MMPlan& p, void* ws, const float* A, const float* B, const float* G, cudaStream_t st) {
@@ -359,14 +318,14 @@ int begin(const MMPlan& p, void* ws, const float* A, const float* B, const float
   }
   if (p.ipc) return 0;            // chunked: every step builds its chunks' images
   if (p.sos) {
-    if ((rc = quant(p, ws, 4, A, st))) return rc;
-    if ((rc = quant(p, ws, 5, B, st))) return rc;
+    if ((rc = quant(p, ws, p.Ascand, A, B, st))) return rc;
+    if ((rc = quant(p, ws, p.Bsplit, A, B, st))) return rc;
   } else {
-    if ((rc = quant(p, ws, 1, A, st))) return rc;
+    if ((rc = quant(p, ws, p.Acand, A, B, st))) return rc;
   }
-  if ((rc = quant(p, ws, 0, A, st))) return rc;
-  if ((rc = quant(p, ws, 2, B, st))) return rc;
-  if ((rc = quant(p, ws, 3, B, st))) return rc;
+  if ((rc = quant(p, ws, p.Acur, A, B, st))) return rc;
+  if ((rc = quant(p, ws, p.Bcur, A, B, st))) return rc;
+  if ((rc = quant(p, ws, p.Bcand, A, B, st))) return rc;
   return 0;
 }
 
@@ -443,13 +402,13 @@ extern "C" int p4v_matmul_quant_forward(const p4v_matmul_desc* d, const float* A
   } else {
     P4V_CUDA_OK(cudaMemcpyAsync(at<float>(workspace, p.o_dA), A_interval, (size_t)p.H * 4, cudaMemcpyDeviceToDevice, st));
   }
-  if ((rc = quant(p, workspace, 0, A, st))) return rc;
-  if ((rc = quant(p, workspace, 2, B, st))) return rc;
+  if ((rc = quant(p, workspace, p.Acur, A, B, st))) return rc;
+  if ((rc = quant(p, workspace, p.Bcur, A, B, st))) return rc;
   // fixed scale per head: plain dA*dB ; sos: dB * aux[part]
   if ((rc = tables(p, workspace, p.fwd, p.sos ? 3 : 2, at<float>(workspace, p.o_dB0),
                    p.sos ? at<float>(workspace, p.o_dB) : at<float>(workspace, p.o_dA),
-                   p.sos ? at<float>(workspace, p.o_aux) : at<float>(workspace, p.o_dB), at<float>(workspace, p.o_factors), 0, st))) return rc;
-  SweepParams sp; fill_sweep(p, workspace, p.fwd, sp);
-  sp.out = out; sp.n_cand = 1; sp.order = 0; sp.R_cand = nullptr; sp.C_cand = nullptr;
+                   p.sos ? at<float>(workspace, p.o_aux) : at<float>(workspace, p.o_dB), p.factors.dev(workspace), 0, st))) return rc;
+  SweepParams sp; fill_sweep(p, workspace, p.fwd, sp, Chunk{0, p.P});
+  sp.out = out; sp.R_cand = nullptr; sp.C_cand = nullptr;
   return run_sweep(p, p.fwd, sp, st);
 }
