@@ -177,6 +177,14 @@ P4V_API int p4v_profile_collect(double* sweep_ms, long long* sweep_launches, dou
  * GEMMs, out[3..5] = tensor-core operations they executed, out[6..8] = launches, out[9..11] = the longest single launch
  * (ms, operations, kind).  n must be >= 12. */
 P4V_API int p4v_profile_collect_kinds(double* out, int n);
+/* One row of P4V_LAUNCH_COLS doubles per launch recorded since profiling was enabled, in launch order, for tests that
+ * pin the path a shape takes: kind (0 bf16 sweep, 1 int8 sweep, 2 Gram GEMM), the SIMT kernel ran (0/1), consumer mode
+ * (0 multi-segment, 1 single, 2 pair; -1 for SIMT sweeps and Gram GEMMs), shared-memory ring stages, resident row-operand
+ * buffers, resident row-operand bytes (0: streamed), resident column-image bytes (0: streamed), CTAs launched, tiles,
+ * candidates, candidate groups, candidate jobs.  Writes at most max_rows rows, sets *n_rows to the number recorded and
+ * does not clear the record (p4v_profile_collect_kinds does). */
+#define P4V_LAUNCH_COLS 12
+P4V_API int p4v_profile_collect_launches(double* out, int max_rows, int* n_rows);
 /* Device self-test of the quantiser's division shortcut: evaluates round(v / delta) for n pseudo-random (v, delta)
  * pairs (plus pairs placed on and next to rounding ties) both with IEEE division, as the reference does
  * (quant_layers/linear.py:99-103 `(x / interval).round_()`), and with the reciprocal-based sequence the operand

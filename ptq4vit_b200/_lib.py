@@ -56,7 +56,7 @@ _SIGNATURES = {
                              _P, _P, _P],
 }
 EXPORTS = sorted(list(_SIGNATURES) + ["p4v_last_error", "p4v_version", "p4v_launch_count", "p4v_profile_enable", "p4v_profile_collect",
-                                     "p4v_profile_collect_kinds",
+                                     "p4v_profile_collect_kinds", "p4v_profile_collect_launches",
                                      "p4v_selftest_rint_div"])
 
 _lib = None
@@ -82,6 +82,7 @@ def lib():
         l.p4v_selftest_rint_div.argtypes = [C.c_ulonglong, C.c_ulonglong, C.POINTER(C.c_ulonglong), C.c_void_p]
         l.p4v_profile_collect.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_longlong), C.POINTER(C.c_double)]
         l.p4v_profile_collect_kinds.argtypes = [C.POINTER(C.c_double), C.c_int]
+        l.p4v_profile_collect_launches.argtypes = [C.POINTER(C.c_double), C.c_int, C.POINTER(C.c_int)]
         _lib = l
     return _lib
 

@@ -115,7 +115,16 @@ extern "C" void p4v_set_error(const char* fmt, ...);
   do { if (!(cond)) { p4v_set_error(__VA_ARGS__); return 1; } } while (0)
 
 // ---- kernel launchers shared between translation units ----------------------
-int p4v_launch_sweep_tc(const SweepParams& p, const P4VJob* host_jobs, int num_sms, cudaStream_t st);
+// What p4v_launch_sweep_tc decided for one launch (p4v_profile_collect_launches reports it).
+struct P4VLaunchDecision {
+  int mode;                       // consumer mode: 0 multi-segment, 1 single, 2 pair
+  int n_stages, resident_bufs;    // shared-memory ring stages, resident row-operand buffers
+  unsigned int resident_bytes;    // resident row operand of the tile (P4V_JOB_RRES jobs), 0 if streamed
+  unsigned int cres_bytes;        // resident column image of the tile (P4V_JOB_CRES jobs), 0 if streamed
+  int grid;                       // CTAs launched
+};
+int p4v_launch_sweep_tc(const SweepParams& p, const P4VJob* host_jobs, int num_sms, cudaStream_t st,
+                        P4VLaunchDecision* decision = nullptr);
 int p4v_launch_sweep_simt(const SweepParams& p, cudaStream_t st);
 
 // ---- library runtime (runtime.cu) -------------------------------------------

@@ -24,7 +24,10 @@ void p4v_count_launch() { ++g_launches; }
 // recorded with its kind and the tensor-core operations (2*MAC) it executes.
 enum { P4V_PROF_SWEEP_BF16 = 0, P4V_PROF_SWEEP_INT8 = 1, P4V_PROF_GRAM_GEMM = 2, P4V_PROF_KINDS = 3 };
 static bool g_prof = false;
-struct ProfRec { cudaEvent_t e0, e1; int kind; double ops; int n_cand, nfg, ncg, nfj, ncj, out; long long tiles; };
+struct ProfRec {
+  cudaEvent_t e0, e1; int kind; double ops; int n_cand, nfg, ncg, nfj, ncj, out; long long tiles;
+  int simt; P4VLaunchDecision dec;    // sweeps: the SIMT kernel ran, or what the tensor-core launcher decided
+};
 static std::vector<ProfRec> g_prof_recs;
 static std::vector<cudaEvent_t> g_prof_pool;
 static cudaEvent_t prof_event() {
@@ -35,7 +38,7 @@ bool p4v_prof_on() { return g_prof; }
 void p4v_prof_begin(cudaStream_t st, cudaEvent_t* e0) { *e0 = prof_event(); cudaEventRecord(*e0, st); }
 void p4v_prof_end(cudaStream_t st, cudaEvent_t e0, int kind, double ops) {
   cudaEvent_t e1 = prof_event(); cudaEventRecord(e1, st);
-  g_prof_recs.push_back(ProfRec{e0, e1, kind, ops, 0, 0, 0, 0, 0, 0, 0});
+  g_prof_recs.push_back(ProfRec{e0, e1, kind, ops, 0, 0, 0, 0, 0, 0, 0, 0, P4VLaunchDecision{-1, 0, 0, 0, 0, 0}});
 }
 extern "C" int p4v_profile_enable(int on) { g_prof = on != 0; return 0; }
 // out[0..2] ms per kind (bf16 sweep, int8 sweep, Gram GEMM), out[3..5] executed ops, out[6..8] launches,
@@ -56,6 +59,18 @@ extern "C" int p4v_profile_collect_kinds(double* out, int n) {
     g_prof_pool.push_back(r.e0); g_prof_pool.push_back(r.e1);
   }
   g_prof_recs.clear();
+  return 0;
+}
+extern "C" int p4v_profile_collect_launches(double* out, int max_rows, int* n_rows) {
+  P4V_REQUIRE(n_rows && (out || max_rows == 0) && max_rows >= 0, "profile_collect_launches: bad arguments");
+  *n_rows = (int)g_prof_recs.size();
+  for (int i = 0; i < *n_rows && i < max_rows; ++i) {
+    const ProfRec& r = g_prof_recs[i];
+    const double row[P4V_LAUNCH_COLS] = {(double)r.kind, (double)r.simt, (double)r.dec.mode, (double)r.dec.n_stages,
+                                         (double)r.dec.resident_bufs, (double)r.dec.resident_bytes, (double)r.dec.cres_bytes,
+                                         (double)r.dec.grid, (double)r.tiles, (double)r.n_cand, (double)r.ncg, (double)r.ncj};
+    for (int c = 0; c < P4V_LAUNCH_COLS; ++c) out[(size_t)i * P4V_LAUNCH_COLS + c] = row[c];
+  }
   return 0;
 }
 extern "C" int p4v_profile_collect(double* sweep_ms, long long* sweep_launches, double* executed_ops) {
@@ -80,12 +95,14 @@ int p4v_run_sweep(const SweepParams& sp, const P4VJob* host_jobs, int kernel, cu
   ++g_launches;
   cudaEvent_t e0 = nullptr;
   if (g_prof) p4v_prof_begin(st, &e0);
-  int rc = kernel == P4V_KERNEL_SIMT ? p4v_launch_sweep_simt(sp, st) : p4v_launch_sweep_tc(sp, host_jobs, p4v_num_sms(), st);
+  P4VLaunchDecision dec{-1, 0, 0, 0, 0, 0};
+  int rc = kernel == P4V_KERNEL_SIMT ? p4v_launch_sweep_simt(sp, st) : p4v_launch_sweep_tc(sp, host_jobs, p4v_num_sms(), st, &dec);
   if (g_prof) {
     p4v_prof_end(st, e0, sp.is_int8 ? P4V_PROF_SWEEP_INT8 : P4V_PROF_SWEEP_BF16, sweep_ops(sp, host_jobs));
     ProfRec& r = g_prof_recs.back();
     r.n_cand = sp.n_cand; r.nfg = sp.n_fixed_groups; r.ncg = sp.n_cand_groups; r.nfj = sp.n_fixed_jobs; r.ncj = sp.n_cand_jobs;
     r.out = sp.out != nullptr; r.tiles = (long long)sp.P * sp.tiles_m * sp.tiles_n;
+    r.simt = kernel == P4V_KERNEL_SIMT; r.dec = dec;
   }
   return rc;
 }

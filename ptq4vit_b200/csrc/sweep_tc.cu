@@ -659,7 +659,8 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
 
 }  // namespace
 
-int p4v_launch_sweep_tc(const SweepParams& p_in, const P4VJob* host_jobs, int num_sms, cudaStream_t st) {
+int p4v_launch_sweep_tc(const SweepParams& p_in, const P4VJob* host_jobs, int num_sms, cudaStream_t st,
+                        P4VLaunchDecision* decision) {
   SweepParams p = p_in;
   const int n_jobs = p.n_fixed_jobs + p.n_cand_jobs;
   P4V_REQUIRE(n_jobs <= P4V_MAX_JOBS, "sweep: too many jobs (%d)", n_jobs);
@@ -718,6 +719,7 @@ int p4v_launch_sweep_tc(const SweepParams& p_in, const P4VJob* host_jobs, int nu
     }
   }
   const int mode = single ? kModeSingle : pair ? kModePair : kModeMulti;
+  if (decision) *decision = P4VLaunchDecision{mode, nst, (int)p.resident_bufs, p.resident_bytes, p.cres_bytes, grid};
 #define P4V_LAUNCH(I8, MODE)                                                                           \
   do {                                                                                                 \
     P4V_CUDA_OK(cudaFuncSetAttribute(sweep_tc_kernel<I8, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
