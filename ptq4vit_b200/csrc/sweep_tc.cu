@@ -110,6 +110,39 @@ __device__ __forceinline__ void bulk_g2s_addr(uint32_t dst, const void* src, uin
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, void* bar) {
   bulk_g2s_addr(dst, src, bytes, smem_u32(bar));
 }
+// Phase clocks (build with -DP4V_SWEEP_PHASE_CLOCKS, tools/sweep_phases.py): consumer warp 0 of each warpgroup and the
+// producer add their clock64() cycles per phase into g_sweep_phases[kernel instantiation][phase]; p4v_sweep_phase_clocks
+// reads them back.  Without the flag PhaseClock is empty and the kernel compiles to the same code as without it.
+enum { kPhFull, kPhWgWait, kPhFixed, kPhCand, kPhFinal, kPhReduce, kPhConsumer, kPhEmpty, kPhProducer, kPhases };
+#ifdef P4V_SWEEP_PHASE_CLOCKS
+__device__ unsigned long long g_sweep_phases[6][kPhases];
+struct PhaseClock {
+  long long t0, mark;
+  uint32_t t[kPhases];
+  __device__ __forceinline__ void start() {
+    t0 = mark = clock64();
+#pragma unroll
+    for (int k = 0; k < kPhases; ++k) t[k] = 0;
+  }
+  __device__ __forceinline__ void skip() { mark = clock64(); }   // the time since the last mark is not attributed
+  __device__ __forceinline__ void lap(int k) { const long long n = clock64(); t[k] += (uint32_t)(n - mark); mark = n; }
+  __device__ __forceinline__ void flush(int kind, int total, bool writer) {
+    t[total] = (uint32_t)(clock64() - t0);
+    if (writer)
+#pragma unroll
+      for (int k = 0; k < kPhases; ++k)
+        if (t[k]) atomicAdd(&g_sweep_phases[kind][k], (unsigned long long)t[k]);
+  }
+};
+#else
+struct PhaseClock {
+  __device__ __forceinline__ void start() {}
+  __device__ __forceinline__ void skip() {}
+  __device__ __forceinline__ void lap(int) {}
+  __device__ __forceinline__ void flush(int, int, bool) {}
+};
+#endif
+
 // Warp-uniform single-lane election for the bulk copies.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
@@ -256,6 +289,14 @@ __device__ __forceinline__ bool next_frag(const SweepParams& P, Sched& s, Frag& 
   return true;
 }
 
+// Predicated read-only load (0 when !ok): a predicated instruction, not a branch around a load.
+__device__ __forceinline__ float ldg_if(const float* p, bool ok) {
+  float x;
+  asm("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\tmov.b32 %0, 0;\n\t@q ld.global.nc.f32 %0, [%1];\n\t}"
+      : "=f"(x) : "l"(p), "r"((uint32_t)ok));
+  return x;
+}
+
 __device__ __forceinline__ float acc_to_float(uint32_t a) { return __int2float_rn((int)a); }
 __device__ __forceinline__ float acc_to_float(float a) { return a; }
 
@@ -324,6 +365,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
     // ======================= bulk-copy producer (whole warp runs the loop, one elected lane issues) =======================
     uint32_t stage = 0, phase = 0, rbuf = 0, rphase = 0, cphase = 0;
     const uint32_t full0 = smem_u32(&S.full[0]), empty0 = smem_u32(&S.empty[0]);
+    PhaseClock pc; pc.start();
     while (next_frag(P, sched, f)) {
       const size_t rt = P.R_shared ? (size_t)f.tm : (size_t)(f.p * P.tiles_m + f.tm), ct = (size_t)(f.p * P.tiles_n + f.tn);
       const uint8_t* r_cur = P.R_cur + rt * P.R_tile_bytes;
@@ -351,7 +393,9 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
         if (++rbuf == P.resident_bufs) { rbuf = 0; rphase ^= 1; }
       }
       auto issue = [&](const P4VJob j, const uint8_t* rr, const uint8_t* cc) {
+        pc.skip();
         mbar_wait_addr(empty0 + stage * 8, phase ^ 1);
+        pc.lap(kPhEmpty);
         const uint32_t bytes = p4v_job_bytes(j);
         if (elect_one()) {
           const uint32_t fb = full0 + stage * 8;
@@ -374,6 +418,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
         r_cand += P.R_cand_stride; c_cand += P.C_cand_stride;
       }
     }
+    pc.flush((kInt8 ? 3 : 0) + kMode, kPhProducer, lane == 0);
     return;
   }
 
@@ -399,12 +444,15 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
   int nb = 0, rb = 0;                                // score reduction: candidates in the open batch, buffer
   AccT acc[64];
   float r[64];
+  PhaseClock pc; pc.start();
 
   // One job = one stage: wait for its bytes; per sub-accumulator run its K steps (a FIRST job starts from zero) and call
   // on_last() after a LAST one; the stage goes back to the producer with the last sub-accumulator.
   auto run = [&](const P4VJob jb, const uint32_t ra16, auto&& on_last) {
     const uint32_t flags = jb.flags, kb = jb.kb, nsub = p4v_job_nsub(jb);
+    pc.skip();
     mbar_wait_addr(full0 + stage * 8, phase);
+    pc.lap(kPhFull);
     uint32_t a16 = (flags & P4V_JOB_RRES) ? ra16 : ringR16 + stage * sR16;
     uint32_t b16 = (flags & P4V_JOB_CRES) ? resC16 + (jb.c_off >> 4) : ringC16 + stage * sC16;
     for (uint32_t sub = 0; sub < nsub; ++sub) {
@@ -414,7 +462,9 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
       // branch around a wgmma batch serialises it, C7520)
       const uint32_t nk = __shfl_sync(0xffffffffu, kb >> 5, 0);
       wgmma_stage(acc, nk, da, db, (flags & P4V_JOB_FIRST) ? 0u : 1u);
+      pc.skip();
       wg_wait0();
+      pc.lap(kPhWgWait);
       if (sub + 1 == nsub) warp_arrive(&S.empty[stage], lane);
       if (flags & P4V_JOB_LAST) on_last();
       a16 += kb * 8; b16 += kb * 8;        // kb * 128 bytes, in 16-byte units
@@ -481,9 +531,11 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
       int gi = 0;
       for (int j = 0; j < P.n_fixed_jobs; ++j)
         run(S.jobs[j], 0u, [&] {
+          pc.skip();
 #pragma unroll
           for (int v = 0; v < 64; ++v) r[v] = fmaf(-S.fixs[gi][v >> 3], acc_to_float(acc[v]), r[v]);
           ++gi;
+          pc.lap(kPhFixed);
         });
     }
     if (P.out != nullptr) {
@@ -499,19 +551,23 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
 #pragma unroll
       for (int v = 0; v < 64; v += 2) park[(v >> 1) * kConsumers] = make_float2(r[v], r[v + 1]);
     }
-    // g of values (v, v + 1): parked (single-segment and pair steps) or from global memory
-    const bool gvec = ((P.ld | P.prob_stride) & 1) == 0 && (f.tn + 1) * P4V_TILE <= P.N &&
-                      (reinterpret_cast<uintptr_t>(P.Gr) & 7) == 0;
-    const float* const grow = P.Gr + pbase + (size_t)gm * P.ld + gc;
+    // g of values (v, v + 1): parked (single-segment and pair steps) or, in multi-segment steps, read from global memory
+    // (L2) once per candidate.  Those reads are predicated scalar loads with no branch around them: with a branch per
+    // pair, ptxas puts each load and its use in a reconvergence region of its own, so the 32 L2 round trips of a
+    // candidate's final epilogue ran one after another (a third of the consumer's time in the int8 activation steps).
+    const float* const g0p = P.Gr + pbase + (size_t)gm * P.ld + gc;   // row gm; row gm + 8 below
+    const float* const g8p = g0p + 8 * P.ld;
+    const bool g0ok = gm < P.M, g8ok = gm + 8 < P.M;
     auto gpair = [&](const int v) -> float2 {
       if constexpr (!kMulti) {
         return park[(v >> 1) * kConsumers];
       } else {
         const int h = (v >> 1) & 1, dc = 8 * (v >> 2);
-        if (gm + 8 * h >= P.M) return make_float2(0.f, 0.f);
-        const float* gp = grow + (size_t)(8 * h) * P.ld + dc;
-        if (gvec) { const float2 x = *reinterpret_cast<const float2*>(gp); return make_float2(x.x * gs, x.y * gs); }
-        return make_float2(gc + dc < P.N ? gp[0] * gs : 0.f, gc + dc + 1 < P.N ? gp[1] * gs : 0.f);
+        const bool row = h ? g8ok : g0ok;
+        const bool ok0 = row & (gc + dc < P.N), ok1 = row & (gc + dc + 1 < P.N);
+        const float* const gp = (h ? g8p : g0p) + dc;
+        const float x0 = ldg_if(gp, ok0), x1 = ldg_if(gp + 1, ok1);
+        return make_float2(ok0 ? x0 * gs : 0.f, ok1 ? x1 * gs : 0.f);
       }
     };
 
@@ -587,6 +643,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
         for (int jj = 0; jj < P.n_cand_jobs; ++jj) {
           const P4VJob jb = S.jobs[P.n_fixed_jobs + jj];
           run(jb, res16 + (jb.res_off >> 4) + wg * 64, [&] {
+            pc.skip();
             const bool noA = (P.cand_noA_mask >> gi) & 1ull;
             if (gi + 1 < P.n_cand_groups) {
               if constexpr (kMulti) {
@@ -597,6 +654,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
                   for (int e = 0; e < 8; ++e) r[8 * k + e] = fmaf(-s, acc_to_float(acc[8 * k + e]), r[8 * k + e]);
                 }
               }
+              pc.lap(kPhCand);
             } else {
               // final segment: (g * (r - s*acc))^2; r itself is not modified
 #pragma unroll
@@ -614,6 +672,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
                 }
                 ph[k][0] = q[0]; ph[k][1] = q[1];
               }
+              pc.lap(kPhFinal);
             }
             ++gi;
           });
@@ -633,6 +692,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
         continue;
       }
       // per warp: totals of its 16 rows per column group; the two warps of a quarter add theirs every kRedBatch candidates
+      pc.skip();
       if constexpr (!kPair) {
 #pragma unroll
         for (int k = 0; k < P4V_TILE_CG; ++k) p[k] = ph[k][0] + ph[k][1];
@@ -648,6 +708,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
               rbase[(j * 2) * P4V_TILE_CG + k] + rbase[(j * 2 + 1) * P4V_TILE_CG + k];
         rb ^= 1; nb = 0;
       }
+      pc.lap(kPhReduce);
     }
     if (resB) {
       warp_arrive(&S.res_empty[rbuf], lane);       // every MMA reading the resident buffer has completed
@@ -655,9 +716,25 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
     }
     if (cresB) warp_arrive(&S.cres_empty, lane);
   }
+  pc.flush((kInt8 ? 3 : 0) + kMode, kPhConsumer, lane == 0 && (cw & 3) == 0);
 }
 
 }  // namespace
+
+#ifdef P4V_SWEEP_PHASE_CLOCKS
+// Phase clocks since the last reset: out[kernel][phase] (kernel = 3 * int8 + consumer mode, phases in kPh* order), clock64
+// cycles summed over consumer warp 0 of each warpgroup (consumer phases) or the producer warp (kPhEmpty, kPhProducer)
+// of every CTA.
+extern "C" __attribute__((visibility("default"))) int p4v_sweep_phase_clocks(unsigned long long* out, int reset) {
+  P4V_CUDA_OK(cudaDeviceSynchronize());
+  P4V_CUDA_OK(cudaMemcpyFromSymbol(out, g_sweep_phases, sizeof(g_sweep_phases)));
+  if (reset) {
+    static const unsigned long long zero[6][kPhases] = {};
+    P4V_CUDA_OK(cudaMemcpyToSymbol(g_sweep_phases, zero, sizeof(zero)));
+  }
+  return 0;
+}
+#endif
 
 int p4v_launch_sweep_tc(const SweepParams& p_in, const P4VJob* host_jobs, int num_sms, cudaStream_t st,
                         P4VLaunchDecision* decision) {
