@@ -145,11 +145,18 @@ typedef struct p4v_conv_desc {
   double eq_alpha, eq_beta;
   int32_t has_bias;
   int32_t kernel;    /* P4V_KERNEL_TCGEN05 only */
+  int32_t layerwise; /* 0: channel-wise (above).  1: BatchingEasyQuantConv2d with a_bit >= 32 (conv.py:279-441, wired by
+                        configs/BasePTQ.py:48-50): ONE weight step size for the whole kernel, initial max|W| / (qmax - 0.5)
+                        (:313), score -sum_images mean_positions mean_channels (g*(y - yhat))^2 (:387-394), first argmax
+                        (:395-396).  The same search with every channel given that step size. */
 } p4v_conv_desc;
 P4V_API int p4v_conv_workspace_bytes(const p4v_conv_desc* d, size_t* bytes);
 /* Replaces ChannelwiseBatchingQuantConv2d.calibration_step2() (conv.py:591-603): _initialize_intervals (:482-496) and
  * _search_best_w_interval (:526-557).  out: w_interval [out_channels] (reference shape oc,1,1,1), score_log NULL or
- * [eq_n][out_channels].  The search is the same in every round when the activations are not quantised: it runs once. */
+ * [eq_n][out_channels].  The search is the same in every round when the activations are not quantised: it runs once.
+ * With desc.layerwise = 1 it replaces BatchingEasyQuantConv2d.calibration_step2() (conv.py:429-441): _initialize_intervals
+ * (:312-320, weight part) and _search_best_w_interval (:365-396); out: w_interval [1] (reference shape 1,1,1,1),
+ * score_log NULL or [eq_n]. */
 P4V_API int p4v_conv_calibrate(const p4v_conv_desc* d, const float* cols, const float* weight, const float* bias,
                        const float* raw_out, const float* raw_grad, void* workspace, size_t workspace_bytes,
                        float* w_interval, float* score_log, void* stream);

@@ -31,7 +31,7 @@ class MatMulDesc(C.Structure):
 class ConvDesc(C.Structure):
     _fields_ = [("images", C.c_int32), ("out_channels", C.c_int32), ("K", C.c_int32), ("positions", C.c_int32),
                 ("w_bit", C.c_int32), ("eq_n", C.c_int32), ("eq_alpha", C.c_double), ("eq_beta", C.c_double),
-                ("has_bias", C.c_int32), ("kernel", C.c_int32)]
+                ("has_bias", C.c_int32), ("kernel", C.c_int32), ("layerwise", C.c_int32)]
 
 
 _P = C.c_void_p

@@ -10,6 +10,12 @@
 // per-ROW scale; the sweep's scales are per column group, so delta0[o] is folded into the targets once:
 //     (g * (y - b - f*d0*D))^2 = (g*d0 * ((y - b)/d0 - f*D))^2
 // and the candidate scale is the plain factor f_c.  Scores are kept per row (SweepParams::row_keys).
+//
+// Layer-wise mode (desc.layerwise = 1: BatchingEasyQuantConv2d with a_bit >= 32, conv.py:279-441, as wired by
+// configs/BasePTQ.py:48-50): one step size for the whole kernel.  It is the channel-wise search with every row given the
+// same delta0 = max|W| / (qmax - 0.5) (conv.py:313): one block over the kernel, the same planes, prescale, sweep and
+// per-row sums; only the selection differs, summing the O per-channel keys of a candidate into one score
+//     score_c = -sum_images mean_positions mean_channels (g * (y - yhat_c))^2                 (conv.py:387-394)
 #include "../../include/ptq4vit_b200.h"
 #include "plan.cuh"
 
@@ -18,6 +24,7 @@ namespace {
 struct ConvPlan {
   p4v_conv_desc d;
   int P, O, K, L, tiles_o, tiles_l, kb, w_qmax;
+  int n_d;             // step sizes searched: O (channel-wise) or 1 (layer-wise)
   Table<P4VJob> jobs; Table<P4VSeg> segW, segC; Table<float> factors;
   Image Wcand, Cimg;   // candidate planes of the integer kernel; the three-term split of the im2col matrix
   size_t o_keys, o_d0, o_d, o_gscale, o_ones, o_scores, o_best, o_candA, o_candB, o_fix, o_partial, o_Y, o_G, total;
@@ -31,6 +38,8 @@ int build_plan(const p4v_conv_desc* d, ConvPlan& p) {
   P4V_REQUIRE(d->w_bit >= 2 && d->w_bit <= 8, "conv: w_bit must be in [2,8]");
   P4V_REQUIRE(d->eq_n >= 1 && d->eq_n <= P4V_MAX_CAND, "conv: eq_n must be in [1,%d]", P4V_MAX_CAND);
   P4V_REQUIRE(d->kernel == P4V_KERNEL_TCGEN05, "conv: the channel-wise search runs on the tensor-core kernel only");
+  P4V_REQUIRE(d->layerwise == 0 || d->layerwise == 1, "conv: layerwise must be 0 or 1 (got %d)", d->layerwise);
+  p.n_d = d->layerwise ? 1 : p.O;
   p.w_qmax = 1 << (d->w_bit - 1);
   p.tiles_o = p4v_cdiv(p.O, P4V_TILE); p.tiles_l = p4v_cdiv(p.L, P4V_TILE);
   p.kb = (int)align_up((size_t)p.K * 2, 32);                    // bf16 row bytes of one term
@@ -43,9 +52,9 @@ int build_plan(const p4v_conv_desc* d, ConvPlan& p) {
   p.Wcand = Image{0, p.kb, p.tiles_o, 1, d->eq_n, false}; p.Cimg = Image{0, 3 * p.kb, p.tiles_l, p.P, 1, false};
   Carver c{0};
   const int n_c = d->eq_n;
-  p.factors.off = c.take(p.factors.bytes()); p.o_keys = c.take((p.O + 1) * 4);
-  p.o_d0 = c.take(p.O * 4); p.o_d = c.take(p.O * 4); p.o_gscale = c.take(4); p.o_ones = c.take(4);
-  p.o_scores = c.take((size_t)n_c * p.O * 8); p.o_best = c.take(p.O * 4);
+  p.factors.off = c.take(p.factors.bytes()); p.o_keys = c.take((p.n_d + 1) * 4);
+  p.o_d0 = c.take(p.n_d * 4); p.o_d = c.take(p.n_d * 4); p.o_gscale = c.take(4); p.o_ones = c.take(4);
+  p.o_scores = c.take((size_t)n_c * p.O * 8); p.o_best = c.take(p.n_d * 4);
   p.o_candA = c.take((size_t)n_c * 4); p.o_candB = c.take(4); p.o_fix = c.take(4);
   p.jobs.off = c.take(p.jobs.bytes()); p.segW.off = c.take(p.segW.bytes()); p.segC.off = c.take(p.segC.bytes());
   p.o_partial = c.take((size_t)p.P * p.tiles_o * p.tiles_l * n_c * 256 * 4);
@@ -56,12 +65,14 @@ int build_plan(const p4v_conv_desc* d, ConvPlan& p) {
   return 0;
 }
 
-// y' = (y - b[o]) / d0[o] ,  g' = g * d0[o]      ([P][O][L], one thread per element)
+// y' = (y - b[o]) / d0[o * d_stride] ,  g' = g * d0[o * d_stride]      ([P][O][L], one thread per element; d_stride 0:
+// one step size for every channel)
 __global__ void conv_prescale_kernel(const float* __restrict__ y, const float* __restrict__ g, const float* __restrict__ bias,
-                                     const float* __restrict__ d0, int O, int L, long long n, float* __restrict__ yo, float* __restrict__ go) {
+                                     const float* __restrict__ d0, int d_stride, int O, int L, long long n, float* __restrict__ yo,
+                                     float* __restrict__ go) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const int o = (int)((i / L) % O);
-    const float d = d0[o];
+    const float d = d0[o * d_stride];
     yo[i] = __fdiv_rn(y[i] - (bias ? bias[o] : 0.f), d);
     go[i] = g[i] * d;
   }
@@ -111,26 +122,27 @@ extern "C" int p4v_conv_calibrate(const p4v_conv_desc* d, const float* cols, con
   cudaStream_t st = (cudaStream_t)stream;
   if ((rc = p.factors.upload(ws, st)) || (rc = p.jobs.upload(ws, st)) || (rc = p.segW.upload(ws, st)) ||
       (rc = p.segC.upload(ws, st))) return rc;
-  // min-max step size per output channel (conv.py:487) and the gradient scale
+  // min-max step size per output channel (conv.py:487) or of the whole kernel (conv.py:313), and the gradient scale
+  const int rows_per_d = p.O / p.n_d;
   int* keys = at<int>(ws, p.o_keys);
-  if ((rc = p4v_keys_reset(keys, p.O + 1, st))) return rc;
-  if ((rc = p4v_block_max(weight, p.K, p.O, 1, p.O, p.K, 1, 1, keys, st))) return rc;
-  if ((rc = p4v_group_absmax(raw_grad, (long long)p.P * p.O * p.L, 1, 1, keys + p.O, st))) return rc;
-  if ((rc = p4v_keys_to_delta(keys, p.O, (float)p.w_qmax - 0.5f, at<float>(ws, p.o_d0), at<float>(ws, p.o_d), st))) return rc;
-  if ((rc = p4v_make_gscale(keys + p.O, at<float>(ws, p.o_gscale), st))) return rc;
+  if ((rc = p4v_keys_reset(keys, p.n_d + 1, st))) return rc;
+  if ((rc = p4v_block_max(weight, p.K, p.O, rows_per_d, p.n_d, p.K, 1, 1, keys, st))) return rc;
+  if ((rc = p4v_group_absmax(raw_grad, (long long)p.P * p.O * p.L, 1, 1, keys + p.n_d, st))) return rc;
+  if ((rc = p4v_keys_to_delta(keys, p.n_d, (float)p.w_qmax - 0.5f, at<float>(ws, p.o_d0), at<float>(ws, p.o_d), st))) return rc;
+  if ((rc = p4v_make_gscale(keys + p.n_d, at<float>(ws, p.o_gscale), st))) return rc;
   conv_fill_kernel<<<p4v_cdiv(d->eq_n, 128), 128, 0, st>>>(at<float>(ws, p.o_candA), p.factors.dev(ws), d->eq_n, at<float>(ws, p.o_candB));
   p4v_count_launch();
   const long long n = (long long)p.P * p.O * p.L;
-  conv_prescale_kernel<<<132 * 8, 256, 0, st>>>(raw_out, raw_grad, d->has_bias ? bias : nullptr, at<float>(ws, p.o_d0), p.O, p.L, n,
-                                                 at<float>(ws, p.o_Y), at<float>(ws, p.o_G));
+  conv_prescale_kernel<<<132 * 8, 256, 0, st>>>(raw_out, raw_grad, d->has_bias ? bias : nullptr, at<float>(ws, p.o_d0),
+                                                 p.n_d == 1 ? 0 : 1, p.O, p.L, n, at<float>(ws, p.o_Y), at<float>(ws, p.o_G));
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
-  {   // candidate planes of the integer kernel: rows = channels, one step size per row
+  {   // candidate planes of the integer kernel: rows = channels, one step size per row (per kernel when layer-wise)
     QuantImageArgs q{};
     p.Wcand.fill(q, ws);
     q.src = weight; q.ld = p.K; q.prob_stride = 0; q.src_transposed = 0; q.rows = p.O;
     q.factors = p.factors.dev(ws); q.delta = at<float>(ws, p.o_d0);
-    q.rows_per_block = 1; q.d_stride = 1; q.d_mod = 1; q.segs = p.segW.dev(ws); q.nseg = 1;
+    q.rows_per_block = rows_per_d; q.d_stride = 1; q.d_mod = 1; q.segs = p.segW.dev(ws); q.nseg = 1;
     if ((rc = p4v_quant_image(q, st))) return rc;
   }
   {   // exact three-term bf16 split of the FP32 im2col matrix: rows = output positions
@@ -159,12 +171,14 @@ extern "C" int p4v_conv_calibrate(const p4v_conv_desc* d, const float* cols, con
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   SelectArgs f{};
-  f.sums = at<double>(ws, p.o_scores); f.n_cand = d->eq_n; f.n_keys = p.O; f.n_groups = p.O; f.keys_per_group = 1;
-  f.inv_count = 1.0 / (double)p.L;                          // mean over the output positions, sum over the images (conv.py:548-549)
+  f.sums = at<double>(ws, p.o_scores); f.n_cand = d->eq_n; f.n_keys = p.O; f.n_groups = p.n_d; f.keys_per_group = rows_per_d;
+  // mean over the output positions, sum over the images (conv.py:548-549); layer-wise also the mean over the channels
+  // (conv.py:387-389): the O per-channel sums of a candidate are added in a fixed order into its one score
+  f.inv_count = 1.0 / ((double)rows_per_d * (double)p.L);
   f.gscale = at<float>(ws, p.o_gscale); f.factors = p.factors.dev(ws);
   f.d0 = at<float>(ws, p.o_d0); f.d = at<float>(ws, p.o_d); f.d_stride = 1; f.d_col = 0;
   f.best = at<int>(ws, p.o_best); f.score_log = score_log; f.has_next = 0;
   if ((rc = p4v_select_step(f, st))) return rc;
-  P4V_CUDA_OK(cudaMemcpyAsync(w_interval, at<float>(ws, p.o_d), (size_t)p.O * 4, cudaMemcpyDeviceToDevice, st));
+  P4V_CUDA_OK(cudaMemcpyAsync(w_interval, at<float>(ws, p.o_d), (size_t)p.n_d * 4, cudaMemcpyDeviceToDevice, st));
   return 0;
 }

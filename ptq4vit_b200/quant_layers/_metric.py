@@ -14,6 +14,15 @@ in the reference itself (linear.py:433).
 import torch
 
 
+METRICS = ("hessian", "L2_norm", "linear_weighted_L2_norm", "square_weighted_L2_norm")
+
+
+def check_metric(metric):
+    """Raise, as metric_weight would, for a metric the search kernels do not implement -- before any work is done."""
+    if metric not in METRICS:
+        raise NotImplementedError(f"metric {metric} not implemented!")
+
+
 def metric_weight(metric, y, raw_grad, what):
     if metric == "hessian":
         assert raw_grad is not None, f"raw_grad is None in {what}!"

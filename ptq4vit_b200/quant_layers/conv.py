@@ -5,6 +5,10 @@ PTQ4ViT wraps exactly one convolution per network, the patch embedding, with
 step sizes, activations left in FP32.  The search runs in the CUDA library as a batched product over
 the images: rows = output channels (candidate planes of the quantised kernel), columns = output
 positions (im2col of the FP32 input, split exactly into three bf16 terms), one score per channel.
+
+BasePTQ wraps it with `BatchingEasyQuantConv2d(..., a_bit=32)` (configs/BasePTQ.py:48-50): one weight
+step size for the whole kernel.  The library runs the same search with every channel given that step
+size and sums the per-channel scores of a candidate into one (`p4v_conv_desc.layerwise`).
 """
 import ctypes
 
@@ -13,7 +17,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _lib
-from ._metric import metric_weight
+from ._metric import check_metric, metric_weight
 
 
 class MinMaxQuantConv2d(nn.Conv2d):
@@ -111,36 +115,37 @@ class PTQSLQuantConv2d(MinMaxQuantConv2d):
         self.last_scores = None
 
 
-class ChannelwiseBatchingQuantConv2d(PTQSLQuantConv2d):
-    """reference: quant_layers/conv.py:444-613.  `a_bit >= 32` turns the activation quantizer off (the only way
-    PTQ4ViT uses this class); the weight step size is searched per output channel."""
+class _BatchingConvSearch(PTQSLQuantConv2d):
+    """The weight search of the Batching conv classes with a_bit >= 32, run by the library (csrc/conv_api.cu): per output
+    channel, or one step size for the whole kernel when `layerwise` is set."""
     batching = True
+    layerwise = False
 
     def __init__(self, *args, **kwargs):
         super().__init__(*args, **kwargs)
-        self.n_V = self.out_channels
-        self.n_H = 1
         self.calib_size = None
         self.calib_batch_size = None
         self.calib_need_batching = False
 
     def _initialize_calib_parameters(self):
-        """reference: conv.py:467-480; a whole layer fits in HBM, no batching."""
+        """reference: conv.py:297-310, :467-480; a whole layer fits in HBM, no batching."""
         self.calib_size = int(self.raw_input.shape[0])
         self.calib_batch_size = int(self.raw_input.shape[0])
 
     def _grad_for_metric(self, y):
-        """Per-element weight of the metric (conv.py:509-522); see _metric.py."""
+        """Per-element weight of the metric (conv.py:336-349, :509-522); see _metric.py."""
         return metric_weight(self.metric, y, self.raw_grad, "_get_similarity")
 
-    def calibration_step2(self):
-        """reference: conv.py:591-603.  The weight search does not depend on anything the rounds change when the
-        activations are not quantized, so its result is the same in every round: it is run once."""
+    def _check_supported(self):
+        name = type(self).__name__
+        check_metric(self.metric)
         if self.a_bit < 32:
-            raise NotImplementedError("ChannelwiseBatchingQuantConv2d: the CUDA path implements a_bit >= 32 "
-                                      "(activation quantizer off), as configs/PTQ4ViT.py:54 uses it")
+            raise NotImplementedError(f"{name}: the CUDA path implements a_bit >= 32 (activation quantizer off), as "
+                                      "configs/PTQ4ViT.py:54 and configs/BasePTQ.py:50 use it")
         if self.groups != 1 or self.init_layerwise:
-            raise NotImplementedError("ChannelwiseBatchingQuantConv2d: groups == 1 and init_layerwise=False only")
+            raise NotImplementedError(f"{name}: groups == 1 and init_layerwise=False only")
+
+    def _native_weight_search(self):
         self._initialize_calib_parameters()
         dev = self.weight.device
         if dev.type != "cuda":
@@ -150,6 +155,7 @@ class ChannelwiseBatchingQuantConv2d(PTQSLQuantConv2d):
         g = self._grad_for_metric(y).to(dev).float().contiguous()
         n, oc = y.shape[0], y.shape[1]
         L = y.shape[2] * y.shape[3]
+        nw = 1 if self.layerwise else oc
         # im2col of the FP32 input: [n, L, K] (row l = one output position), K = ic*kh*kw in the kernel's own order
         cols = F.unfold(x, self.kernel_size, self.dilation, self.padding, self.stride).transpose(1, 2).contiguous()
         K = cols.shape[2]
@@ -161,19 +167,51 @@ class ChannelwiseBatchingQuantConv2d(PTQSLQuantConv2d):
         d.eq_alpha, d.eq_beta = float(self.eq_alpha), float(self.eq_beta)
         d.has_bias = 0 if b is None else 1
         d.kernel = _lib.default_kernel()
+        d.layerwise = 1 if self.layerwise else 0
         lib = _lib.lib()
         nbytes = ctypes.c_size_t()
         _lib.check(lib.p4v_conv_workspace_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "p4v_conv_workspace_bytes")
         ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
-        w_int = torch.empty(oc, dtype=torch.float32, device=dev)
-        log = torch.empty(self.eq_n * oc, dtype=torch.float32, device=dev) if self.keep_scores else None
+        w_int = torch.empty(nw, dtype=torch.float32, device=dev)
+        log = torch.empty(self.eq_n * nw, dtype=torch.float32, device=dev) if self.keep_scores else None
         _lib.check(lib.p4v_conv_calibrate(ctypes.byref(d), _lib.ptr(cols), _lib.ptr(w2), _lib.ptr(b), _lib.ptr(y.view(n, oc, L)),
                                           _lib.ptr(g.view(n, oc, L)), _lib.ptr(ws), nbytes.value, _lib.ptr(w_int), _lib.ptr(log),
                                           ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
                    "p4v_conv_calibrate")
-        self.w_interval = w_int.view(oc, 1, 1, 1)
-        self.a_interval = (x.abs().max() / (self.a_qmax - 0.5)).detach().view(1)   # conv.py:490-496 (unused when a_bit >= 32)
-        self.last_scores = [log.view(self.eq_n, oc)] * int(self.search_round) if log is not None else None
+        self.w_interval = w_int.view(nw, 1, 1, 1)
+        # conv.py:312-320, :490-496: max over the calibration batches of max|x| / (a_qmax - 0.5) (unused when a_bit >= 32)
+        self.a_interval = (x.abs().max() / (self.a_qmax - 0.5)).detach().view(1)
+        self.last_scores = [log.view(self.eq_n, nw)] * int(self.search_round) if log is not None else None
         self.calibrated = True
         del self.raw_input, self.raw_out, self.raw_grad
+
+    def calibration_step2(self):
+        """The weight search does not depend on anything the rounds change when the activations are not quantized, so
+        its result is the same in every round: it is run once."""
+        self._check_supported()
+        self._native_weight_search()
         return None
+
+
+class BatchingEasyQuantConv2d(_BatchingConvSearch):
+    """reference: quant_layers/conv.py:279-441 (layer-wise EasyQuant).  `a_bit >= 32` turns the activation quantizer off
+    (the only way BasePTQ uses this class); ONE weight step size for the whole kernel, searched over
+    fl(f_c * max|W| / (w_qmax - 0.5)) (:313, :432) by the first maximum of
+    -sum_images mean_positions mean_channels (g * (y - yhat_c))^2 (:387-396).  w_interval has shape [1,1,1,1].
+    quant_weight_bias / quant_forward are MinMaxQuantConv2d's (a scalar step size broadcasts)."""
+    layerwise = True
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.n_V = 1
+        self.n_H = 1
+
+
+class ChannelwiseBatchingQuantConv2d(_BatchingConvSearch):
+    """reference: quant_layers/conv.py:444-613.  `a_bit >= 32` turns the activation quantizer off (the only way
+    PTQ4ViT uses this class); the weight step size is searched per output channel."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.n_V = self.out_channels
+        self.n_H = 1

@@ -25,7 +25,7 @@ import torch.nn.functional as F
 
 from .. import _lib
 from ..quant_layers._chunking import device_free_bytes
-from ..quant_layers.conv import MinMaxQuantConv2d
+from ..quant_layers.conv import BatchingEasyQuantConv2d, MinMaxQuantConv2d
 from ..quant_layers.linear import MinMaxQuantLinear, PTQSLBatchingQuantLinear, PTQSLQuantLinear
 from ..quant_layers.matmul import MinMaxQuantMatMul, PTQSLBatchingQuantMatMul, PTQSLQuantMatMul
 
@@ -180,6 +180,7 @@ def min_search_workspace_bytes(module, n_img, shapes):
         d.images, d.out_channels, d.K, d.positions = n_img, module.out_channels, shapes["conv_K"], shapes["positions"]
         d.w_bit, d.eq_n, d.eq_alpha, d.eq_beta = int(module.w_bit), int(module.eq_n), float(module.eq_alpha), float(module.eq_beta)
         d.has_bias = 0 if module.bias is None else 1
+        d.layerwise = 1 if isinstance(module, BatchingEasyQuantConv2d) else 0
         _lib.check(lib.p4v_conv_workspace_bytes(ctypes.byref(d), ctypes.byref(n)), "p4v_conv_workspace_bytes")
         return n.value + 4 * n_img * shapes["positions"] * shapes["conv_K"]
     return 0
@@ -222,10 +223,15 @@ def pack_result(module, width):
     return row
 
 
+def _conv_weight_steps(module):
+    """Weight step sizes of a searched conv: one (layer-wise EasyQuant) or one per output channel."""
+    return 1 if isinstance(module, BatchingEasyQuantConv2d) else module.out_channels
+
+
 def unpack_result(module, row, heads=None):
     """Inverse of pack_result (the module's static block structure gives the split points)."""
     if isinstance(module, MinMaxQuantConv2d):
-        nw = module.out_channels
+        nw = _conv_weight_steps(module)
         module.w_interval = row[:nw].clone().view(nw, 1, 1, 1)
         module.a_interval = row[nw:nw + 1].clone()
     elif isinstance(module, MinMaxQuantLinear):
@@ -249,7 +255,7 @@ def result_width(modules):
     w = 1
     for m in modules:
         if isinstance(m, MinMaxQuantConv2d):
-            w = max(w, m.out_channels + 1)      # per-channel weight step sizes + the (unused) activation step size
+            w = max(w, _conv_weight_steps(m) + 1)      # weight step sizes + the (unused) activation step size
         elif isinstance(m, MinMaxQuantLinear):
             w = max(w, m.n_V * m.n_H + m.n_a)
         else:
