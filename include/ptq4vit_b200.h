@@ -98,6 +98,28 @@ P4V_API int p4v_linear_quant_forward(const p4v_linear_desc* d, const float* x, c
                              const float* w_interval, const float* a_interval, void* workspace, size_t workspace_bytes,
                              float* out, void* stream);
 
+/* Frozen Linear layer: the integer weights of a calibrated layer packed once, and a forward that reads no FP32 weight.
+ * Replaces, per call of quant_forward (linear.py:62-67), the re-quantisation of the weight (quant_weight_bias, :46-55 /
+ * :152-162) and the separate activation pass (quant_input, :57-60 / :164-169 / :601-607): the output is bit-identical to
+ * p4v_linear_quant_forward with the same step sizes.
+ * `packed` (p4v_linear_pack_bytes bytes, independent of d->rows; 256-byte aligned) holds what does not depend on the
+ * batch: the int8 weight operand image (the layout the forward step uses with P4V_OPERAND_INT8: 128-row tiles, K-major
+ * 16-byte chunks, segments padded to 32 B), the scale table step_W[v,h] * step_X[a] (post-GELU: also step_W[v,h] * the
+ * constant negative-part step) per (segment group, 16-column group), the activation step sizes and the job and segment
+ * tables of the forward step.  p4v_linear_pack may copy small tables from the host; p4v_linear_frozen_forward enqueues
+ * kernels only -- no allocation, no host-to-device copy, no synchronisation -- so it can be captured in a CUDA graph.
+ * p4v_linear_frozen_path: 1 = one fused kernel quantises each 128-row tile of x into shared memory and multiplies it
+ * there (workspace 0 bytes); 0 = the quantised tile does not fit shared memory beside a two-stage weight ring (ViT-B
+ * fc2: K = 3072, two parts): the activations are quantised into an int8 image in `workspace` and multiplied by the
+ * sweep kernel.  A pure function of the descriptor without its rows. */
+P4V_API int p4v_linear_pack_bytes(const p4v_linear_desc* d, size_t* bytes);
+P4V_API int p4v_linear_pack(const p4v_linear_desc* d, const float* weight, const float* w_interval, const float* a_interval,
+                    void* packed, size_t packed_bytes, void* stream);
+P4V_API int p4v_linear_frozen_path(const p4v_linear_desc* d, int* path);
+P4V_API int p4v_linear_frozen_workspace_bytes(const p4v_linear_desc* d, size_t* bytes);
+P4V_API int p4v_linear_frozen_forward(const p4v_linear_desc* d, const float* x, const float* bias, const void* packed,
+                              void* workspace, size_t workspace_bytes, float* out, void* stream);
+
 /* One wrapped MatMul (head-wise groups, n_V = n_H = 1 per operand, as forced by
  * PTQSLBatchingQuantMatMul._get_padding_parameters, matmul.py:411-417, and used by
  * configs/PTQ4ViT.py:36-48).  A [batch,heads,S1,S2] @ B [batch,heads,S2,S3]. */

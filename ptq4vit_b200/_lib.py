@@ -45,6 +45,11 @@ _SIGNATURES = {
     "p4v_linear_intervals": [C.POINTER(LinearDesc), _P, _P, _P, _P],
     "p4v_linear_quant_forward_workspace_bytes": [C.POINTER(LinearDesc), C.POINTER(C.c_size_t)],
     "p4v_linear_quant_forward": [C.POINTER(LinearDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P],
+    "p4v_linear_pack_bytes": [C.POINTER(LinearDesc), C.POINTER(C.c_size_t)],
+    "p4v_linear_pack": [C.POINTER(LinearDesc), _P, _P, _P, _P, C.c_size_t, _P],
+    "p4v_linear_frozen_path": [C.POINTER(LinearDesc), C.POINTER(C.c_int)],
+    "p4v_linear_frozen_workspace_bytes": [C.POINTER(LinearDesc), C.POINTER(C.c_size_t)],
+    "p4v_linear_frozen_forward": [C.POINTER(LinearDesc), _P, _P, _P, _P, C.c_size_t, _P, _P],
     "p4v_matmul_workspace_bytes": [C.POINTER(MatMulDesc), C.POINTER(C.c_size_t)],
     "p4v_matmul_score_log_floats": [C.POINTER(MatMulDesc), C.POINTER(C.c_size_t)],
     "p4v_matmul_calibrate": [C.POINTER(MatMulDesc), _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P, _P, _P],

@@ -101,6 +101,16 @@ __device__ __forceinline__ float p4v_rint_div(float v, float delta, float rcp) {
 
 __device__ __forceinline__ bool p4v_rint_div_ok(float delta) { const float ad = fabsf(delta); return ad > 7.9e-31f && ad < 1.2e30f; }
 
+// One element of a plain operand image: clamp(rne(v / delta), lo, hi); fast / rcp = p4v_rint_div_ok(delta) /
+// __frcp_rn(delta).  by_rcp: the step size is one the reference holds as a Python scalar, divided by as v * (1/delta)
+// (rcp_scalar = __fdiv_rn(1, delta); see quant_image_kernel).  Shared by the operand-image kernel and the fused forward,
+// whose integers must be the same.
+__device__ __forceinline__ float p4v_quant_plain(float v, float delta, bool fast, float rcp, bool by_rcp, float rcp_scalar,
+                                                 float lo, float hi) {
+  if (by_rcp) return fminf(fmaxf(rintf(v * rcp_scalar), lo), hi);
+  return fminf(fmaxf(fast ? p4v_rint_div(v, delta, rcp) : rintf(__fdiv_rn(v, delta)), lo), hi);
+}
+
 #endif
 
 // ---- error plumbing (host) --------------------------------------------------

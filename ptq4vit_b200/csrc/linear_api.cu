@@ -699,3 +699,125 @@ extern "C" int p4v_linear_quant_forward(const p4v_linear_desc* d, const float* x
   sp.R_cand = nullptr; sp.C_cand = nullptr;
   return run_sweep(p, p.fwd, sp, st);
 }
+
+// ---- frozen layers: integer weights packed once, forward without any FP32 weight ----------------------------------
+namespace {
+
+// The forward-only plan of the layer with int8 operands, its tables addressed inside the packed buffer:
+//   [int8 weight image][scale table][activation step sizes][jobs][activation segments][weight segments][group meta]
+struct FrozenPlan {
+  LinPlan p;
+  size_t o_dX, bytes;
+  int stages, stage_kb;                 // fused kernel: ring stages (0 = streamed path) and bytes of K per row of a stage
+  Image X;                              // streamed path: the int8 activation image in the caller's workspace
+};
+
+// for_pack: the rows of the descriptor are ignored (nothing in the packed buffer, nor the path, depends on them)
+int build_frozen(const p4v_linear_desc* d, FrozenPlan& f, bool for_pack) {
+  P4V_REQUIRE(d != nullptr, "null desc");
+  p4v_linear_desc dd = *d;
+  dd.operand = P4V_OPERAND_INT8; dd.kernel = P4V_KERNEL_TCGEN05; dd.rows_per_chunk = 0;
+  if (for_pack) dd.rows = dd.tokens = 1;
+  LinPlan& p = f.p;
+  int rc = build_plan(&dd, p, false);
+  if (rc) return rc;
+  Carver c{0};
+  p.Wcur.off = c.take(p.Wcur.bytes());
+  p.o_fix = c.take((size_t)p.fwd.nfg * p.nsg * 4);
+  f.o_dX = p.o_dX = c.take((size_t)dd.n_a * 4);
+  p.jobs.off = c.take(p.jobs.bytes());
+  p.segsX.off = c.take(p.segsX.bytes());
+  p.segsW.off = c.take(p.segsW.bytes());
+  p.metas.off = c.take(p.metas.bytes());
+  f.bytes = c.end;
+  f.stage_kb = 32;
+  for (int j = 0; j < p.fwd.nfj; ++j) {
+    const P4VJob& jb = p.jobs.host[p.fwd.job_off + j];
+    f.stage_kb = std::max(f.stage_kb, (int)(jb.kb * p4v_job_nsub(jb)));
+  }
+  f.X = p.Xcur; f.X.off = 0;
+  f.stages = frozen_ring_stages(f.X.tile_bytes(), (size_t)f.stage_kb * P4V_TILE, p.Wcur.kb / 16);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int p4v_linear_pack_bytes(const p4v_linear_desc* d, size_t* bytes) {
+  FrozenPlan f; int rc = build_frozen(d, f, true);
+  if (rc) return rc;
+  P4V_REQUIRE(bytes != nullptr, "null output");
+  *bytes = f.bytes;
+  return 0;
+}
+
+extern "C" int p4v_linear_pack(const p4v_linear_desc* d, const float* weight, const float* w_interval, const float* a_interval,
+                               void* packed, size_t packed_bytes, void* stream) {
+  FrozenPlan f; int rc = build_frozen(d, f, true);
+  if (rc) return rc;
+  const LinPlan& p = f.p;
+  P4V_REQUIRE(weight && w_interval && a_interval && packed, "linear_pack: null pointer");
+  P4V_REQUIRE(packed_bytes >= f.bytes, "linear_pack: packed buffer too small (%zu < %zu)", packed_bytes, f.bytes);
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = p.jobs.upload(packed, st)) || (rc = p.segsX.upload(packed, st)) || (rc = p.segsW.upload(packed, st)) ||
+      (rc = p.metas.upload(packed, st))) return rc;
+  P4V_CUDA_OK(cudaMemcpyAsync(at<float>(packed, f.o_dX), a_interval, (size_t)d->n_a * 4, cudaMemcpyDeviceToDevice, st));
+  if ((rc = quant(p, packed, p.Wcur, p.segsW, true, weight, Rows{0, p.O}, w_interval, false, st))) return rc;
+  StepTablesArgs t = tables_args(p, packed, p.fwd, -1, 0);
+  t.dW = w_interval; t.dX = a_interval;
+  return p4v_step_tables(t, st);
+}
+
+extern "C" int p4v_linear_frozen_path(const p4v_linear_desc* d, int* path) {
+  FrozenPlan f; int rc = build_frozen(d, f, true);
+  if (rc) return rc;
+  P4V_REQUIRE(path != nullptr, "null output");
+  *path = f.stages >= 2 ? 1 : 0;
+  return 0;
+}
+
+extern "C" int p4v_linear_frozen_workspace_bytes(const p4v_linear_desc* d, size_t* bytes) {
+  FrozenPlan f; int rc = build_frozen(d, f, false);
+  if (rc) return rc;
+  P4V_REQUIRE(bytes != nullptr, "null output");
+  *bytes = f.stages >= 2 ? 0 : f.X.bytes();
+  return 0;
+}
+
+extern "C" int p4v_linear_frozen_forward(const p4v_linear_desc* d, const float* x, const float* bias, const void* packed_in,
+                                         void* workspace, size_t workspace_bytes, float* out, void* stream) {
+  FrozenPlan f; int rc = build_frozen(d, f, false);
+  if (rc) return rc;
+  const LinPlan& p = f.p;
+  void* packed = const_cast<void*>(packed_in);      // the plan's accessors take the buffer they index; nothing writes it
+  P4V_REQUIRE(x && packed && out, "linear_frozen_forward: null pointer");
+  P4V_REQUIRE(!d->has_bias || bias, "linear_frozen_forward: has_bias set but bias is null");
+  cudaStream_t st = (cudaStream_t)stream;
+  const P4VJob* host_jobs = p.jobs.host.data() + p.fwd.job_off;
+  if (f.stages >= 2) {
+    FwdParams q{};
+    q.x = x; q.ld = p.K; q.M = p.M; q.N = p.O; q.bias = d->has_bias ? bias : nullptr; q.out = out;
+    q.W = p.Wcur.ptr(packed); q.W_tile_bytes = p.Wcur.tile_bytes(); q.tiles_m = p.tiles_m; q.tiles_n = p.tiles_o;
+    q.scale = at<float>(packed, p.o_fix); q.nsg = p.nsg; q.n_groups = p.fwd.nfg;
+    q.jobs = p.jobs.dev(packed) + p.fwd.job_off; q.n_jobs = p.fwd.nfj;
+    q.segs = p.segsX.dev(packed); q.nseg = (int)p.segs.size();
+    q.dX = at<float>(packed, f.o_dX);
+    q.twin = p.twin; q.d_neg = p.d_neg; q.lo = p.twin ? 0.f : (float)-p.a_qmax; q.hi = (float)(p.a_qmax - 1);
+    q.neg_lo = (float)-p.a_qmax; q.ieee_div = p4v_scalar_div_ieee();
+    q.plane_bytes = (unsigned)p.Wcur.tile_bytes(); q.a_bytes = (unsigned)f.X.tile_bytes();
+    q.stage_bytes = (unsigned)f.stage_kb * P4V_TILE; q.n_stages = (unsigned)f.stages; q.n_chunks = (unsigned)p.Wcur.kb / 16;
+    return p4v_launch_forward_tc(q, p4v_num_sms(), st);
+  }
+  P4V_REQUIRE(workspace && workspace_bytes >= f.X.bytes(), "linear_frozen_forward: workspace too small (%zu < %zu)",
+              workspace ? workspace_bytes : (size_t)0, f.X.bytes());
+  QuantImageArgs qa{};
+  f.X.fill(qa, workspace);
+  qa.src = x; qa.ld = p.K; qa.rows = p.M; qa.delta = at<float>(packed, f.o_dX); qa.d_mod = 1;
+  qa.rows_per_block = p.M + P4V_TILE; qa.segs = p.segsX.dev(packed); qa.nseg = (int)p.segsX.host.size();
+  if ((rc = p4v_quant_image(qa, st))) return rc;
+  SweepParams sp; fill_sweep(p, packed, p.fwd, sp, all_rows(p));
+  sp.R_cur = f.X.ptr(workspace);
+  sp.bias = d->has_bias ? bias : nullptr;
+  sp.out = out; sp.n_cand = 1; sp.order = 0;
+  sp.R_cand = nullptr; sp.C_cand = nullptr;
+  return run_sweep(p, p.fwd, sp, st);
+}

@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <vector>
 
+#include "forward.cuh"
 #include "prep.cuh"
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -93,6 +94,16 @@ inline void fill_images(SweepParams& sp, void* ws, const Image& Rcur, const Imag
   sp.R_cand_tile_bytes = Rcand.tile_bytes(); sp.C_cand_tile_bytes = Ccand.tile_bytes();
   sp.R_cand_stride = Rcand.plane_stride(); sp.C_cand_stride = Ccand.plane_stride();
   sp.is_int8 = Ccur.i8;
+}
+
+// Forward of a frozen Linear layer: weight-ring stages of stage_bytes that fit in shared memory beside the resident
+// quantised activation tile of a_bytes (all segments; both parts of a post-GELU layer).  At least two, and a plane whose
+// 16-byte chunks fit the kernel's chunk table: the fused kernel (forward_tc.cu).  0: the layer streams an int8 activation
+// image through the sweep kernel instead.
+inline int frozen_ring_stages(size_t a_bytes, size_t stage_bytes, size_t plane_chunks) {
+  const size_t usable = P4V_FWD_SMEM - P4V_FWD_CTL_BYTES;
+  if (plane_chunks > P4V_FWD_MAX_CHUNKS || a_bytes + 2 * stage_bytes > usable) return 0;
+  return (int)std::min<size_t>((usable - a_bytes) / stage_bytes, P4V_FWD_MAX_STAGES);
 }
 
 // A commit copies the chosen candidate's slabs from the planes of cand into cur

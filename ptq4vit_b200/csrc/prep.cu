@@ -185,8 +185,7 @@ __global__ void quant_image_kernel(const QuantImageArgs a, int chunks_total, int
             // twin quantizer, linear.py:574, :605) is divided by as `x * (1/delta)` on the GPU: torch's CUDA true-divide
             // multiplies by the fp32 reciprocal when the divisor is a CPU scalar (ATen BinaryDivTrueKernel.cu).  Tensors
             // (every searched step size) take the IEEE division.
-            if (sg.fixed_delta > 0.f && !a.ieee_div) q = fminf(fmaxf(rintf(v * rcp_fixed), sg.lo), sg.hi);
-            else q = fminf(fmaxf(fast ? p4v_rint_div(v, delta, rcp) : rintf(__fdiv_rn(v, delta)), sg.lo), sg.hi);
+            q = p4v_quant_plain(v, delta, fast, rcp, sg.fixed_delta > 0.f && !a.ieee_div, rcp_fixed, sg.lo, sg.hi);
           }
           if (!(q == q)) q = 0.f;   // NaN (0/0) cannot be represented in the integer operand
         }

@@ -65,6 +65,7 @@ class MinMaxQuantLinear(nn.Linear):
         self.bias_correction = bias_correction
         # block structure of the base class: one block
         self.n_V = self.n_H = self.n_a = 1
+        self._packed = None                  # freeze(): packed integer weights and tables (torch.uint8, device)
 
     def forward(self, x):
         if self.mode == "raw":
@@ -118,7 +119,68 @@ class MinMaxQuantLinear(nn.Linear):
             return _QuantLinearFn.apply(self, x, self.weight, self.bias)
         return self._quant_forward_native(x)
 
+    # ---- frozen layer: integer weights packed once (csrc/forward_tc.cu) ----
+    def _interval_versions(self):
+        a = self.a_interval[0] if isinstance(self.a_interval, (list, tuple)) else self.a_interval
+        return tuple(getattr(t, "_version", None) for t in (self.w_interval, a))
+
+    def freeze(self, weight=None):
+        """Pack the layer's int8 weights and scale tables once; until unfreeze(), quant_forward runs the frozen forward,
+        which reads no FP32 weight and is bit-identical to the unfrozen one.  `weight`: quantise this [out, in] tensor
+        instead of self.weight (utils/deploy.py passes the dequantised integers of a saved model)."""
+        if not getattr(self, "calibrated", None):
+            raise RuntimeError(f"freeze() needs a calibrated module: {self}")
+        dev = self._device()
+        d = self._desc(1, 1)
+        lib = _lib.lib()
+        nbytes, path = ctypes.c_size_t(), ctypes.c_int()
+        _lib.check(lib.p4v_linear_pack_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "p4v_linear_pack_bytes")
+        _lib.check(lib.p4v_linear_frozen_path(ctypes.byref(d), ctypes.byref(path)), "p4v_linear_frozen_path")
+        packed = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        w = (self.weight if weight is None else weight).detach().to(dev).reshape(self.out_features, self.in_features).contiguous().float()
+        wi, ai = self._w_flat(), self._a_flat()
+        _lib.check(lib.p4v_linear_pack(ctypes.byref(d), _lib.ptr(w), _lib.ptr(wi), _lib.ptr(ai), _lib.ptr(packed), nbytes.value,
+                                       ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "p4v_linear_pack")
+        self._packed, self._frozen_fused, self._frozen_ws = packed, bool(path.value), None
+        # the step sizes that were packed: the objects (kept, so their identity cannot be reused) and their versions
+        self._frozen_intervals = (self.w_interval, self.a_interval, self._interval_versions())
+        return self
+
+    def unfreeze(self):
+        self._packed = self._frozen_ws = self._frozen_intervals = None
+        return self
+
+    @property
+    def frozen(self):
+        return self._packed is not None
+
+    def _frozen_forward(self, x):
+        w0, a0, v0 = self._frozen_intervals
+        if self.w_interval is not w0 or self.a_interval is not a0 or self._interval_versions() != v0:
+            raise RuntimeError(f"{self}: the step sizes changed after freeze(); call unfreeze() (and freeze() again) "
+                               "before running the layer")
+        dev = self._packed.device
+        x2 = _flat2d(x.to(dev))
+        d = self._desc(x2.shape[0], 1)
+        lib = _lib.lib()
+        ws, ws_bytes = None, 0
+        if not self._frozen_fused:           # streamed path: one int8 activation image, kept between calls
+            nbytes = ctypes.c_size_t()
+            _lib.check(lib.p4v_linear_frozen_workspace_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "frozen_workspace")
+            if self._frozen_ws is None or self._frozen_ws.numel() < nbytes.value:
+                self._frozen_ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+            ws, ws_bytes = self._frozen_ws, self._frozen_ws.numel()
+        out = torch.empty(x2.shape[0], self.out_features, dtype=torch.float32, device=dev)
+        b = None if self.bias is None else self.bias.detach().contiguous().float()
+        _lib.check(lib.p4v_linear_frozen_forward(ctypes.byref(d), _lib.ptr(x2), _lib.ptr(b), _lib.ptr(self._packed), _lib.ptr(ws),
+                                                 ws_bytes, _lib.ptr(out),
+                                                 ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                   "p4v_linear_frozen_forward")
+        return out.reshape(*x.shape[:-1], self.out_features)
+
     def _quant_forward_native(self, x):
+        if self._packed is not None:
+            return self._frozen_forward(x)
         dev = self._device()
         x2 = _flat2d(x.to(dev))
         d = self._desc(x2.shape[0], 1)

@@ -1,0 +1,88 @@
+"""After calibration: freeze a wrapped model's Linear layers into packed integer weights, save the quantised model and
+load it back.  What the reference does right after calibrating (example/test_all.py:31-36 evaluates with quant_forward,
+example/get_int.py exports the integer weights) as one deployable state.
+
+File format (`torch.save`): {"format": 1, "modules": {name: entry}} with, per wrapped module, its step sizes
+(`w_interval`, `a_interval`, `A_interval`, `B_interval`, `split` -- whichever it has, stored as they are) and, for Linear
+layers on a CUDA device, `w_int`: the int8 weight as `utils.integer.quantize_int_weight` exports it, and `w_bit`.  The
+`w_int` entries alone are what the reference's get_model_int_weight returns.
+
+Loading freezes every Linear from the integers in the file: the pack kernel is fed with `w_int * step_W` (the block's
+step size) and quantises it again.  That returns the same integers exactly: fl(q * s) = q s (1 + e) with |e| <= 2^-24,
+and the IEEE quotient by s is within |q| * 2^-23 <= 2^-16 of q, far from a rounding tie, so rne gives q.  No FP32
+weight of the module is read, and the frozen forward reads none either.
+
+MatMul and Conv modules are not frozen (both MatMul operands are activations); they keep their quant_forward.
+"""
+import torch
+
+from ..quant_layers.linear import MinMaxQuantLinear
+from . import integer
+
+INTERVALS = ("w_interval", "a_interval", "A_interval", "B_interval", "split")
+
+
+def freeze_model(wrapped_modules):
+    """Freeze every calibrated Linear; returns the names of the modules left as they are."""
+    left = []
+    for name, m in wrapped_modules.items():
+        if isinstance(m, MinMaxQuantLinear) and getattr(m, "calibrated", None):
+            m.freeze()
+        else:
+            left.append(name)
+    return left
+
+
+def unfreeze_model(wrapped_modules):
+    for m in wrapped_modules.values():
+        if isinstance(m, MinMaxQuantLinear):
+            m.unfreeze()
+
+
+def _to(v, device):
+    """A step size as stored / restored: tensors cloned onto `device`, lists element-wise, Python numbers as they are."""
+    if torch.is_tensor(v):
+        return v.detach().to(device).clone()
+    if isinstance(v, (list, tuple)):
+        return [_to(e, device) for e in v]
+    return v
+
+
+def save_quantized(wrapped_modules, path):
+    modules = {}
+    for name, m in wrapped_modules.items():
+        entry = {k: _to(getattr(m, k), "cpu") for k in INTERVALS if getattr(m, k, None) is not None}
+        if isinstance(m, MinMaxQuantLinear) and getattr(m, "calibrated", None) and m.weight.device.type == "cuda":
+            O, K = m.out_features, m.in_features
+            entry["w_int"] = integer._export(m.weight.detach().reshape(O, K), m.w_interval, O // m.n_V, m.n_V, K // m.n_H,
+                                             m.n_H, integer.MODE_INT8, m.w_bit).cpu()
+            entry["w_bit"] = int(m.w_bit)
+        modules[name] = entry
+    torch.save({"format": 1, "modules": modules}, path)
+
+
+def load_quantized(wrapped_modules, path):
+    """Restore the step sizes of every module in the file, mark the modules calibrated and freeze the Linear layers from
+    the file's int8 weights.  Returns the names of the modules that were not frozen."""
+    state = torch.load(path, map_location="cpu", weights_only=True)
+    if state.get("format") != 1:
+        raise RuntimeError(f"{path}: not a ptq4vit_b200 quantised-model file")
+    missing = sorted(set(state["modules"]) ^ set(wrapped_modules))
+    if missing:
+        raise RuntimeError(f"{path}: modules differ from the wrapped model: {missing[:8]}")
+    params = [p for m in wrapped_modules.values() for p in m.parameters()]
+    device = params[0].device if params else torch.device("cpu")      # MatMul modules have no parameters of their own
+    left = []
+    for name, m in wrapped_modules.items():
+        entry = state["modules"][name]
+        for k in INTERVALS:
+            if k in entry:
+                setattr(m, k, _to(entry[k], device))
+        m.calibrated = True
+        if isinstance(m, MinMaxQuantLinear) and "w_int" in entry and m.weight.device.type == "cuda":
+            if entry["w_bit"] != m.w_bit:
+                raise RuntimeError(f"{path}: {name} was saved with w_bit {entry['w_bit']}, the module has {m.w_bit}")
+            m.freeze(weight=integer.dequantize_int_weight(m, entry["w_int"].to(device)))
+        else:
+            left.append(name)
+    return left
