@@ -156,6 +156,25 @@ P4V_API int p4v_matmul_quant_forward(const p4v_matmul_desc* d, const float* A, c
                              const float* B_interval, const float* split, void* workspace, size_t workspace_bytes,
                              float* out, void* stream);
 
+/* Frozen MatMul module: the step sizes and scale tables of a calibrated module packed once, and a forward that only
+ * enqueues one kernel.  Replaces, per call of quant_forward (matmul.py:40-45 / :140-145; split-of-softmax quant_input_A
+ * with A_interval = split / (A_qmax - 1), :595-598 / :628-629), the separate quantisation passes of both operands: the
+ * output is bit-identical to p4v_matmul_quant_forward with the same step sizes.
+ * `packed` (p4v_matmul_pack_bytes bytes; 16-byte aligned) depends on heads, the bit widths and sos only, not on batch
+ * or the sequence lengths: the per-head step sizes A_interval [heads] (unused with sos) and B_interval [heads], split
+ * [1] (sos), and the scale table of the unfrozen forward -- plain dA[h] * dB[h]; sos dB[h] * (1 / (A_qmax - 1)) and
+ * dB[h] * (split / (A_qmax - 1)) -- computed by the same kernels.  p4v_matmul_pack copies a small table from the host.
+ * p4v_matmul_frozen_forward reads A [batch,heads,S1,S2] and B [batch,heads,S2,S3] in place through element strides
+ * (A_strides / B_strides: batch, head, then the two matrix dimensions, as torch's Tensor.stride()); A must have unit
+ * stride along S2, B unit stride along S2 or S3 (the permuted q / k^T / v views of an attention block qualify).  `out` is
+ * [batch,heads,S1,S3] contiguous.  No allocation, no host-to-device copy, no synchronisation, no workspace: it can be
+ * captured in a CUDA graph.  Every argument is validated before the launch. */
+P4V_API int p4v_matmul_pack_bytes(const p4v_matmul_desc* d, size_t* bytes);
+P4V_API int p4v_matmul_pack(const p4v_matmul_desc* d, const float* A_interval, const float* B_interval, const float* split,
+                    void* packed, size_t packed_bytes, void* stream);
+P4V_API int p4v_matmul_frozen_forward(const p4v_matmul_desc* d, const float* A, const long long* A_strides, const float* B,
+                              const long long* B_strides, const void* packed, float* out, void* stream);
+
 /* The patch-embedding convolution: ChannelwiseBatchingQuantConv2d with a_bit >= 32 (quant_layers/conv.py:444-614, wired
  * by configs/PTQ4ViT.py:52-54): one weight step size per output channel, activations left in FP32.  The caller passes
  * the im2col matrix of the FP32 input (torch.nn.functional.unfold, [images, positions, K], K = in_channels*kh*kw in the

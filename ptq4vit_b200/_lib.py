@@ -55,6 +55,9 @@ _SIGNATURES = {
     "p4v_matmul_calibrate": [C.POINTER(MatMulDesc), _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P, _P, _P],
     "p4v_matmul_quant_forward_workspace_bytes": [C.POINTER(MatMulDesc), C.POINTER(C.c_size_t)],
     "p4v_matmul_quant_forward": [C.POINTER(MatMulDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P],
+    "p4v_matmul_pack_bytes": [C.POINTER(MatMulDesc), C.POINTER(C.c_size_t)],
+    "p4v_matmul_pack": [C.POINTER(MatMulDesc), _P, _P, _P, _P, C.c_size_t, _P],
+    "p4v_matmul_frozen_forward": [C.POINTER(MatMulDesc), _P, C.POINTER(C.c_longlong), _P, C.POINTER(C.c_longlong), _P, _P, _P],
     "p4v_conv_workspace_bytes": [C.POINTER(ConvDesc), C.POINTER(C.c_size_t)],
     "p4v_conv_calibrate": [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P],
     "p4v_export_quantized": [_P, C.c_longlong, C.c_longlong, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,

@@ -111,6 +111,14 @@ __device__ __forceinline__ float p4v_quant_plain(float v, float delta, bool fast
   return fminf(fmaxf(fast ? p4v_rint_div(v, delta, rcp) : rintf(__fdiv_rn(v, delta)), lo), hi);
 }
 
+// One element of a split-of-softmax operand image (matmul.py:595-598): part 1 (high) = rne(clamp(v, split, 1) * qm1),
+// part 2 (low) = rne(clamp(v, 0, split) / (split / qm1)), both clamped to [0, qm1].  Shared by the operand-image kernel
+// and the fused MatMul forward, whose integers must be the same.
+__device__ __forceinline__ float p4v_quant_sos(float v, float split, float qm1, int part) {
+  if (part == 1) return fminf(fmaxf(rintf(fminf(fmaxf(v, split), 1.f) * qm1), 0.f), qm1);
+  return fminf(fmaxf(rintf(__fdiv_rn(fminf(fmaxf(v, 0.f), split), __fdiv_rn(split, qm1))), 0.f), qm1);
+}
+
 #endif
 
 // ---- error plumbing (host) --------------------------------------------------

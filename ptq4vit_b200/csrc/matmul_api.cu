@@ -37,11 +37,17 @@ struct MMPlan {
       o_partial, total;
 };
 
-int build_plan(const p4v_matmul_desc* d, MMPlan& p, bool with_search) {
+// the checks every entry point makes of the shape and the bit widths
+int check_shape(const p4v_matmul_desc* d) {
   P4V_REQUIRE(d != nullptr, "null desc");
-  p.d = *d;
   P4V_REQUIRE(d->batch > 0 && d->heads > 0 && d->S1 > 0 && d->S2 > 0 && d->S3 > 0, "matmul: empty shape");
   P4V_REQUIRE(d->A_bit >= 2 && d->A_bit <= 8 && d->B_bit >= 2 && d->B_bit <= 8, "matmul: bit widths must be in [2,8]");
+  return 0;
+}
+
+int build_plan(const p4v_matmul_desc* d, MMPlan& p, bool with_search) {
+  if (int rc = check_shape(d)) return rc;
+  p.d = *d;
   P4V_REQUIRE(d->eq_n >= 1 && d->eq_n <= P4V_MAX_CAND, "matmul: eq_n must be in [1,%d]", P4V_MAX_CAND);
   P4V_REQUIRE(d->images_per_chunk >= 0 && d->images_per_chunk <= d->batch,
               "matmul: images_per_chunk must be in [0, batch=%d] (got %d; 0 = whole layer)", d->batch, d->images_per_chunk);
@@ -411,4 +417,94 @@ extern "C" int p4v_matmul_quant_forward(const p4v_matmul_desc* d, const float* A
   SweepParams sp; fill_sweep(p, workspace, p.fwd, sp, Chunk{0, p.P});
   sp.out = out; sp.R_cand = nullptr; sp.C_cand = nullptr;
   return run_sweep(p, p.fwd, sp, st);
+}
+
+// ---- frozen modules: step sizes and scale tables packed once, a forward that only enqueues one kernel -------------
+namespace {
+
+// The packed buffer of a module: [dA heads][dB heads][split][aux 2][scale groups x heads][group meta groups].  A function
+// of heads and sos only.
+struct Packed {
+  int groups;
+  size_t o_dA, o_dB, o_split, o_aux, o_scale, o_meta, bytes;
+};
+Packed packed_layout(const p4v_matmul_desc* d) {
+  Packed k{};
+  k.groups = d->sos ? 2 : 1;
+  Carver c{0};
+  k.o_dA = c.take((size_t)d->heads * 4); k.o_dB = c.take((size_t)d->heads * 4);
+  k.o_split = c.take(4); k.o_aux = c.take(2 * 4);
+  k.o_scale = c.take((size_t)k.groups * d->heads * 4);
+  k.o_meta = c.take((size_t)k.groups * sizeof(GroupMeta));
+  k.bytes = c.end;
+  return k;
+}
+
+}  // namespace
+
+extern "C" int p4v_matmul_pack_bytes(const p4v_matmul_desc* d, size_t* bytes) {
+  if (int rc = check_shape(d)) return rc;
+  P4V_REQUIRE(bytes != nullptr, "null output");
+  *bytes = packed_layout(d).bytes;
+  return 0;
+}
+
+extern "C" int p4v_matmul_pack(const p4v_matmul_desc* d, const float* A_interval, const float* B_interval, const float* split,
+                               void* packed, size_t packed_bytes, void* stream) {
+  if (int rc = check_shape(d)) return rc;
+  const Packed k = packed_layout(d);
+  P4V_REQUIRE(B_interval && packed && (d->sos ? split != nullptr : A_interval != nullptr), "matmul_pack: null pointer");
+  P4V_REQUIRE(packed_bytes >= k.bytes, "matmul_pack: packed buffer too small (%zu < %zu)", packed_bytes, k.bytes);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(packed) & 15) == 0, "matmul_pack: packed must be 16-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int H = d->heads;
+  const float qm1 = (float)((1 << (d->A_bit - 1)) - 1);
+  // the forward step's groups as the unfrozen forward plans them (build_plan: one plain group; sos: high, low part)
+  std::vector<GroupMeta> metas;
+  for (int g = 0; g < k.groups; ++g) metas.push_back(GroupMeta{0, (short)g, 0, 0});
+  P4V_CUDA_OK(cudaMemcpyAsync(at<void>(packed, k.o_meta), metas.data(), metas.size() * sizeof(GroupMeta), cudaMemcpyHostToDevice, st));
+  P4V_CUDA_OK(cudaMemcpyAsync(at<float>(packed, k.o_dB), B_interval, (size_t)H * 4, cudaMemcpyDeviceToDevice, st));
+  if (d->sos) {
+    P4V_CUDA_OK(cudaMemcpyAsync(at<float>(packed, k.o_split), split, 4, cudaMemcpyDeviceToDevice, st));
+    sos_aux_kernel<<<1, 1, 0, st>>>(at<float>(packed, k.o_split), qm1, at<float>(packed, k.o_aux), nullptr);
+    p4v_count_launch();
+    P4V_CUDA_OK(cudaGetLastError());
+  } else {
+    P4V_CUDA_OK(cudaMemcpyAsync(at<float>(packed, k.o_dA), A_interval, (size_t)H * 4, cudaMemcpyDeviceToDevice, st));
+  }
+  // the scale table of p4v_matmul_quant_forward: plain dA[h] * dB[h]; sos dB[h] * aux[part]
+  StepTablesArgs t{};
+  t.kind = d->sos ? 3 : 2; t.n_V = H; t.n_H = 1; t.crb_rows = P4V_CG; t.n_a = 1;
+  t.dW = at<float>(packed, d->sos ? k.o_dB : k.o_dA);
+  t.dX = at<float>(packed, d->sos ? k.o_aux : k.o_dB);
+  t.fixed_meta = at<GroupMeta>(packed, k.o_meta); t.n_fixed_groups = k.groups;
+  t.nsg = H; t.fix_scale = at<float>(packed, k.o_scale);
+  return p4v_step_tables(t, st);
+}
+
+extern "C" int p4v_matmul_frozen_forward(const p4v_matmul_desc* d, const float* A, const long long* A_strides, const float* B,
+                                         const long long* B_strides, const void* packed, float* out, void* stream) {
+  if (int rc = check_shape(d)) return rc;
+  P4V_REQUIRE(A && A_strides && B && B_strides && packed && out, "matmul_frozen_forward: null pointer");
+  for (int i = 0; i < 4; ++i)
+    P4V_REQUIRE(A_strides[i] >= 0 && B_strides[i] >= 0, "matmul_frozen_forward: negative stride");
+  P4V_REQUIRE(A_strides[3] == 1, "matmul_frozen_forward: A must have unit stride along K (got %lld)", A_strides[3]);
+  P4V_REQUIRE(B_strides[2] == 1 || B_strides[3] == 1,
+              "matmul_frozen_forward: B must have unit stride along K or along N (got %lld, %lld)", B_strides[2], B_strides[3]);
+  P4V_REQUIRE(((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(out)) & 3) == 0,
+              "matmul_frozen_forward: A, B and out must be 4-byte aligned");
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(packed) & 15) == 0, "matmul_frozen_forward: packed must be 16-byte aligned");
+  const Packed k = packed_layout(d);
+  const int A_qmax = 1 << (d->A_bit - 1), B_qmax = 1 << (d->B_bit - 1);
+  FwdMMParams q{};
+  q.A = A; q.sA_b = A_strides[0]; q.sA_h = A_strides[1]; q.sA_m = A_strides[2];
+  q.B = B; q.sB_b = B_strides[0]; q.sB_h = B_strides[1]; q.sB_k = B_strides[2]; q.sB_n = B_strides[3];
+  q.out = out;
+  q.batch = d->batch; q.heads = d->heads; q.S1 = d->S1; q.S2 = d->S2; q.S3 = d->S3;
+  void* pk = const_cast<void*>(packed);         // read only
+  q.dA = at<float>(pk, k.o_dA); q.dB = at<float>(pk, k.o_dB); q.split = at<float>(pk, k.o_split);
+  q.scale = at<float>(pk, k.o_scale);
+  q.A_lo = (float)-A_qmax; q.A_hi = (float)(A_qmax - 1); q.B_lo = (float)-B_qmax; q.B_hi = (float)(B_qmax - 1);
+  q.qm1 = (float)(A_qmax - 1);
+  return p4v_launch_forward_mm_tc(q, d->sos != 0, (cudaStream_t)stream);
 }

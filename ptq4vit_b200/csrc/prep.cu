@@ -176,10 +176,8 @@ __global__ void quant_image_kernel(const QuantImageArgs a, int chunks_total, int
             const float b1 = __bfloat162float(__float2bfloat16_rn(v));
             const float b2 = __bfloat162float(__float2bfloat16_rn(v - b1));
             q = sg.split3 == 1 ? b1 : (sg.split3 == 2 ? b2 : __bfloat162float(__float2bfloat16_rn((v - b1) - b2)));
-          } else if (sg.sos_part == 1) {
-            q = fminf(fmaxf(rintf(fminf(fmaxf(v, split), 1.f) * sg.qm1), 0.f), sg.qm1);
-          } else if (sg.sos_part == 2) {
-            q = fminf(fmaxf(rintf(__fdiv_rn(fminf(fmaxf(v, 0.f), split), __fdiv_rn(split, sg.qm1))), 0.f), sg.qm1);
+          } else if (sg.sos_part) {
+            q = p4v_quant_sos(v, split, sg.qm1, sg.sos_part);
           } else {
             // A step size that the reference holds as a Python scalar (the constant negative-part step of the post-GELU
             // twin quantizer, linear.py:574, :605) is divided by as `x * (1/delta)` on the GPU: torch's CUDA true-divide

@@ -45,6 +45,7 @@ class MinMaxQuantMatMul(nn.Module):
         self.mode = mode
         self.raw_input = None
         self.raw_out = None
+        self._packed = None                  # freeze(): {heads: packed step sizes and scale tables (torch.uint8, device)}
 
     def forward(self, A, B):
         if self.mode == "raw":
@@ -82,8 +83,11 @@ class MinMaxQuantMatMul(nn.Module):
     def _desc(self, A, B, search_round=1, eq=(0.0, 1.0, 1)):
         assert A.dim() == 4 and B.dim() == 4 and A.shape[:2] == B.shape[:2] and A.shape[3] == B.shape[2], \
             f"expected A [b,H,S1,S2] and B [b,H,S2,S3], got {tuple(A.shape)} and {tuple(B.shape)}"
+        return self._desc_dims(A.shape[0], A.shape[1], A.shape[2], A.shape[3], B.shape[3], search_round, eq)
+
+    def _desc_dims(self, batch, heads, S1, S2, S3, search_round=1, eq=(0.0, 1.0, 1)):
         d = _lib.MatMulDesc()
-        d.batch, d.heads, d.S1, d.S2, d.S3 = int(A.shape[0]), int(A.shape[1]), int(A.shape[2]), int(A.shape[3]), int(B.shape[3])
+        d.batch, d.heads, d.S1, d.S2, d.S3 = int(batch), int(heads), int(S1), int(S2), int(S3)
         d.A_bit, d.B_bit = int(self.A_bit), int(self.B_bit)
         d.eq_n, d.search_round = int(eq[2]), int(search_round)
         d.eq_alpha, d.eq_beta = float(eq[0]), float(eq[1])
@@ -108,7 +112,101 @@ class MinMaxQuantMatMul(nn.Module):
             return _QuantMatMulFn.apply(self, A, B)
         return self._quant_forward_native(A, B)
 
+    # ---- frozen module: step sizes packed once (csrc/forward_mm_tc.cu) ----
+    def _intervals(self):
+        return (self.A_interval, self.B_interval, self.split if self.sos else None)
+
+    def _interval_versions(self):
+        return tuple(getattr(t, "_version", None) for t in self._intervals())
+
+    def _n_steps(self):
+        """Step-size entries per operand: the heads (head-wise layout) or 1 (n_G = 1: one step size for all heads)."""
+        sizes = [torch.as_tensor(self.B_interval).numel()] + ([] if self.sos else [torch.as_tensor(self.A_interval).numel()])
+        n = max(sizes)
+        if any(k not in (1, n) for k in sizes):
+            raise RuntimeError(f"{self}: A_interval and B_interval hold {sizes[1]} and {sizes[0]} step sizes")
+        return n
+
+    def _pack(self, heads, dev):
+        """The packed tables for `heads` heads (a single step size is expanded to all of them, as the unfrozen forward does)."""
+        def flat(v):
+            t = torch.as_tensor(v, dtype=torch.float32, device=dev).reshape(-1)
+            return (t if t.numel() == heads else t.expand(heads)).contiguous()
+        a = None if self.sos else flat(self.A_interval)
+        b = flat(self.B_interval)
+        split = torch.as_tensor(self.split, dtype=torch.float32, device=dev).reshape(1) if self.sos else None
+        d = self._desc_dims(1, heads, 1, 1, 1)
+        lib = _lib.lib()
+        nbytes = ctypes.c_size_t()
+        _lib.check(lib.p4v_matmul_pack_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "p4v_matmul_pack_bytes")
+        packed = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        _lib.check(lib.p4v_matmul_pack(ctypes.byref(d), _lib.ptr(a), _lib.ptr(b), _lib.ptr(split), _lib.ptr(packed), nbytes.value,
+                                       ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "p4v_matmul_pack")
+        return packed
+
+    def freeze(self):
+        """Pack the module's step sizes and scale tables once; until unfreeze(), quant_forward runs the fused frozen forward
+        (one kernel, both operands quantised in shared memory, strided q / k / v views read in place), which is
+        bit-identical to the unfrozen one.  With one step size for all heads (n_G = 1) the tables for a given number of
+        heads are packed at the first call with that many heads."""
+        if not getattr(self, "calibrated", None):
+            raise RuntimeError(f"freeze() needs a calibrated module: {self}")
+        b = self.B_interval
+        if not torch.is_tensor(b) or b.device.type != "cuda":
+            raise RuntimeError("ptq4vit_b200 MatMul quant layers freeze step sizes held on a CUDA device (no CPU path)")
+        n = self._n_steps()
+        self._packed = {n: self._pack(n, b.device)}
+        # the step sizes that were packed: the objects (kept, so their identity cannot be reused) and their versions
+        self._frozen_intervals = (self._intervals(), self._interval_versions())
+        return self
+
+    def unfreeze(self):
+        self._packed = self._frozen_intervals = None
+        return self
+
+    @property
+    def frozen(self):
+        return self._packed is not None
+
+    @staticmethod
+    def _strides(t, unit_dims):
+        """Element strides for the kernel; a dimension of size 1 gets the stride the kernel expects (never used)."""
+        return (ctypes.c_longlong * 4)(*[(1 if i in unit_dims else 0) if n == 1 else st
+                                         for i, (n, st) in enumerate(zip(t.shape, t.stride()))])
+
+    def _frozen_forward(self, A, B):
+        i0, v0 = self._frozen_intervals
+        if any(a is not b for a, b in zip(self._intervals(), i0)) or self._interval_versions() != v0:
+            raise RuntimeError(f"{self}: the step sizes changed after freeze(); call unfreeze() (and freeze() again) "
+                               "before running the layer")
+        assert A.dim() == 4 and B.dim() == 4 and A.shape[:2] == B.shape[:2] and A.shape[3] == B.shape[2], \
+            f"expected A [b,H,S1,S2] and B [b,H,S2,S3], got {tuple(A.shape)} and {tuple(B.shape)}"
+        dev = next(iter(self._packed.values())).device
+        A_, B_ = A.to(dev, torch.float32), B.to(dev, torch.float32)
+        # read in place: A with unit stride along K, B along K (k^T) or N (v); any other layout is copied once
+        if A_.shape[3] > 1 and A_.stride(3) != 1:
+            A_ = A_.contiguous()
+        if B_.shape[2] > 1 and B_.shape[3] > 1 and 1 not in B_.stride()[2:]:
+            B_ = B_.contiguous()
+        batch, H, S1, S2 = A_.shape
+        S3 = B_.shape[3]
+        packed = self._packed.get(H)
+        if packed is None:
+            if self._n_steps() != 1:
+                raise RuntimeError(f"{self}: frozen with {self._n_steps()} head-wise step sizes, called with {H} heads")
+            packed = self._packed[H] = self._pack(H, dev)
+        out = torch.empty(batch, H, S1, S3, dtype=torch.float32, device=dev)
+        d = self._desc_dims(batch, H, S1, S2, S3)
+        sb = self._strides(B_, (2,) if B_.shape[2] == 1 or B_.stride(2) == 1 else (3,))
+        _lib.check(_lib.lib().p4v_matmul_frozen_forward(ctypes.byref(d), _lib.ptr(A_), self._strides(A_, (3,)), _lib.ptr(B_), sb,
+                                                        _lib.ptr(packed), _lib.ptr(out),
+                                                        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                   "p4v_matmul_frozen_forward")
+        return out
+
     def _quant_forward_native(self, A, B):
+        if self._packed is not None:
+            return self._frozen_forward(A, B)
         A_, B_ = self._cuda(A), self._cuda(B)
         dev = A_.device
         d = self._desc(A_, B_)

@@ -1,5 +1,5 @@
-"""After calibration: freeze a wrapped model's Linear layers into packed integer weights, save the quantised model and
-load it back.  What the reference does right after calibrating (example/test_all.py:31-36 evaluates with quant_forward,
+"""After calibration: freeze a wrapped model's Linear layers into packed integer weights (and, on request, its MatMul
+modules into packed step sizes), save the quantised model and load it back.  What the reference does right after calibrating (example/test_all.py:31-36 evaluates with quant_forward,
 example/get_int.py exports the integer weights) as one deployable state.
 
 File format (`torch.save`): {"format": 1, "modules": {name: entry}} with, per wrapped module, its step sizes
@@ -12,21 +12,32 @@ step size) and quantises it again.  That returns the same integers exactly: fl(q
 and the IEEE quotient by s is within |q| * 2^-23 <= 2^-16 of q, far from a rounding tie, so rne gives q.  No FP32
 weight of the module is read, and the frozen forward reads none either.
 
-MatMul and Conv modules are not frozen (both MatMul operands are activations); they keep their quant_forward.
+With `matmul=True` the MatMul modules are frozen as well: their step sizes and scale tables are packed once and every
+call runs one fused kernel that quantises both activation operands in shared memory (csrc/forward_mm_tc.cu), with the
+same bits.  A model frozen that way runs its whole quantised forward without host work between kernels, so it can be
+captured in one CUDA graph.  The default leaves the MatMul modules as they are.  The Conv module is never frozen: its
+quant_forward is torch operations on the device and already capturable.
 """
 import torch
 
 from ..quant_layers.linear import MinMaxQuantLinear
+from ..quant_layers.matmul import MinMaxQuantMatMul
 from . import integer
 
 INTERVALS = ("w_interval", "a_interval", "A_interval", "B_interval", "split")
 
 
-def freeze_model(wrapped_modules):
-    """Freeze every calibrated Linear; returns the names of the modules left as they are."""
+def _freezes(m, matmul):
+    return isinstance(m, MinMaxQuantLinear) or (matmul and isinstance(m, MinMaxQuantMatMul))
+
+
+def freeze_model(wrapped_modules, matmul=False):
+    """Freeze every calibrated Linear and, with matmul=True, every calibrated MatMul; returns the names of the modules
+    left as they are.  By default (matmul=False) the MatMul modules keep their quant_forward and are among the names
+    returned, as before the MatMul modules could be frozen."""
     left = []
     for name, m in wrapped_modules.items():
-        if isinstance(m, MinMaxQuantLinear) and getattr(m, "calibrated", None):
+        if _freezes(m, matmul) and getattr(m, "calibrated", None):
             m.freeze()
         else:
             left.append(name)
@@ -35,7 +46,7 @@ def freeze_model(wrapped_modules):
 
 def unfreeze_model(wrapped_modules):
     for m in wrapped_modules.values():
-        if isinstance(m, MinMaxQuantLinear):
+        if isinstance(m, (MinMaxQuantLinear, MinMaxQuantMatMul)):
             m.unfreeze()
 
 
@@ -61,9 +72,10 @@ def save_quantized(wrapped_modules, path):
     torch.save({"format": 1, "modules": modules}, path)
 
 
-def load_quantized(wrapped_modules, path):
+def load_quantized(wrapped_modules, path, matmul=False):
     """Restore the step sizes of every module in the file, mark the modules calibrated and freeze the Linear layers from
-    the file's int8 weights.  Returns the names of the modules that were not frozen."""
+    the file's int8 weights (and, with matmul=True, the MatMul modules from their step sizes).  Returns the names of the
+    modules that were not frozen."""
     state = torch.load(path, map_location="cpu", weights_only=True)
     if state.get("format") != 1:
         raise RuntimeError(f"{path}: not a ptq4vit_b200 quantised-model file")
@@ -83,6 +95,8 @@ def load_quantized(wrapped_modules, path):
             if entry["w_bit"] != m.w_bit:
                 raise RuntimeError(f"{path}: {name} was saved with w_bit {entry['w_bit']}, the module has {m.w_bit}")
             m.freeze(weight=integer.dequantize_int_weight(m, entry["w_int"].to(device)))
+        elif matmul and isinstance(m, MinMaxQuantMatMul) and device.type == "cuda":
+            m.freeze()
         else:
             left.append(name)
     return left
