@@ -175,6 +175,35 @@ P4V_API int p4v_matmul_pack(const p4v_matmul_desc* d, const float* A_interval, c
 P4V_API int p4v_matmul_frozen_forward(const p4v_matmul_desc* d, const float* A, const long long* A_strides, const float* B,
                               const long long* B_strides, const void* packed, float* out, void* stream);
 
+/* Fused frozen attention core: one attention call of a block whose matmul1 and matmul2 modules are frozen.  Replaces the
+ * reference's attention forward between the qkv and proj Linears (utils/models.py:10-26 for ViT / DeiT, :28-56 for
+ * Swin windows) -- matmul1 (matmul.py:40-45), the `* scale`, relative-position bias and shifted-window mask, the softmax,
+ * matmul2 (split-of-softmax A operand :595-598) and the transpose to [B, N, C] -- with one kernel
+ * (csrc/forward_attn_tc.cu) whose output is bit-identical to that sequence on the frozen modules and torch's softmax.
+ *   qkv        the qkv Linear's output as [batch, N, 3, heads, head_dim] with unit stride along head_dim; qkv_strides are
+ *              the element strides of the batch, token, part (q / k / v) and head dimensions.  4-byte aligned.
+ *   mm1, pack1 matmul1's descriptor and p4v_matmul_pack blob, as packed (heads must be a->heads; not split-of-softmax);
+ *   mm2, pack2 matmul2's, likewise (plain or split-of-softmax).  pack*_bytes: the size of each blob.
+ *   bias       [heads, N, N] contiguous, added to the scores, or NULL;
+ *   mask       [n_windows, N, N] contiguous, added after the bias to image b's scores from window b % n_windows, or NULL.
+ *   out        [batch, N, heads * head_dim] contiguous, 8-byte aligned.
+ * Shapes: N <= 256 (the scores of one query tile stay in shared memory), head_dim a multiple of 16, at most 64.
+ * p4v_attention_fused_ok says whether a shape qualifies (a pure function of N and head_dim).  Every argument is validated
+ * before the launch; no allocation, no copy, no synchronisation: the call can be captured in a CUDA graph. */
+typedef struct p4v_attention_desc {
+  int32_t batch;       /* images, or windows of all images (Swin)                                      */
+  int32_t tokens;      /* N: queries = keys                                                              */
+  int32_t heads, head_dim;
+  int32_t scale_on_q;  /* 0: scores = matmul1 * scale (ViT, DeiT); 1: matmul1(q * scale, k^T) (Swin)     */
+  int32_t n_windows;   /* rows of mask; 0 without a mask                                                 */
+  double scale;        /* a Python float in the model: applied as (float)scale                           */
+} p4v_attention_desc;
+P4V_API int p4v_attention_fused_ok(int32_t tokens, int32_t head_dim, int* ok);
+P4V_API int p4v_attention_frozen_forward(const p4v_attention_desc* a, const float* qkv, const long long* qkv_strides,
+                                 const p4v_matmul_desc* mm1, const void* pack1, size_t pack1_bytes,
+                                 const p4v_matmul_desc* mm2, const void* pack2, size_t pack2_bytes,
+                                 const float* bias, const float* mask, float* out, void* stream);
+
 /* The patch-embedding convolution: ChannelwiseBatchingQuantConv2d with a_bit >= 32 (quant_layers/conv.py:444-614, wired
  * by configs/PTQ4ViT.py:52-54): one weight step size per output channel, activations left in FP32.  The caller passes
  * the im2col matrix of the FP32 input (torch.nn.functional.unfold, [images, positions, K], K = in_channels*kh*kw in the

@@ -28,6 +28,11 @@ class MatMulDesc(C.Structure):
                 ("kernel", C.c_int32), ("init_layerwise", C.c_int32), ("images_per_chunk", C.c_int32)]
 
 
+class AttentionDesc(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("tokens", C.c_int32), ("heads", C.c_int32), ("head_dim", C.c_int32),
+                ("scale_on_q", C.c_int32), ("n_windows", C.c_int32), ("scale", C.c_double)]
+
+
 class ConvDesc(C.Structure):
     _fields_ = [("images", C.c_int32), ("out_channels", C.c_int32), ("K", C.c_int32), ("positions", C.c_int32),
                 ("w_bit", C.c_int32), ("eq_n", C.c_int32), ("eq_alpha", C.c_double), ("eq_beta", C.c_double),
@@ -58,6 +63,9 @@ _SIGNATURES = {
     "p4v_matmul_pack_bytes": [C.POINTER(MatMulDesc), C.POINTER(C.c_size_t)],
     "p4v_matmul_pack": [C.POINTER(MatMulDesc), _P, _P, _P, _P, C.c_size_t, _P],
     "p4v_matmul_frozen_forward": [C.POINTER(MatMulDesc), _P, C.POINTER(C.c_longlong), _P, C.POINTER(C.c_longlong), _P, _P, _P],
+    "p4v_attention_fused_ok": [C.c_int32, C.c_int32, C.POINTER(C.c_int)],
+    "p4v_attention_frozen_forward": [C.POINTER(AttentionDesc), _P, C.POINTER(C.c_longlong), C.POINTER(MatMulDesc), _P, C.c_size_t,
+                                     C.POINTER(MatMulDesc), _P, C.c_size_t, _P, _P, _P, _P],
     "p4v_conv_workspace_bytes": [C.POINTER(ConvDesc), C.POINTER(C.c_size_t)],
     "p4v_conv_calibrate": [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P],
     "p4v_export_quantized": [_P, C.c_longlong, C.c_longlong, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,

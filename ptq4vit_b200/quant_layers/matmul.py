@@ -174,14 +174,25 @@ class MinMaxQuantMatMul(nn.Module):
         return (ctypes.c_longlong * 4)(*[(1 if i in unit_dims else 0) if n == 1 else st
                                          for i, (n, st) in enumerate(zip(t.shape, t.stride()))])
 
-    def _frozen_forward(self, A, B):
+    def _frozen_pack(self, heads):
+        """The packed tables of a frozen module for `heads` heads, after checking that its step sizes are the ones
+        freeze() packed (with one step size for all heads, the tables for a new head count are packed here)."""
         i0, v0 = self._frozen_intervals
         if any(a is not b for a, b in zip(self._intervals(), i0)) or self._interval_versions() != v0:
             raise RuntimeError(f"{self}: the step sizes changed after freeze(); call unfreeze() (and freeze() again) "
                                "before running the layer")
+        packed = self._packed.get(heads)
+        if packed is None:
+            if self._n_steps() != 1:
+                raise RuntimeError(f"{self}: frozen with {self._n_steps()} head-wise step sizes, called with {heads} heads")
+            packed = self._packed[heads] = self._pack(heads, next(iter(self._packed.values())).device)
+        return packed
+
+    def _frozen_forward(self, A, B):
         assert A.dim() == 4 and B.dim() == 4 and A.shape[:2] == B.shape[:2] and A.shape[3] == B.shape[2], \
             f"expected A [b,H,S1,S2] and B [b,H,S2,S3], got {tuple(A.shape)} and {tuple(B.shape)}"
-        dev = next(iter(self._packed.values())).device
+        packed = self._frozen_pack(A.shape[1])
+        dev = packed.device
         A_, B_ = A.to(dev, torch.float32), B.to(dev, torch.float32)
         # read in place: A with unit stride along K, B along K (k^T) or N (v); any other layout is copied once
         if A_.shape[3] > 1 and A_.stride(3) != 1:
@@ -190,11 +201,6 @@ class MinMaxQuantMatMul(nn.Module):
             B_ = B_.contiguous()
         batch, H, S1, S2 = A_.shape
         S3 = B_.shape[3]
-        packed = self._packed.get(H)
-        if packed is None:
-            if self._n_steps() != 1:
-                raise RuntimeError(f"{self}: frozen with {self._n_steps()} head-wise step sizes, called with {H} heads")
-            packed = self._packed[H] = self._pack(H, dev)
         out = torch.empty(batch, H, S1, S3, dtype=torch.float32, device=dev)
         d = self._desc_dims(batch, H, S1, S2, S3)
         sb = self._strides(B_, (2,) if B_.shape[2] == 1 or B_.stride(2) == 1 else (3,))
@@ -226,6 +232,44 @@ class MinMaxQuantMatMul(nn.Module):
                                                 ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
                    "p4v_matmul_quant_forward")
         return out
+
+
+def frozen_attention_applies(matmul1, matmul2, tokens, head_dim, *inputs):
+    """Whether one call of an attention block can run as the fused frozen attention core: both MatMul modules frozen and
+    in quant_forward mode, matmul1 not split-of-softmax, no input that requires grad under grad mode, and a shape the
+    kernel holds (p4v_attention_fused_ok: at most 256 tokens, head_dim a multiple of 16 up to 64)."""
+    if not all(isinstance(m, MinMaxQuantMatMul) and m.frozen and m.mode == "quant_forward" for m in (matmul1, matmul2)):
+        return False
+    if matmul1.sos or (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in inputs)):
+        return False
+    ok = ctypes.c_int()
+    _lib.check(_lib.lib().p4v_attention_fused_ok(int(tokens), int(head_dim), ctypes.byref(ok)), "p4v_attention_fused_ok")
+    return bool(ok.value)
+
+
+def frozen_attention(matmul1, matmul2, qkv, scale, scale_on_q, bias=None, mask=None):
+    """The attention core between the qkv and proj Linears in one kernel (csrc/forward_attn_tc.cu), for a call where
+    frozen_attention_applies holds.  `qkv` is the qkv Linear's output viewed as [B, N, 3, heads, head_dim]; returns
+    matmul2(softmax(S), v).transpose(1, 2).reshape(B, N, C) with S = matmul1(q, k^T) * scale (scale_on_q=False, ViT) or
+    matmul1(q * scale, k^T) + bias [+ mask of window b % nW] (scale_on_q=True, Swin), with the bits of that sequence."""
+    B, N, _, H, D = qkv.shape
+    p1, p2 = matmul1._frozen_pack(H), matmul2._frozen_pack(H)
+    dev = p1.device
+    qkv = qkv.to(dev, torch.float32)
+    if qkv.stride(4) != 1:
+        qkv = qkv.contiguous()
+    bias = None if bias is None else bias.to(dev, torch.float32).contiguous()
+    mask = None if mask is None else mask.to(dev, torch.float32).contiguous()
+    a = _lib.AttentionDesc()
+    a.batch, a.tokens, a.heads, a.head_dim = int(B), int(N), int(H), int(D)
+    a.scale_on_q, a.n_windows, a.scale = int(bool(scale_on_q)), 0 if mask is None else int(mask.shape[0]), float(scale)
+    d1, d2 = matmul1._desc_dims(1, H, 1, 1, 1), matmul2._desc_dims(1, H, 1, 1, 1)
+    out = torch.empty(B, N, H * D, dtype=torch.float32, device=dev)
+    _lib.check(_lib.lib().p4v_attention_frozen_forward(
+        ctypes.byref(a), _lib.ptr(qkv), (ctypes.c_longlong * 4)(*qkv.stride()[:4]), ctypes.byref(d1), _lib.ptr(p1), p1.numel(),
+        ctypes.byref(d2), _lib.ptr(p2), p2.numel(), _lib.ptr(bias), _lib.ptr(mask), _lib.ptr(out),
+        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "p4v_attention_frozen_forward")
+    return out
 
 
 class PTQSLQuantMatMul(MinMaxQuantMatMul):

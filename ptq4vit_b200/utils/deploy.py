@@ -17,12 +17,18 @@ call runs one fused kernel that quantises both activation operands in shared mem
 same bits.  A model frozen that way runs its whole quantised forward without host work between kernels, so it can be
 captured in one CUDA graph.  The default leaves the MatMul modules as they are.  The Conv module is never frozen: its
 quant_forward is torch operations on the device and already capturable.
+
+`fuse_attention(net)` goes one step further for attention blocks whose two MatMul modules are frozen: the whole core
+between the qkv and proj Linears -- matmul1, the scale, bias and mask, the softmax, matmul2 and the transpose to
+[B, N, C] -- runs as one kernel (csrc/forward_attn_tc.cu) with the bits of the unfused sequence, and the score matrix
+never reaches HBM.  It is opt-in; `unfuse_attention(net)` undoes it.
 """
 import torch
 
 from ..quant_layers.linear import MinMaxQuantLinear
 from ..quant_layers.matmul import MinMaxQuantMatMul
 from . import integer
+from .models import Attention, WindowAttention
 
 INTERVALS = ("w_interval", "a_interval", "A_interval", "B_interval", "split")
 
@@ -48,6 +54,26 @@ def unfreeze_model(wrapped_modules):
     for m in wrapped_modules.values():
         if isinstance(m, (MinMaxQuantLinear, MinMaxQuantMatMul)):
             m.unfreeze()
+
+
+def fuse_attention(net):
+    """Mark every attention module of `net` whose matmul1 and matmul2 are frozen MatMul modules as fused: each call that
+    qualifies (no input requiring grad under grad mode, at most 256 tokens, head_dim a multiple of 16 up to 64) runs the
+    fused attention core; any other call runs the modules as before.  Returns the names of the attention modules left
+    unfused because a MatMul module is not frozen."""
+    left = []
+    for name, m in net.named_modules():
+        if isinstance(m, (Attention, WindowAttention)):
+            m.fused = all(isinstance(mm, MinMaxQuantMatMul) and mm.frozen for mm in (m.matmul1, m.matmul2))
+            if not m.fused:
+                left.append(name)
+    return left
+
+
+def unfuse_attention(net):
+    for m in net.modules():
+        if isinstance(m, (Attention, WindowAttention)):
+            m.fused = False
 
 
 def _to(v, device):

@@ -5,6 +5,8 @@ available offline, so weights are synthetic (trunc-normal 0.02) -- this is harne
 import torch
 import torch.nn as nn
 
+from ..quant_layers.matmul import frozen_attention, frozen_attention_applies
+
 
 class MatMul(nn.Module):
     def forward(self, A, B):
@@ -21,9 +23,15 @@ class Attention(nn.Module):
         self.matmul1 = MatMul()
         self.matmul2 = MatMul()
 
+    fused = False      # set by utils.deploy.fuse_attention: run the frozen attention core as one kernel when it applies
+
     def forward(self, x):
         B, N, C = x.shape
-        qkv = self.qkv(x).reshape(B, N, 3, self.num_heads, C // self.num_heads).permute(2, 0, 3, 1, 4)
+        y = self.qkv(x)
+        if self.fused and frozen_attention_applies(self.matmul1, self.matmul2, N, C // self.num_heads, y):
+            qkv5 = y.reshape(B, N, 3, self.num_heads, C // self.num_heads)
+            return self.proj(frozen_attention(self.matmul1, self.matmul2, qkv5, self.scale, scale_on_q=False))
+        qkv = y.reshape(B, N, 3, self.num_heads, C // self.num_heads).permute(2, 0, 3, 1, 4)
         q, k, v = qkv.unbind(0)
         attn = self.matmul1(q, k.transpose(-2, -1)) * self.scale
         attn = attn.softmax(dim=-1)
@@ -131,9 +139,18 @@ class WindowAttention(nn.Module):
         self.matmul1 = MatMul()
         self.matmul2 = MatMul()
 
+    fused = False      # set by utils.deploy.fuse_attention, as Attention.fused
+
     def forward(self, x, mask=None):
         B_, N, C = x.shape
-        qkv = self.qkv(x).reshape(B_, N, 3, self.num_heads, C // self.num_heads).permute(2, 0, 3, 1, 4)
+        y = self.qkv(x)
+        if self.fused:
+            bias = self.relative_position_bias_table[self.relative_position_index.view(-1)].view(N, N, -1).permute(2, 0, 1).contiguous()
+            if frozen_attention_applies(self.matmul1, self.matmul2, N, C // self.num_heads, y, bias, mask):
+                qkv5 = y.reshape(B_, N, 3, self.num_heads, C // self.num_heads)
+                return self.proj(frozen_attention(self.matmul1, self.matmul2, qkv5, self.scale, scale_on_q=True, bias=bias,
+                                                  mask=mask))
+        qkv = y.reshape(B_, N, 3, self.num_heads, C // self.num_heads).permute(2, 0, 3, 1, 4)
         q, k, v = qkv.unbind(0)
         q = q * self.scale
         attn = self.matmul1(q, k.transpose(-2, -1))
