@@ -102,7 +102,9 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t da, uint64_t
 
 __global__ void __launch_bounds__(kThreads, 1) gram_gemm_kernel(const __grid_constant__ GramGemmArgs a) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
+  // 128-byte aligned base, formed by pointer arithmetic on the __shared__ array (not an integer round trip) so that
+  // the compiler keeps the shared state space: LDS / STS instead of generic loads and stores with 64-bit addresses.
+  uint8_t* smem = smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u);
   Ctl& S = *reinterpret_cast<Ctl*>(smem + (size_t)kStages * kStageBytes);
   const uint32_t ring = smem_u32(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;

@@ -336,7 +336,9 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
   using AccT = typename std::conditional<kInt8, uint32_t, float>::type;
   constexpr bool kPair = kMode == kModePair, kMulti = kMode == kModeMulti;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
+  // 128-byte aligned base, formed by pointer arithmetic on the __shared__ array (not an integer round trip) so that
+  // the compiler keeps the shared state space: LDS / STS instead of generic loads and stores with 64-bit addresses.
+  uint8_t* smem = smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u);
   // carve: [ring R stages][ring C stages][resident R x bufs][resident C][control][score reduction][gradient tile]
   const uint32_t sR = P.stage_r_bytes, sC = P.stage_c_bytes, nst = P.n_stages, resB = P.resident_bytes, cresB = P.cres_bytes;
   const uint32_t ringR = smem_u32(smem), ringC = ringR + nst * sR, resR = ringC + nst * sC, resC = resR + P.resident_bufs * resB;
