@@ -119,6 +119,13 @@ __device__ __forceinline__ float p4v_quant_sos(float v, float split, float qm1, 
   return fminf(fmaxf(rintf(__fdiv_rn(fminf(fmaxf(v, 0.f), split), __fdiv_rn(split, qm1))), 0.f), qm1);
 }
 
+// The int8 operand byte of a quantised value q (p4v_quant_plain / p4v_quant_sos): the integer's low byte.  NaN (0/0)
+// cannot be represented in the integer operand and becomes 0.
+__device__ __forceinline__ uint32_t p4v_qbyte(float q) {
+  if (!(q == q)) q = 0.f;
+  return (uint32_t)((int)q & 0xff);
+}
+
 #endif
 
 // ---- error plumbing (host) --------------------------------------------------

@@ -26,6 +26,7 @@
 // dimension to 32 for matmul1 and 64 for matmul2 (zero bytes).  Shared memory is a function of the padded key length:
 // 112 KiB at 256 keys with split-of-softmax, so two CTAs share an SM.
 #include "forward.cuh"
+#include "sm90.cuh"
 #include <climits>
 
 namespace {
@@ -43,34 +44,6 @@ __host__ __device__ inline AttnLayout attn_layout(int sp, int kd, bool sos) {
   L.s = L.v + kRows * sp;
   L.total = L.s + kRows * sp * 4;
   return L;
-}
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
-// K-major, no swizzle: LBO = rows x 16 B between the 16-byte K chunks, SBO = 128 B between 8-row groups
-__device__ __forceinline__ uint64_t mm_desc(uint32_t addr, uint32_t rows) {
-  return (uint64_t)((addr & 0x3FFFF) >> 4) | ((uint64_t)((rows * 16) >> 4) << 16) | ((uint64_t)(128 >> 4) << 32);
-}
-__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-
-#define AT_D32                                                                                                      \
-  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29," \
-  "%30,%31}"
-#define AT_OP8(i) "+r"(d[i]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3]), "+r"(d[i + 4]), "+r"(d[i + 5]), "+r"(d[i + 6]), "+r"(d[i + 7])
-
-// D[64 rows][64 cols] += A[64][32 int8 of K] * B[64][32 int8 of K]^T
-__device__ __forceinline__ void mma_k32(uint32_t (&d)[32], uint64_t da, uint64_t db) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 " AT_D32 ", %32, %33, p;\n\t}"
-               : AT_OP8(0), AT_OP8(8), AT_OP8(16), AT_OP8(24) : "l"(da), "l"(db));
-}
-
-// one operand element as the frozen MatMul forward quantises it (forward_mm_tc.cu): the integer's low byte
-__device__ __forceinline__ uint32_t qbyte(float q) {
-  if (!(q == q)) q = 0.f;                    // NaN (0/0) cannot be represented in the integer operand
-  return (uint32_t)((int)q & 0xff);
 }
 
 template <bool SOS>
@@ -114,7 +87,7 @@ __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_
       const int r = warp + 8 * i;
       const float xs = P.scale_on_q ? __fmul_rn(x[i], P.scale) : x[i];
       sQ[((d >> 4) * kRows + r) * 16 + (d & 15)] =
-          (uint8_t)((r < rows && d < P.D) ? qbyte(p4v_quant_plain(xs, dA1, fA1, rA1, false, 0.f, P.A1_lo, P.A1_hi)) : 0u);
+          (uint8_t)((r < rows && d < P.D) ? p4v_qbyte(p4v_quant_plain(xs, dA1, fA1, rA1, false, 0.f, P.A1_lo, P.A1_hi)) : 0u);
     }
   }
 #pragma unroll 1
@@ -131,7 +104,7 @@ __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_
     for (int i = 0; i < 8; ++i) {
       const int n = n0 + warp + 8 * i;
       sK[((d >> 4) * P.sp + n) * 16 + (d & 15)] =
-          (uint8_t)((n < P.N && d < P.D) ? qbyte(p4v_quant_plain(x[i], dB1, fB1, rB1, false, 0.f, P.B1_lo, P.B1_hi)) : 0u);
+          (uint8_t)((n < P.N && d < P.D) ? p4v_qbyte(p4v_quant_plain(x[i], dB1, fB1, rB1, false, 0.f, P.B1_lo, P.B1_hi)) : 0u);
     }
   }
 #pragma unroll 1
@@ -144,10 +117,10 @@ __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_
     uint32_t w[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
     for (int e = 0; e < 16; ++e)
-      if (d < P.D && kb + e < P.N) w[e >> 2] |= qbyte(p4v_quant_plain(x[e], dB2, fB2, rB2, false, 0.f, P.B2_lo, P.B2_hi)) << ((e & 3) * 8);
+      if (d < P.D && kb + e < P.N) w[e >> 2] |= p4v_qbyte(p4v_quant_plain(x[e], dB2, fB2, rB2, false, 0.f, P.B2_lo, P.B2_hi)) << ((e & 3) * 8);
     *reinterpret_cast<uint4*>(sV + (kb / 16 * 64 + d) * 16) = make_uint4(w[0], w[1], w[2], w[3]);
   }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma (async proxy) reads
+  fence_proxy_async();   // generic-proxy stores -> wgmma (async proxy) reads
   __syncthreads();
 
   // ---- 2. matmul1 and the module's operations on the scores
@@ -162,7 +135,8 @@ __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_
     wg_fence();
 #pragma unroll 1
     for (int ks = 0; ks < P.kd / 32; ++ks)
-      mma_k32(acc, mm_desc(base + L.q + ks * 2 * kRows * 16, kRows), mm_desc(base + L.k + (c * 64 + ks * 2 * P.sp) * 16, P.sp));
+      wgmma_n64_k32(acc, make_desc(base + L.q + ks * 2 * kRows * 16, kRows),
+                    make_desc(base + L.k + (c * 64 + ks * 2 * P.sp) * 16, P.sp), 1u);
     wg_commit();
     wg_wait0();
 #pragma unroll
@@ -218,15 +192,15 @@ __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_
         const float pr = __fdiv_rn(x[it], sum);
         uint8_t* dst = sP + ((j >> 4) * kRows + r) * 16 + (j & 15);
         if (SOS) {
-          dst[0] = (uint8_t)(in ? qbyte(p4v_quant_sos(pr, split, P.qm1, 1)) : 0u);
-          dst[plane] = (uint8_t)(in ? qbyte(p4v_quant_sos(pr, split, P.qm1, 2)) : 0u);
+          dst[0] = (uint8_t)(in ? p4v_qbyte(p4v_quant_sos(pr, split, P.qm1, 1)) : 0u);
+          dst[plane] = (uint8_t)(in ? p4v_qbyte(p4v_quant_sos(pr, split, P.qm1, 2)) : 0u);
         } else {
-          dst[0] = (uint8_t)(in ? qbyte(p4v_quant_plain(pr, dA2, fA2, rA2, false, 0.f, P.A2_lo, P.A2_hi)) : 0u);
+          dst[0] = (uint8_t)(in ? p4v_qbyte(p4v_quant_plain(pr, dA2, fA2, rA2, false, 0.f, P.A2_lo, P.A2_hi)) : 0u);
         }
       }
     }
   }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  fence_proxy_async();
   __syncthreads();
   if (wg != 0) return;
 
@@ -237,9 +211,9 @@ __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_
   wg_fence();
 #pragma unroll 1
   for (int ks = 0; ks < P.sp / 32; ++ks) {
-    const uint64_t db = mm_desc(base + L.v + ks * 2 * 64 * 16, 64);
-    mma_k32(acc0, mm_desc(base + L.p + ks * 2 * kRows * 16, kRows), db);
-    if constexpr (SOS) mma_k32(acc1, mm_desc(base + L.p + plane + ks * 2 * kRows * 16, kRows), db);
+    const uint64_t db = make_desc(base + L.v + ks * 2 * 64 * 16, 64);
+    wgmma_n64_k32(acc0, make_desc(base + L.p + ks * 2 * kRows * 16, kRows), db, 1u);
+    if constexpr (SOS) wgmma_n64_k32(acc1, make_desc(base + L.p + plane + ks * 2 * kRows * 16, kRows), db, 1u);
   }
   wg_commit();
   wg_wait0();

@@ -25,6 +25,7 @@
 // integer (every partial sum is below 2^24), so the output is bit-identical to p4v_matmul_quant_forward.
 // Shared memory does not depend on S2: any sequence length takes this path.
 #include "forward.cuh"
+#include "sm90.cuh"
 #include <climits>
 
 namespace {
@@ -41,36 +42,18 @@ template <int BN, bool SOS> struct MMLayout {
   static constexpr int smem = (2 * stage > out_bytes ? 2 * stage : out_bytes) + 128;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
-// K-major, no swizzle: LBO = rows x 16 B between the 16-byte K chunks, SBO = 128 B between 8-row groups
-__device__ __forceinline__ uint64_t mm_desc(uint32_t addr, uint32_t rows) {
-  return (uint64_t)((addr & 0x3FFFF) >> 4) | ((uint64_t)((rows * 16) >> 4) << 16) | ((uint64_t)(128 >> 4) << 32);
-}
-__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-
-#define MM_D32                                                                                                      \
-  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29," \
-  "%30,%31}"
-#define MM_D64                                                                                                      \
-  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29," \
-  "%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,"    \
-  "%57,%58,%59,%60,%61,%62,%63}"
-#define MM_OP8(i) "+r"(d[i]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3]), "+r"(d[i + 4]), "+r"(d[i + 5]), "+r"(d[i + 6]), "+r"(d[i + 7])
-#define MM_OP32 MM_OP8(0), MM_OP8(8), MM_OP8(16), MM_OP8(24)
-#define MM_OP64 MM_OP32, MM_OP8(32), MM_OP8(40), MM_OP8(48), MM_OP8(56)
-
-// D[64 rows][BN cols] += A[64][32 int8 of K] * B[BN][32 int8 of K]^T
-// (the accumulators start at 0: scale-d is always set)
+// D[64 rows][BN cols] += A[64][32 int8 of K] * B[BN][32 int8 of K]^T.  The accumulators start at 0, so scale-d is the
+// constant 1 here rather than the register predicate of wgmma_k32 / wgmma_n64_k32 (sm90.cuh): with a register, ptxas
+// allocates forward_mm_kernel<64, false> differently.
 __device__ __forceinline__ void mma_k32(uint32_t (&d)[64], uint64_t da, uint64_t db) {
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 " MM_D64 ", %64, %65, p;\n\t}" : MM_OP64 : "l"(da), "l"(db));
+               "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 " P4V_WG_D64 ", %64, %65, p;\n\t}"
+               : P4V_WG_OP64(P4V_R) : "l"(da), "l"(db));
 }
 __device__ __forceinline__ void mma_k32(uint32_t (&d)[32], uint64_t da, uint64_t db) {
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 " MM_D32 ", %32, %33, p;\n\t}" : MM_OP32 : "l"(da), "l"(db));
+               "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 " P4V_WG_D32 ", %32, %33, p;\n\t}"
+               : P4V_WG_OP32(P4V_R) : "l"(da), "l"(db));
 }
 
 // Two CTAs per SM (128 registers) overlap one tile's quantisation with another's MMAs and stores; the split-of-softmax
@@ -97,15 +80,9 @@ __global__ void __launch_bounds__(kThreads, (SOS && BN == 128) ? 1 : 2) forward_
   const bool fastA = p4v_rint_div_ok(dA), fastB = p4v_rint_div_ok(dB);
   const float rcpA = fastA ? __frcp_rn(dA) : 0.f, rcpB = fastB ? __frcp_rn(dB) : 0.f;
   const float split = SOS ? __ldg(P.split) : 0.f;
-  auto qB = [&](float v) -> uint32_t {
-    float q = p4v_quant_plain(v, dB, fastB, rcpB, false, 0.f, P.B_lo, P.B_hi);
-    if (!(q == q)) q = 0.f;               // NaN (0/0) cannot be represented in the integer operand
-    return (uint32_t)((int)q & 0xff);
-  };
-  auto qA = [&](float v, int part) -> uint32_t {
-    float q = SOS ? p4v_quant_sos(v, split, P.qm1, part) : p4v_quant_plain(v, dA, fastA, rcpA, false, 0.f, P.A_lo, P.A_hi);
-    if (!(q == q)) q = 0.f;
-    return (uint32_t)((int)q & 0xff);
+  auto qB = [&](float v) { return p4v_qbyte(p4v_quant_plain(v, dB, fastB, rcpB, false, 0.f, P.B_lo, P.B_hi)); };
+  auto qA = [&](float v, int part) {
+    return p4v_qbyte(SOS ? p4v_quant_sos(v, split, P.qm1, part) : p4v_quant_plain(v, dA, fastA, rcpA, false, 0.f, P.A_lo, P.A_hi));
   };
 
   // quantise K slab s into stage `buf`; elements outside the problem are 0 (not the quantised 0: the high
@@ -188,7 +165,7 @@ __global__ void __launch_bounds__(kThreads, (SOS && BN == 128) ? 1 : 2) forward_
 
   const int n_slabs = (P.S2 + kSlab - 1) / kSlab;
   load_slab(0, 0);
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma (async proxy) reads
+  fence_proxy_async();   // generic-proxy stores -> wgmma (async proxy) reads
   __syncthreads();
   const uint32_t base = smem_u32(smem);
   for (int s = 0; s < n_slabs; ++s) {
@@ -196,13 +173,13 @@ __global__ void __launch_bounds__(kThreads, (SOS && BN == 128) ? 1 : 2) forward_
     wg_fence();
 #pragma unroll
     for (int k = 0; k < 2; ++k) {             // +32 bytes of K = 2 chunks
-      mma_k32(acc0, mm_desc(sa + k * 2 * kAPlane / 4, P4V_TILE), mm_desc(sb + k * 2 * BN * 16, BN));
-      if constexpr (SOS) mma_k32(acc1, mm_desc(sa + kAPlane + k * 2 * kAPlane / 4, P4V_TILE), mm_desc(sb + k * 2 * BN * 16, BN));
+      mma_k32(acc0, make_desc(sa + k * 2 * kAPlane / 4, P4V_TILE), make_desc(sb + k * 2 * BN * 16, BN));
+      if constexpr (SOS) mma_k32(acc1, make_desc(sa + kAPlane + k * 2 * kAPlane / 4, P4V_TILE), make_desc(sb + k * 2 * BN * 16, BN));
     }
     wg_commit();
     if (s + 1 < n_slabs) load_slab(s + 1, (s + 1) & 1);   // under the MMAs of slab s
     wg_wait0();
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    fence_proxy_async();
     __syncthreads();                           // slab s + 1 visible; every warpgroup is done with stage s & 1
   }
 

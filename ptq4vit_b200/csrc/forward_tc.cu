@@ -17,9 +17,9 @@
 //      r = -bias, r = fmaf(-scale[g][col / 16], (float)acc, r) in the step's group order, out = -r.  Same integers, same
 //      fp32 operations in the same order: the output is bit-identical to p4v_linear_quant_forward.
 // 288 threads leave 224 registers per thread without setmaxnreg; the bounded mbarrier wait is inline, and the k32 steps of
-// a stage are one straight-line batch selected by a warp-uniform count (ptxas C7520, see sweep_tc.cu).
+// a stage are one straight-line batch selected by a warp-uniform count (ptxas C7520, see sm90.cuh).
 #include "forward.cuh"
-#include <cstdio>
+#include "sm90.cuh"
 
 namespace {
 
@@ -37,97 +37,6 @@ struct FwdCtl {
   unsigned long long empty[P4V_FWD_MAX_STAGES];
 };
 static_assert(sizeof(FwdCtl) + 256 <= P4V_FWD_CTL_BYTES, "control block outgrew its shared-memory reserve");
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void mbar_init(void* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(void* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool mbar_try(uint32_t addr, uint32_t parity) {
-  uint32_t ok;
-  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-               : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
-  return ok != 0;
-}
-// Bounded: a protocol bug traps, never hangs (~10 s of SM clocks).  Inline; on timeout (block << 32 | thread << 20 |
-// barrier smem address) is left in g_forward_timeout, and printed with -DP4V_SWEEP_DEBUG_PRINTF.
-__device__ unsigned long long g_forward_timeout;
-[[noreturn]] __device__ __forceinline__ void mbar_timeout(uint32_t addr, uint32_t parity) {
-  g_forward_timeout = ((unsigned long long)blockIdx.x << 32) | ((unsigned long long)threadIdx.x << 20) | (addr & 0xFFFFFu);
-  __threadfence();
-#ifdef P4V_SWEEP_DEBUG_PRINTF
-  printf("ptq4vit forward: mbarrier wait timed out (block %d thread %d smem 0x%x parity %u)\n", (int)blockIdx.x,
-         (int)threadIdx.x, addr, parity);
-#endif
-  __trap();
-  while (true) {}
-}
-__device__ __forceinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity) {
-  const long long t0 = clock64();
-  while (!mbar_try(addr, parity))
-    if (clock64() - t0 > 20000000000ll) mbar_timeout(addr, parity);
-}
-__device__ __forceinline__ void mbar_wait_addr(uint32_t addr, uint32_t parity) {
-  if (!mbar_try(addr, parity)) mbar_wait_slow(addr, parity);
-}
-__device__ __forceinline__ void mbar_expect_tx_addr(uint32_t addr, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(addr), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s_addr(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void warp_arrive(void* bar, int lane) {
-  __syncwarp();
-  if (lane == 0) mbar_arrive(bar);
-}
-
-// K-major, no swizzle (the canonical layout of common.cuh): LBO = 128 rows x 16 B between the 16-byte K chunks,
-// SBO = 128 B between 8-row groups; the 14-bit start address (16-byte units) is added per use.
-__device__ __forceinline__ uint64_t desc_const() {
-  constexpr uint64_t lbo = (P4V_TILE * 16) >> 4, sbo = 128 >> 4;
-  return (lbo << 16) | (sbo << 32);
-}
-__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-
-#define P4V_WG_D64                                                                                                 \
-  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29," \
-  "%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,"    \
-  "%57,%58,%59,%60,%61,%62,%63}"
-#define P4V_WG_OP8(i) "+r"(d[i]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3]), "+r"(d[i + 4]), "+r"(d[i + 5]), "+r"(d[i + 6]), "+r"(d[i + 7])
-#define P4V_WG_OP64 P4V_WG_OP8(0), P4V_WG_OP8(8), P4V_WG_OP8(16), P4V_WG_OP8(24), P4V_WG_OP8(32), P4V_WG_OP8(40), P4V_WG_OP8(48), P4V_WG_OP8(56)
-
-// D[64 rows][128 cols] (+)= A[64][32 int8 of K] * B[128][32 int8 of K]^T, both K-major in shared memory.
-__device__ __forceinline__ void wgmma_k32(uint32_t (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 " P4V_WG_D64 ", %64, %65, p;\n\t}"
-               : P4V_WG_OP64 : "l"(da), "l"(db), "r"(accumulate));
-}
-template <int N>
-__device__ __forceinline__ void wgmma_seq(uint32_t (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
-  wgmma_k32(d, da, db, accumulate);
-#pragma unroll
-  for (int k = 1; k < N; ++k) wgmma_k32(d, da + 256 * k, db + 256 * k, 1u);   // +32 bytes of K = 2 x 128 rows x 16 B
-}
-__device__ __forceinline__ void wgmma_stage(uint32_t (&d)[64], uint32_t nk, uint64_t da, uint64_t db, uint32_t accumulate) {
-  wg_fence();
-  switch (nk) {
-    case 1: wgmma_seq<1>(d, da, db, accumulate); break;
-    case 2: wgmma_seq<2>(d, da, db, accumulate); break;
-    case 3: wgmma_seq<3>(d, da, db, accumulate); break;
-    default: wgmma_seq<4>(d, da, db, accumulate); break;
-  }
-  wg_commit();
-}
 
 // 16 quantised values -> one 16-byte chunk of int8
 __device__ __forceinline__ void pack16(uint32_t (&w)[4], int e, float q) {
@@ -158,7 +67,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
   }
   if (threadIdx.x == 0) {
     for (uint32_t i = 0; i < nst; ++i) { mbar_init(&S.full[i], 1); mbar_init(&S.empty[i], kConsumerWarps); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
   }
   __syncthreads();
 
@@ -203,7 +112,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
       *reinterpret_cast<uint4*>(dst) = make_uint4(wp[0], wp[1], wp[2], wp[3]);
       if (P.twin) *reinterpret_cast<uint4*>(dst + P.plane_bytes) = make_uint4(wn[0], wn[1], wn[2], wn[3]);
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma (async proxy) reads
+    fence_proxy_async();   // generic-proxy stores -> wgmma (async proxy) reads
   }
   __syncthreads();
 
@@ -232,7 +141,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
   const int wg = et >> 7;                            // row half of the tile
   const int frow = warp * 16 + (lane >> 2);          // fragment rows frow, frow + 8 (inside the tile)
   const int fcol = 2 * (lane & 3);                   // fragment columns 8 * i + fcol + {0, 1}
-  const uint64_t dconst = desc_const();
+  const uint64_t dconst = desc_const(P4V_TILE);
   const uint32_t sC16 = sC >> 4;
   const uint32_t resA16 = ((resA & 0x3FFFF) >> 4) + wg * 64, ring16 = (ring & 0x3FFFF) >> 4;   // +64 rows x 16 B
   const uint32_t full0 = smem_u32(&S.full[0]);

@@ -13,7 +13,7 @@
 // Roles: warp 0 = bulk-copy producer; warpgroups 1-2 = consumers, each issuing wgmma m64n128 for 64 of the 128 output
 // channels of the tile.
 #include "gram.cuh"
-#include <cstdio>
+#include "sm90.cuh"
 
 namespace {
 
@@ -29,77 +29,6 @@ struct Ctl {
   alignas(8) unsigned long long full[kStages], empty[kStages];
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void mbar_init(void* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ bool mbar_try(uint32_t addr, uint32_t parity) {
-  uint32_t ok;
-  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-               : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
-  return ok != 0;
-}
-// Bounded: a protocol bug traps, never hangs.  Inline and call-free (a call splits the wgmma pipeline, C7510); on timeout
-// (block << 32 | thread << 20 | barrier smem address) is left in g_gram_timeout, and printed with -DP4V_SWEEP_DEBUG_PRINTF.
-__device__ unsigned long long g_gram_timeout;
-[[noreturn]] __device__ __forceinline__ void mbar_timeout(uint32_t addr, uint32_t parity) {
-  g_gram_timeout = ((unsigned long long)blockIdx.x << 32) | ((unsigned long long)threadIdx.x << 20) | (addr & 0xFFFFFu);
-  __threadfence();
-#ifdef P4V_SWEEP_DEBUG_PRINTF
-  printf("ptq4vit gram gemm: mbarrier wait timed out (block %d thread %d smem 0x%x parity %u)\n", (int)blockIdx.x,
-         (int)threadIdx.x, addr, parity);
-#endif
-  __trap();
-  while (true) {}
-}
-__device__ __forceinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity) {
-  const long long t0 = clock64();
-  while (!mbar_try(addr, parity))
-    if (clock64() - t0 > 20000000000ll) mbar_timeout(addr, parity);
-}
-__device__ __forceinline__ void mbar_wait(void* bar, uint32_t parity) {
-  const uint32_t addr = smem_u32(bar);
-  if (!mbar_try(addr, parity)) mbar_wait_slow(addr, parity);
-}
-__device__ __forceinline__ void mbar_arrive(void* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(void* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, void* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-// K-major, no swizzle (same canonical layout as the sweep kernel): core matrix = 8 rows x 16 B, SBO = 128 B between
-// 8-row groups, LBO = 128 rows x 16 B between the 16-byte K chunks of a stage tile.
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  constexpr uint64_t lbo = (128 * 16) >> 4, sbo = 128 >> 4;
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (lbo << 16) | (sbo << 32);
-}
-__device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
-      "%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,"
-      "%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(da), "l"(db), "r"(accumulate));
-}
-
 __global__ void __launch_bounds__(kThreads, 1) gram_gemm_kernel(const __grid_constant__ GramGemmArgs a) {
   extern __shared__ uint8_t smem_raw[];
   // 128-byte aligned base, formed by pointer arithmetic on the __shared__ array (not an integer round trip) so that
@@ -110,7 +39,7 @@ __global__ void __launch_bounds__(kThreads, 1) gram_gemm_kernel(const __grid_con
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) { mbar_init(&S.full[i], 1); mbar_init(&S.empty[i], kConsumerWarps); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
   }
   __syncthreads();
   const int tiles = a.tiles_o * a.tiles_p * 2;                      // (output-channel tile, pair tile, pair half)
@@ -176,26 +105,25 @@ __global__ void __launch_bounds__(kThreads, 1) gram_gemm_kernel(const __grid_con
       const uint32_t k0 = ch * kStageKB, kb = (term - k0 < kStageKB) ? term - k0 : kStageKB;
       mbar_wait(&S.full[stage], phase);
       const uint32_t s0 = ring + stage * kStageBytes;
-      const uint64_t rhi = make_desc(s0) + a_off, rlo = make_desc(s0 + kTerm) + a_off;
-      const uint64_t chi = make_desc(s0 + 2 * kTerm), clo = make_desc(s0 + 3 * kTerm);
+      const uint64_t rhi = make_desc(s0, 128) + a_off, rlo = make_desc(s0 + kTerm, 128) + a_off;
+      const uint64_t chi = make_desc(s0 + 2 * kTerm, 128), clo = make_desc(s0 + 3 * kTerm, 128);
       // one K step = 16 bf16 = two 16-byte chunks; a stage holds two (kb = 64) or, at the end of a term, one (kb = 32).
       // Each case is one straight-line batch: a loop or branch between the wgmmas of a batch makes ptxas wait for each
       // one before issuing the next (C7520).
       auto kstep = [&](const uint32_t ks, const uint32_t accumulate) {
         const uint64_t k16 = ks * ((2u * 128 * 16) >> 4);
-        wgmma_bf16(acc, rhi + k16, chi + k16, accumulate);
-        wgmma_bf16(acc, rhi + k16, clo + k16, 1u);
-        wgmma_bf16(acc, rlo + k16, chi + k16, 1u);
+        wgmma_k32(acc, rhi + k16, chi + k16, accumulate);
+        wgmma_k32(acc, rhi + k16, clo + k16, 1u);
+        wgmma_k32(acc, rlo + k16, chi + k16, 1u);
       };
       // (the count is broadcast from lane 0 after the per-lane spin wait, so that ptxas can prove the branch warp-uniform)
       const bool two = __shfl_sync(0xffffffffu, kb == kStageKB ? 1 : 0, 0) != 0;
-      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+      wg_fence();
       if (two) { kstep(0, first ? 0u : 1u); kstep(1, 1u); }
       else     { kstep(0, first ? 0u : 1u); }
-      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-      asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&S.empty[stage]);
+      wg_commit();
+      wg_wait0();
+      warp_arrive(&S.empty[stage], lane);
       if (++stage == kStages) { stage = 0; phase ^= 1; }
       if (last) {
 #pragma unroll

@@ -26,8 +26,8 @@
 // bounded mbarrier wait is inline and the scheduler divides in 32 bits.  The k32 steps of a stage are issued as one
 // straight-line batch selected by a warp-uniform count, so ptxas pipelines them instead of waiting on each (C7520).
 #include "common.cuh"
+#include "sm90.cuh"
 #include <algorithm>
-#include <cstdio>
 #include <cstdlib>
 #include <type_traits>
 
@@ -56,60 +56,6 @@ struct SmemCtl {
   unsigned long long cres_full, cres_empty;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-__device__ __forceinline__ void mbar_init(void* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(void* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(void* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool mbar_try(uint32_t addr, uint32_t parity) {
-  uint32_t ok;
-  asm volatile("{\n\t.reg .pred p;\n\t"
-               "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-               "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
-  return ok != 0;
-}
-// Bounded wait: a protocol bug must surface as a trapped launch (cudaErrorLaunchFailure), never as a hung GPU.  The bound
-// is ~10 s of SM clocks: clock64 keeps counting while a context is time-sliced, a legitimate wait of a sub-millisecond
-// kernel must never reach it.  The wait is inline and makes no call: a call anywhere in the kernel makes ptxas ignore
-// setmaxnreg (C7507).  On timeout it leaves (block << 32 | thread << 20 | barrier smem address) in g_sweep_timeout for
-// a debugger-free post-mortem; building with -DP4V_SWEEP_DEBUG_PRINTF also prints it.
-__device__ unsigned long long g_sweep_timeout;
-[[noreturn]] __device__ __forceinline__ void mbar_timeout(uint32_t addr, uint32_t parity) {
-  g_sweep_timeout = ((unsigned long long)blockIdx.x << 32) | ((unsigned long long)threadIdx.x << 20) | (addr & 0xFFFFFu);
-  __threadfence();
-#ifdef P4V_SWEEP_DEBUG_PRINTF
-  printf("ptq4vit sweep: mbarrier wait timed out (block %d thread %d smem 0x%x parity %u)\n",
-         (int)blockIdx.x, (int)threadIdx.x, addr, parity);
-#endif
-  __trap();
-  while (true) {}
-}
-__device__ __forceinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity) {
-  const long long t0 = clock64();
-  while (!mbar_try(addr, parity))
-    if (clock64() - t0 > 20000000000ll) mbar_timeout(addr, parity);
-}
-__device__ __forceinline__ void mbar_wait_addr(uint32_t addr, uint32_t parity) {
-  if (!mbar_try(addr, parity)) mbar_wait_slow(addr, parity);
-}
-__device__ __forceinline__ void mbar_wait(void* bar, uint32_t parity) { mbar_wait_addr(smem_u32(bar), parity); }
-__device__ __forceinline__ void mbar_expect_tx_addr(uint32_t addr, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(addr), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s_addr(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, void* bar) {
-  bulk_g2s_addr(dst, src, bytes, smem_u32(bar));
-}
 // Phase clocks (build with -DP4V_SWEEP_PHASE_CLOCKS, tools/sweep_phases.py): consumer warp 0 of each warpgroup and the
 // producer add their clock64() cycles per phase into g_sweep_phases[kernel instantiation][phase]; p4v_sweep_phase_clocks
 // reads them back.  Without the flag PhaseClock is empty and the kernel compiles to the same code as without it.
@@ -143,88 +89,9 @@ struct PhaseClock {
 };
 #endif
 
-// Warp-uniform single-lane election for the bulk copies.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-// One consumer warp's arrival (count kConsumerWarps) once all its lanes are past the point being signalled.
-__device__ __forceinline__ void warp_arrive(void* bar, int lane) {
-  __syncwarp();
-  if (lane == 0) mbar_arrive(bar);
-}
-
-// ---- wgmma ----------------------------------------------------------------------------------------
-// K-major, no swizzle: core matrix = 8 rows x 16 B; LBO = stride between the 16-byte chunks of K (128 rows x 16 B),
-// SBO = stride between 8-row groups (128 B).  Descriptor with the constant fields only; the 14-bit start-address field
-// (bits 0..13, units of 16 B) is added per use.
-__device__ __forceinline__ uint64_t desc_const() {
-  constexpr uint64_t lbo = (P4V_TILE * 16) >> 4, sbo = 128 >> 4;
-  return (lbo << 16) | (sbo << 32);
-}
-__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-
-#define P4V_WG_D64                                                                                                 \
-  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29," \
-  "%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,"    \
-  "%57,%58,%59,%60,%61,%62,%63}"
-#define P4V_WG_OP8(C, i) C(d[i]), C(d[i + 1]), C(d[i + 2]), C(d[i + 3]), C(d[i + 4]), C(d[i + 5]), C(d[i + 6]), C(d[i + 7])
-#define P4V_WG_OP64(C) P4V_WG_OP8(C, 0), P4V_WG_OP8(C, 8), P4V_WG_OP8(C, 16), P4V_WG_OP8(C, 24), P4V_WG_OP8(C, 32), \
-                       P4V_WG_OP8(C, 40), P4V_WG_OP8(C, 48), P4V_WG_OP8(C, 56)
-#define P4V_F(x) "+f"(x)
-#define P4V_R(x) "+r"(x)
-
-// D[64 rows][128 cols] (+)= A[64][32 bytes of K] * B[128][32 bytes of K]^T, both K-major in shared memory.
-__device__ __forceinline__ void wgmma_k32(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " P4V_WG_D64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
-               : P4V_WG_OP64(P4V_F) : "l"(da), "l"(db), "r"(accumulate));
-}
-__device__ __forceinline__ void wgmma_k32(uint32_t (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 " P4V_WG_D64 ", %64, %65, p;\n\t}"
-               : P4V_WG_OP64(P4V_R) : "l"(da), "l"(db), "r"(accumulate));
-}
-// One stage = nk (1..4) k32 steps, issued as one committed batch.  Each count has its own straight-line sequence: a
-// data-dependent branch between the wgmmas of a batch makes ptxas wait for each one before issuing the next (C7520).
-template <int N, typename AccT>
-__device__ __forceinline__ void wgmma_seq(AccT (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
-  wgmma_k32(d, da, db, accumulate);
-#pragma unroll
-  for (int k = 1; k < N; ++k) wgmma_k32(d, da + 256 * k, db + 256 * k, 1u);   // +32 bytes of K = 2 x 128 rows x 16 B
-}
-template <typename AccT>
-__device__ __forceinline__ void wgmma_stage(AccT (&d)[64], uint32_t nk, uint64_t da, uint64_t db, uint32_t accumulate) {
-  wg_fence();
-  switch (nk) {
-    case 1: wgmma_seq<1>(d, da, db, accumulate); break;
-    case 2: wgmma_seq<2>(d, da, db, accumulate); break;
-    case 3: wgmma_seq<3>(d, da, db, accumulate); break;
-    default: wgmma_seq<4>(d, da, db, accumulate); break;
-  }
-  wg_commit();
-}
-
-// Pair steps: one column half at a time.  D[64 rows][64 cols] (+)= A[64][32 bytes of K] * B[64][32 bytes of K]^T.
-#define P4V_WG_D32                                                                                                 \
-  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29," \
-  "%30,%31}"
-#define P4V_WG_OP32(C) P4V_WG_OP8(C, 0), P4V_WG_OP8(C, 8), P4V_WG_OP8(C, 16), P4V_WG_OP8(C, 24)
-__device__ __forceinline__ void wgmma_n64_k32(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " P4V_WG_D32 ", %32, %33, p, 1, 1, 0, 0;\n\t}"
-               : P4V_WG_OP32(P4V_F) : "l"(da), "l"(db), "r"(accumulate));
-}
-__device__ __forceinline__ void wgmma_n64_k32(uint32_t (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 " P4V_WG_D32 ", %32, %33, p;\n\t}"
-               : P4V_WG_OP32(P4V_R) : "l"(da), "l"(db), "r"(accumulate));
-}
-// One stage of a pair step: the same nk k32 steps of the shared column slab against both row parts (d0: part 0, d1:
-// part 1), one committed straight-line batch per count as in wgmma_stage.
+// Pair steps run one column half at a time (wgmma m64n64).  One stage of a pair step: the same nk k32 steps of the
+// shared column slab against both row parts (d0: part 0, d1: part 1), one committed straight-line batch per count as in
+// wgmma_stage.
 template <int N, typename AccT>
 __device__ __forceinline__ void wgmma_pair_seq(AccT (&d0)[32], AccT (&d1)[32], uint64_t da0, uint64_t da1, uint64_t db,
                                                uint32_t accumulate) {
@@ -354,7 +221,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
     for (uint32_t i = 0; i < nst; ++i) { mbar_init(&S.full[i], 1); mbar_init(&S.empty[i], kConsumerWarps); }
     for (int i = 0; i < 2; ++i) { mbar_init(&S.res_full[i], 1); mbar_init(&S.res_empty[i], kConsumerWarps); }
     mbar_init(&S.cres_full, 1); mbar_init(&S.cres_empty, kConsumerWarps);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
   }
   __syncthreads();
 
@@ -436,7 +303,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
   const int frow = cw * 16 + (lane >> 2);            // fragment rows frow, frow + 8 (inside the tile)
   const int fcol = 2 * (lane & 3);                   // fragment columns 8 * i + fcol + {0, 1}
   const float gs = (P.out && !P.out_residual) ? 1.f : *P.gscale;
-  const uint64_t dconst = desc_const();
+  const uint64_t dconst = desc_const(P4V_TILE);
   const uint32_t sR16 = sR >> 4, sC16 = sC >> 4;
   const uint32_t ringR16 = ((ringR & 0x3FFFF) >> 4) + wg * 64, ringC16 = (ringC & 0x3FFFF) >> 4;   // +64 rows x 16 B
   const uint32_t resC16 = (resC & 0x3FFFF) >> 4;
