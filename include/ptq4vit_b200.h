@@ -187,7 +187,8 @@ P4V_API int p4v_matmul_frozen_forward(const p4v_matmul_desc* d, const float* A, 
  *   bias       [heads, N, N] contiguous, added to the scores, or NULL;
  *   mask       [n_windows, N, N] contiguous, added after the bias to image b's scores from window b % n_windows, or NULL.
  *   out        [batch, N, heads * head_dim] contiguous, 8-byte aligned.
- * Shapes: N <= 256 (the scores of one query tile stay in shared memory), head_dim a multiple of 16, at most 64.
+ * Shapes: N <= 256 (the scores of one query tile stay in shared memory; p4v_attention_frozen_forward_long below takes
+ * ViT / DeiT calls up to 1024 tokens), head_dim a multiple of 16, at most 64.
  * p4v_attention_fused_ok says whether a shape qualifies (a pure function of N and head_dim).  Every argument is validated
  * before the launch; no allocation, no copy, no synchronisation: the call can be captured in a CUDA graph. */
 typedef struct p4v_attention_desc {
@@ -203,6 +204,20 @@ P4V_API int p4v_attention_frozen_forward(const p4v_attention_desc* a, const floa
                                  const p4v_matmul_desc* mm1, const void* pack1, size_t pack1_bytes,
                                  const p4v_matmul_desc* mm2, const void* pack2, size_t pack2_bytes,
                                  const float* bias, const float* mask, float* out, void* stream);
+
+/* The same attention core for longer sequences (ViT / DeiT at 384 pixels: 577 tokens), with its own kernel
+ * (csrc/forward_attn_long_tc.cu) and the same bits.  A CTA quantises all keys and v of one (image, head) once and loops
+ * over its 64-row query tiles, recomputing each tile's scores chunk by chunk instead of storing score rows, so shared
+ * memory grows with N only through the quantised k and v.  The arguments are those of p4v_attention_frozen_forward,
+ * validated the same way before the launch, with these differences: 1 <= N <= 1024 (torch's warp softmax, whose sum
+ * order the kernel restates, covers rows of at most 1024 floats), and scale_on_q = 0, no bias, no mask (no windowed
+ * model has more than 256 tokens).  head_dim: a multiple of 16, at most 64.  p4v_attention_long_ok is the shape rule.
+ * One launch; no allocation, no copy, no synchronisation. */
+P4V_API int p4v_attention_long_ok(int32_t tokens, int32_t head_dim, int* ok);
+P4V_API int p4v_attention_frozen_forward_long(const p4v_attention_desc* a, const float* qkv, const long long* qkv_strides,
+                                      const p4v_matmul_desc* mm1, const void* pack1, size_t pack1_bytes,
+                                      const p4v_matmul_desc* mm2, const void* pack2, size_t pack2_bytes,
+                                      const float* bias, const float* mask, float* out, void* stream);
 
 /* The patch-embedding convolution: ChannelwiseBatchingQuantConv2d with a_bit >= 32 (quant_layers/conv.py:444-614, wired
  * by configs/PTQ4ViT.py:52-54): one weight step size per output channel, activations left in FP32.  The caller passes

@@ -66,6 +66,9 @@ _SIGNATURES = {
     "p4v_attention_fused_ok": [C.c_int32, C.c_int32, C.POINTER(C.c_int)],
     "p4v_attention_frozen_forward": [C.POINTER(AttentionDesc), _P, C.POINTER(C.c_longlong), C.POINTER(MatMulDesc), _P, C.c_size_t,
                                      C.POINTER(MatMulDesc), _P, C.c_size_t, _P, _P, _P, _P],
+    "p4v_attention_long_ok": [C.c_int32, C.c_int32, C.POINTER(C.c_int)],
+    "p4v_attention_frozen_forward_long": [C.POINTER(AttentionDesc), _P, C.POINTER(C.c_longlong), C.POINTER(MatMulDesc), _P,
+                                          C.c_size_t, C.POINTER(MatMulDesc), _P, C.c_size_t, _P, _P, _P, _P],
     "p4v_conv_workspace_bytes": [C.POINTER(ConvDesc), C.POINTER(C.c_size_t)],
     "p4v_conv_calibrate": [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P],
     "p4v_export_quantized": [_P, C.c_longlong, C.c_longlong, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,

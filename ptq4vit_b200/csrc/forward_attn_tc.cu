@@ -144,9 +144,7 @@ __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_
       const int r = wrow + (lane >> 2) + 8 * ((e >> 1) & 1), j = c * 64 + 8 * (e >> 2) + 2 * (lane & 3) + (e & 1);
       if (r < rows && j < P.N) {
         const int i = row0 + r;
-        float rr = 0.f;
-        rr = fmaf(-s1, __int2float_rn((int)acc[e]), rr);
-        float s = -rr;
+        float s = p4v_attn_mm1(acc[e], s1);
         if (!P.scale_on_q) s = __fmul_rn(s, P.scale);
         if (P.bias) s = __fadd_rn(s, __ldg(P.bias + ((long long)h * P.N + i) * P.N + j));
         if (P.mask) s = __fadd_rn(s, __ldg(P.mask + ((long long)(img % P.n_windows) * P.N + i) * P.N + j));
@@ -226,10 +224,7 @@ __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_
     float o[2];
 #pragma unroll
     for (int f = 0; f < 2; ++f) {
-      float rr = 0.f;
-      rr = fmaf(-t0, __int2float_rn((int)acc0[e + f]), rr);
-      if constexpr (SOS) rr = fmaf(-t1, __int2float_rn((int)acc1[e + f]), rr);
-      o[f] = -rr;
+      o[f] = p4v_attn_mm2<SOS>(acc0[e + f], SOS ? acc1[e + f] : 0u, t0, t1);
     }
     *reinterpret_cast<float2*>(P.out + ((long long)img * P.N + row0 + r) * C + (long long)h * P.D + col) = make_float2(o[0], o[1]);
   }

@@ -516,36 +516,45 @@ extern "C" int p4v_attention_fused_ok(int32_t tokens, int32_t head_dim, int* ok)
   return 0;
 }
 
-extern "C" int p4v_attention_frozen_forward(const p4v_attention_desc* a, const float* qkv, const long long* qkv_strides,
-                                            const p4v_matmul_desc* mm1, const void* pack1, size_t pack1_bytes,
-                                            const p4v_matmul_desc* mm2, const void* pack2, size_t pack2_bytes,
-                                            const float* bias, const float* mask, float* out, void* stream) {
-  P4V_REQUIRE(a && qkv && qkv_strides && mm1 && pack1 && mm2 && pack2 && out, "attention_frozen_forward: null pointer");
-  P4V_REQUIRE(a->batch > 0 && a->heads > 0 && a->tokens > 0 && a->head_dim > 0, "attention_frozen_forward: empty shape");
+namespace {
+
+// Validates every argument of an attention call and fills the kernel parameters; `long_seq` applies the long kernel's
+// rules (N <= 1024; no q-scaling, bias or mask).
+int attention_params(const p4v_attention_desc* a, const float* qkv, const long long* qkv_strides, const p4v_matmul_desc* mm1,
+                     const void* pack1, size_t pack1_bytes, const p4v_matmul_desc* mm2, const void* pack2, size_t pack2_bytes,
+                     const float* bias, const float* mask, float* out, bool long_seq, FwdAttnParams& q) {
+  const char* fn = long_seq ? "attention_frozen_forward_long" : "attention_frozen_forward";
+  P4V_REQUIRE(a && qkv && qkv_strides && mm1 && pack1 && mm2 && pack2 && out, "%s: null pointer", fn);
+  P4V_REQUIRE(a->batch > 0 && a->heads > 0 && a->tokens > 0 && a->head_dim > 0, "%s: empty shape", fn);
+  const int max_tokens = long_seq ? P4V_ATTN_LONG_MAX_TOKENS : P4V_ATTN_MAX_TOKENS;
   int ok = 0;
-  p4v_attention_fused_ok(a->tokens, a->head_dim, &ok);
-  P4V_REQUIRE(a->tokens <= P4V_ATTN_MAX_TOKENS, "attention_frozen_forward: %d tokens (at most %d)", a->tokens, P4V_ATTN_MAX_TOKENS);
-  P4V_REQUIRE(ok, "attention_frozen_forward: head_dim %d not supported (a multiple of 16, at most %d)", a->head_dim,
-              P4V_ATTN_MAX_DIM);
+  if (long_seq) p4v_attention_long_ok(a->tokens, a->head_dim, &ok);
+  else p4v_attention_fused_ok(a->tokens, a->head_dim, &ok);
+  P4V_REQUIRE(a->tokens <= max_tokens, "%s: %d tokens (at most %d)", fn, a->tokens, max_tokens);
+  P4V_REQUIRE(ok, "%s: head_dim %d not supported (a multiple of 16, at most %d)", fn, a->head_dim, P4V_ATTN_MAX_DIM);
   if (int rc = check_shape(mm1)) return rc;
   if (int rc = check_shape(mm2)) return rc;
   P4V_REQUIRE(mm1->heads == a->heads && mm2->heads == a->heads,
-              "attention_frozen_forward: packs made for %d and %d heads, the call has %d", mm1->heads, mm2->heads, a->heads);
-  P4V_REQUIRE(!mm1->sos, "attention_frozen_forward: matmul1 cannot be split-of-softmax");
+              "%s: packs made for %d and %d heads, the call has %d", fn, mm1->heads, mm2->heads, a->heads);
+  P4V_REQUIRE(!mm1->sos, "%s: matmul1 cannot be split-of-softmax", fn);
   const Packed k1 = packed_layout(mm1), k2 = packed_layout(mm2);
   P4V_REQUIRE(pack1_bytes == k1.bytes && pack2_bytes == k2.bytes,
-              "attention_frozen_forward: pack sizes %zu and %zu, expected %zu and %zu", pack1_bytes, pack2_bytes, k1.bytes, k2.bytes);
-  for (int i = 0; i < 4; ++i) P4V_REQUIRE(qkv_strides[i] >= 0, "attention_frozen_forward: negative stride");
-  P4V_REQUIRE(!a->scale_on_q || a->scale_on_q == 1, "attention_frozen_forward: scale_on_q must be 0 or 1");
+              "%s: pack sizes %zu and %zu, expected %zu and %zu", fn, pack1_bytes, pack2_bytes, k1.bytes, k2.bytes);
+  for (int i = 0; i < 4; ++i) P4V_REQUIRE(qkv_strides[i] >= 0, "%s: negative stride", fn);
+  P4V_REQUIRE(!a->scale_on_q || a->scale_on_q == 1, "%s: scale_on_q must be 0 or 1", fn);
+  if (long_seq) {
+    P4V_REQUIRE(!a->scale_on_q, "%s: scale_on_q is not supported (scores * scale after matmul1 only)", fn);
+    P4V_REQUIRE(bias == nullptr && mask == nullptr && a->n_windows == 0, "%s: bias and mask are not supported", fn);
+  }
   P4V_REQUIRE(mask == nullptr ? a->n_windows == 0 : (a->n_windows > 0 && a->batch % a->n_windows == 0),
-              "attention_frozen_forward: a mask needs n_windows > 0 dividing batch (and no mask n_windows = 0); got %d for batch %d",
+              "%s: a mask needs n_windows > 0 dividing batch (and no mask n_windows = 0); got %d for batch %d", fn,
               a->n_windows, a->batch);
   P4V_REQUIRE(((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(bias) | reinterpret_cast<uintptr_t>(mask)) & 3) == 0,
-              "attention_frozen_forward: qkv, bias and mask must be 4-byte aligned");
-  P4V_REQUIRE((reinterpret_cast<uintptr_t>(out) & 7) == 0, "attention_frozen_forward: out must be 8-byte aligned");
+              "%s: qkv, bias and mask must be 4-byte aligned", fn);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(out) & 7) == 0, "%s: out must be 8-byte aligned", fn);
   P4V_REQUIRE(((reinterpret_cast<uintptr_t>(pack1) | reinterpret_cast<uintptr_t>(pack2)) & 15) == 0,
-              "attention_frozen_forward: packs must be 16-byte aligned");
-  FwdAttnParams q{};
+              "%s: packs must be 16-byte aligned", fn);
+  q = FwdAttnParams{};
   q.qkv = qkv; q.s_b = qkv_strides[0]; q.s_n = qkv_strides[1]; q.s_p = qkv_strides[2]; q.s_h = qkv_strides[3];
   q.out = out;
   q.batch = a->batch; q.heads = a->heads; q.N = a->tokens; q.D = a->head_dim;
@@ -560,5 +569,34 @@ extern "C" int p4v_attention_frozen_forward(const p4v_attention_desc* a, const f
   q.scale2 = at<float>(p2, k2.o_scale);
   q.A2_lo = (float)-A2; q.A2_hi = (float)(A2 - 1); q.B2_lo = (float)-B2; q.B2_hi = (float)(B2 - 1);
   q.qm1 = (float)(A2 - 1);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int p4v_attention_frozen_forward(const p4v_attention_desc* a, const float* qkv, const long long* qkv_strides,
+                                            const p4v_matmul_desc* mm1, const void* pack1, size_t pack1_bytes,
+                                            const p4v_matmul_desc* mm2, const void* pack2, size_t pack2_bytes,
+                                            const float* bias, const float* mask, float* out, void* stream) {
+  FwdAttnParams q;
+  if (int rc = attention_params(a, qkv, qkv_strides, mm1, pack1, pack1_bytes, mm2, pack2, pack2_bytes, bias, mask, out, false, q))
+    return rc;
   return p4v_launch_forward_attn_tc(q, mm2->sos != 0, (cudaStream_t)stream);
+}
+
+// ---- the long-sequence variant (forward_attn_long_tc.cu) ---------------------------------------------------------
+extern "C" int p4v_attention_long_ok(int32_t tokens, int32_t head_dim, int* ok) {
+  P4V_REQUIRE(ok != nullptr, "null output");
+  *ok = tokens > 0 && tokens <= P4V_ATTN_LONG_MAX_TOKENS && head_dim > 0 && head_dim <= P4V_ATTN_MAX_DIM && head_dim % 16 == 0;
+  return 0;
+}
+
+extern "C" int p4v_attention_frozen_forward_long(const p4v_attention_desc* a, const float* qkv, const long long* qkv_strides,
+                                                 const p4v_matmul_desc* mm1, const void* pack1, size_t pack1_bytes,
+                                                 const p4v_matmul_desc* mm2, const void* pack2, size_t pack2_bytes,
+                                                 const float* bias, const float* mask, float* out, void* stream) {
+  FwdAttnParams q;
+  if (int rc = attention_params(a, qkv, qkv_strides, mm1, pack1, pack1_bytes, mm2, pack2, pack2_bytes, bias, mask, out, true, q))
+    return rc;
+  return p4v_launch_forward_attn_long_tc(q, mm2->sos != 0, (cudaStream_t)stream);
 }

@@ -138,6 +138,17 @@ __device__ __forceinline__ void wgmma_n64_k32(uint32_t (&d)[32], uint64_t da, ui
                "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 " P4V_WG_D32 ", %32, %33, p;\n\t}"
                : P4V_WG_OP32(P4V_R) : "l"(da), "l"(db), "r"(accumulate));
 }
+// D[64 rows][32 cols] (+)= A[64][32 bytes of K] * B[32][32 bytes of K]^T, int8 operands.
+__device__ __forceinline__ void wgmma_n32_k32(uint32_t (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p;\n\t}"
+               : P4V_WG_OP8(P4V_R, 0), P4V_WG_OP8(P4V_R, 8) : "l"(da), "l"(db), "r"(accumulate));
+}
+// Barrier `id` (1..15; 0 is __syncthreads) over `threads` threads, e.g. the 128 of one warpgroup.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 // One stage = nk (1..4) k32 steps of m64n128 over 128-row operand tiles, issued as one committed batch.  Each count has
 // its own straight-line sequence: a data-dependent branch between the wgmmas of a batch makes ptxas wait for each one
 // before issuing the next (C7520).  nk must be provably warp-uniform (callers broadcast it with __shfl_sync).

@@ -234,25 +234,36 @@ class MinMaxQuantMatMul(nn.Module):
         return out
 
 
-def frozen_attention_applies(matmul1, matmul2, tokens, head_dim, *inputs):
+SHORT_ATTENTION_TOKENS = 256      # P4V_ATTN_MAX_TOKENS: the short kernel's limit, and fuse_attention's default
+LONG_ATTENTION_TOKENS = 1024      # P4V_ATTN_LONG_MAX_TOKENS: the long-sequence kernel's limit
+
+
+def frozen_attention_applies(matmul1, matmul2, tokens, head_dim, *inputs, max_tokens=SHORT_ATTENTION_TOKENS):
     """Whether one call of an attention block can run as the fused frozen attention core: both MatMul modules frozen and
-    in quant_forward mode, matmul1 not split-of-softmax, no input that requires grad under grad mode, and a shape the
-    kernel holds (p4v_attention_fused_ok: at most 256 tokens, head_dim a multiple of 16 up to 64)."""
+    in quant_forward mode, matmul1 not split-of-softmax, no input that requires grad under grad mode, and a shape a
+    kernel holds: p4v_attention_fused_ok (at most 256 tokens, head_dim a multiple of 16 up to 64) or, for
+    256 < tokens <= max_tokens, p4v_attention_long_ok (at most 1024 tokens, the same head_dim rule)."""
     if not all(isinstance(m, MinMaxQuantMatMul) and m.frozen and m.mode == "quant_forward" for m in (matmul1, matmul2)):
         return False
     if matmul1.sos or (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in inputs)):
         return False
+    if tokens > max(max_tokens, SHORT_ATTENTION_TOKENS):
+        return False
     ok = ctypes.c_int()
-    _lib.check(_lib.lib().p4v_attention_fused_ok(int(tokens), int(head_dim), ctypes.byref(ok)), "p4v_attention_fused_ok")
+    name = "p4v_attention_fused_ok" if tokens <= SHORT_ATTENTION_TOKENS else "p4v_attention_long_ok"
+    _lib.check(getattr(_lib.lib(), name)(int(tokens), int(head_dim), ctypes.byref(ok)), name)
     return bool(ok.value)
 
 
-def frozen_attention(matmul1, matmul2, qkv, scale, scale_on_q, bias=None, mask=None):
-    """The attention core between the qkv and proj Linears in one kernel (csrc/forward_attn_tc.cu), for a call where
-    frozen_attention_applies holds.  `qkv` is the qkv Linear's output viewed as [B, N, 3, heads, head_dim]; returns
+def frozen_attention(matmul1, matmul2, qkv, scale, scale_on_q, bias=None, mask=None, max_tokens=SHORT_ATTENTION_TOKENS):
+    """The attention core between the qkv and proj Linears in one kernel, for a call where frozen_attention_applies
+    holds: csrc/forward_attn_tc.cu up to 256 tokens, csrc/forward_attn_long_tc.cu for 256 < N <= max_tokens (ViT / DeiT
+    only: no q-scaling, bias or mask).  `qkv` is the qkv Linear's output viewed as [B, N, 3, heads, head_dim]; returns
     matmul2(softmax(S), v).transpose(1, 2).reshape(B, N, C) with S = matmul1(q, k^T) * scale (scale_on_q=False, ViT) or
     matmul1(q * scale, k^T) + bias [+ mask of window b % nW] (scale_on_q=True, Swin), with the bits of that sequence."""
     B, N, _, H, D = qkv.shape
+    if N > max(max_tokens, SHORT_ATTENTION_TOKENS):
+        raise ValueError(f"frozen_attention: {N} tokens, more than max_tokens={max_tokens}")
     p1, p2 = matmul1._frozen_pack(H), matmul2._frozen_pack(H)
     dev = p1.device
     qkv = qkv.to(dev, torch.float32)
@@ -265,10 +276,11 @@ def frozen_attention(matmul1, matmul2, qkv, scale, scale_on_q, bias=None, mask=N
     a.scale_on_q, a.n_windows, a.scale = int(bool(scale_on_q)), 0 if mask is None else int(mask.shape[0]), float(scale)
     d1, d2 = matmul1._desc_dims(1, H, 1, 1, 1), matmul2._desc_dims(1, H, 1, 1, 1)
     out = torch.empty(B, N, H * D, dtype=torch.float32, device=dev)
-    _lib.check(_lib.lib().p4v_attention_frozen_forward(
+    name = "p4v_attention_frozen_forward" if N <= SHORT_ATTENTION_TOKENS else "p4v_attention_frozen_forward_long"
+    _lib.check(getattr(_lib.lib(), name)(
         ctypes.byref(a), _lib.ptr(qkv), (ctypes.c_longlong * 4)(*qkv.stride()[:4]), ctypes.byref(d1), _lib.ptr(p1), p1.numel(),
         ctypes.byref(d2), _lib.ptr(p2), p2.numel(), _lib.ptr(bias), _lib.ptr(mask), _lib.ptr(out),
-        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "p4v_attention_frozen_forward")
+        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), name)
     return out
 
 

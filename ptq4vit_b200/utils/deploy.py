@@ -21,12 +21,14 @@ quant_forward is torch operations on the device and already capturable.
 `fuse_attention(net)` goes one step further for attention blocks whose two MatMul modules are frozen: the whole core
 between the qkv and proj Linears -- matmul1, the scale, bias and mask, the softmax, matmul2 and the transpose to
 [B, N, C] -- runs as one kernel (csrc/forward_attn_tc.cu) with the bits of the unfused sequence, and the score matrix
-never reaches HBM.  It is opt-in; `unfuse_attention(net)` undoes it.
+never reaches HBM.  It is opt-in; `unfuse_attention(net)` undoes it.  `fuse_attention(net, max_tokens=1024)` also fuses
+the ViT / DeiT attention calls of 257 to 1024 tokens (384-pixel models: 577), with a kernel that quantises the keys and
+values of a head once and recomputes the scores instead of storing them (csrc/forward_attn_long_tc.cu).
 """
 import torch
 
 from ..quant_layers.linear import MinMaxQuantLinear
-from ..quant_layers.matmul import MinMaxQuantMatMul
+from ..quant_layers.matmul import LONG_ATTENTION_TOKENS, SHORT_ATTENTION_TOKENS, MinMaxQuantMatMul
 from . import integer
 from .models import Attention, WindowAttention
 
@@ -56,15 +58,23 @@ def unfreeze_model(wrapped_modules):
             m.unfreeze()
 
 
-def fuse_attention(net):
+def fuse_attention(net, max_tokens=SHORT_ATTENTION_TOKENS):
     """Mark every attention module of `net` whose matmul1 and matmul2 are frozen MatMul modules as fused: each call that
     qualifies (no input requiring grad under grad mode, at most 256 tokens, head_dim a multiple of 16 up to 64) runs the
-    fused attention core; any other call runs the modules as before.  Returns the names of the attention modules left
-    unfused because a MatMul module is not frozen."""
+    fused attention core; any other call runs the modules as before.  With max_tokens in (256, 1024], ViT / DeiT
+    `Attention` calls of 256 < N <= max_tokens run fused as well, on the long-sequence kernel (the kernel is chosen from N;
+    Swin's `WindowAttention` keeps the 256-token rule).  Returns the names of the attention modules left unfused because
+    a MatMul module is not frozen."""
+    if isinstance(max_tokens, bool) or not isinstance(max_tokens, int) or \
+            not SHORT_ATTENTION_TOKENS <= max_tokens <= LONG_ATTENTION_TOKENS:
+        raise ValueError(f"fuse_attention: max_tokens must be an int in [{SHORT_ATTENTION_TOKENS}, {LONG_ATTENTION_TOKENS}], "
+                         f"got {max_tokens!r}")
     left = []
     for name, m in net.named_modules():
         if isinstance(m, (Attention, WindowAttention)):
             m.fused = all(isinstance(mm, MinMaxQuantMatMul) and mm.frozen for mm in (m.matmul1, m.matmul2))
+            if isinstance(m, Attention):
+                m.fused_max_tokens = max_tokens
             if not m.fused:
                 left.append(name)
     return left
@@ -74,6 +84,8 @@ def unfuse_attention(net):
     for m in net.modules():
         if isinstance(m, (Attention, WindowAttention)):
             m.fused = False
+        if isinstance(m, Attention):
+            m.fused_max_tokens = SHORT_ATTENTION_TOKENS
 
 
 def _to(v, device):

@@ -24,13 +24,17 @@ class Attention(nn.Module):
         self.matmul2 = MatMul()
 
     fused = False      # set by utils.deploy.fuse_attention: run the frozen attention core as one kernel when it applies
+    fused_max_tokens = 256   # set by utils.deploy.fuse_attention: sequences up to this length run fused (the long
+                             # kernel above 256 tokens)
 
     def forward(self, x):
         B, N, C = x.shape
         y = self.qkv(x)
-        if self.fused and frozen_attention_applies(self.matmul1, self.matmul2, N, C // self.num_heads, y):
+        if self.fused and frozen_attention_applies(self.matmul1, self.matmul2, N, C // self.num_heads, y,
+                                                   max_tokens=self.fused_max_tokens):
             qkv5 = y.reshape(B, N, 3, self.num_heads, C // self.num_heads)
-            return self.proj(frozen_attention(self.matmul1, self.matmul2, qkv5, self.scale, scale_on_q=False))
+            return self.proj(frozen_attention(self.matmul1, self.matmul2, qkv5, self.scale, scale_on_q=False,
+                                              max_tokens=self.fused_max_tokens))
         qkv = y.reshape(B, N, 3, self.num_heads, C // self.num_heads).permute(2, 0, 3, 1, 4)
         q, k, v = qkv.unbind(0)
         attn = self.matmul1(q, k.transpose(-2, -1)) * self.scale

@@ -30,7 +30,7 @@ import torch  # noqa: E402
 import forward_bench as FB  # noqa: E402
 
 
-def _block_pair(m1, m2, qkv5, scale, scale_on_q, bias=None, mask=None):
+def _block_pair(m1, m2, qkv5, scale, scale_on_q, bias=None, mask=None, max_tokens=256):
     """(unfused, fused) callables of one attention core on the frozen modules."""
     from ptq4vit_b200.quant_layers.matmul import frozen_attention
     B, N, _, H, D = qkv5.shape
@@ -50,7 +50,7 @@ def _block_pair(m1, m2, qkv5, scale, scale_on_q, bias=None, mask=None):
         return m2.quant_forward(attn.softmax(dim=-1), v).transpose(1, 2).reshape(B, N, H * D)
 
     def fused():
-        return frozen_attention(m1, m2, qkv5, scale, scale_on_q, bias=bias, mask=mask)
+        return frozen_attention(m1, m2, qkv5, scale, scale_on_q, bias=bias, mask=mask, max_tokens=max_tokens)
     bits = lambda t: t.contiguous().view(torch.int32)
     identical = torch.equal(bits(unfused()), bits(fused()))
     nbytes = 4 * (qkv5.numel() + B * N * H * D + (0 if bias is None else bias.numel()) + (0 if mask is None else mask.numel()))
@@ -163,6 +163,75 @@ def swin_t_stage1(a):
     return out
 
 
+def _minmax_pair(qkv5, scale, m2_cls, bit):
+    """Frozen matmul1 / matmul2 modules with min-max step sizes of this input (split 0.05 for split-of-softmax)."""
+    from ptq4vit_b200.quant_layers import matmul as MM
+    H = qkv5.shape[3]
+    q, k, v = qkv5.permute(2, 0, 3, 1, 4).unbind(0)
+
+    def minmax(m, A, B):
+        amax, bmax = A.abs().amax(dim=(0, 2, 3)), B.abs().amax(dim=(0, 2, 3))
+        m.B_interval = (bmax / (m.B_qmax - 0.5)).view(1, H, 1, 1, 1, 1, 1)
+        if m.sos:
+            m.split = torch.tensor(0.05).cuda()
+            m.A_interval = m.split / (m.A_qmax - 1)
+        else:
+            m.A_interval = (amax / (m.A_qmax - 0.5)).view(1, H, 1, 1, 1, 1, 1)
+        m.calibrated, m.mode = True, "quant_forward"
+        return m.freeze()
+    m1 = minmax(MM.PTQSLBatchingQuantMatMul(A_bit=bit, B_bit=bit), q, k.transpose(-2, -1))
+    m2 = minmax(getattr(MM, m2_cls)(A_bit=bit, B_bit=bit), torch.rand(1, H, 1, 1, device="cuda"), v)
+    return m1, m2
+
+
+def _long_kernel(m1, m2, qkv5, scale):
+    """A callable running p4v_attention_frozen_forward_long on this call, also where frozen_attention would pick the
+    short kernel (N <= 256)."""
+    import ctypes
+
+    from ptq4vit_b200 import _lib
+    B, N, _, H, D = qkv5.shape
+    p1, p2 = m1._frozen_pack(H), m2._frozen_pack(H)
+    a = _lib.AttentionDesc()
+    a.batch, a.tokens, a.heads, a.head_dim, a.scale_on_q, a.n_windows, a.scale = B, N, H, D, 0, 0, scale
+    d1, d2 = m1._desc_dims(1, H, 1, 1, 1), m2._desc_dims(1, H, 1, 1, 1)
+    strides = (ctypes.c_longlong * 4)(*qkv5.stride()[:4])
+
+    def call():
+        out = torch.empty(B, N, H * D, device="cuda")
+        _lib.check(_lib.lib().p4v_attention_frozen_forward_long(
+            ctypes.byref(a), _lib.ptr(qkv5), strides, ctypes.byref(d1), _lib.ptr(p1), p1.numel(), ctypes.byref(d2),
+            _lib.ptr(p2), p2.numel(), None, None, _lib.ptr(out), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)),
+            "p4v_attention_frozen_forward_long")
+        return out
+    return call
+
+
+def long_sequences(a):
+    """ViT-B/384 x 32 blocks (577 tokens, 12 heads of 64): unfused frozen core against the long-sequence kernel; and at
+    ViT-B/224's 197 tokens the short kernel against the long one.  Synthetic qkv output, min-max step sizes."""
+    from ptq4vit_b200.quant_layers.matmul import frozen_attention
+    out = []
+    with torch.no_grad():
+        for N in (577, 197):
+            g = torch.Generator().manual_seed(N)
+            qkv5 = (torch.randn(32, N, 3 * 768, generator=g) * 2.0).cuda().view(32, N, 3, 12, 64)
+            for cls in ("SoSPTQSLBatchingQuantMatMul", "PTQSLBatchingQuantMatMul"):
+                m1, m2 = _minmax_pair(qkv5, 64 ** -0.5, cls, a.bit)
+                unfused, fused, identical, nbytes = _block_pair(m1, m2, qkv5, 64 ** -0.5, False, max_tokens=1024)
+                if N == 577:
+                    out.append(_report(_time_pair(unfused, fused, a), nbytes,
+                                       {"qkv": list(qkv5.shape), "matmul2": cls, "bit_identical": identical}))
+                else:         # the short kernel (fused up to 256 tokens) against the long one, on the same modules
+                    long_ = _long_kernel(m1, m2, qkv5, 64 ** -0.5)
+                    identical = identical and torch.equal(long_().view(torch.int32), unfused().view(torch.int32))
+                    r = _report(_time_pair(fused, long_, a), nbytes, {"qkv": list(qkv5.shape), "matmul2": cls,
+                                                                     "bit_identical": identical})
+                    out.append({"short_kernel_ms": r.pop("unfused_ms"), "long_kernel_ms": r.pop("fused_ms"), **r})
+                del m1, m2
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--images", type=int, default=32, help="calibration images")
@@ -170,14 +239,20 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--window", type=float, default=0.5, help="seconds of calls per timing")
     ap.add_argument("--configs", default="PTQ4ViT,BasePTQ")
+    ap.add_argument("--long-only", action="store_true", help="only the long-sequence blocks")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("tools/attention_bench.py needs a CUDA device (no CPU fallback)")
     torch.cuda.set_device(0)
+    if a.long_only:
+        print(json.dumps({"tool": "attention_bench", "card": FB.card(), "hbm_bytes_per_s_data_sheet": FB.HBM_BYTES_PER_S,
+                          "workload": f"synthetic qkv, min-max step sizes, W{a.bit}A{a.bit}", "long_sequences": long_sequences(a)}))
+        return
     out = {"tool": "attention_bench", "card": FB.card(),
            "workload": f"{FB.MODEL}, synthetic weights, calibrated on {a.images} synthetic imgs, batch 32, W{a.bit}A{a.bit}; "
                        "Swin-T stage 1 windows, synthetic",
            "hbm_bytes_per_s_data_sheet": FB.HBM_BYTES_PER_S,
+           "long_sequences": long_sequences(a),
            "swin_t_stage1": swin_t_stage1(a),
            "vit_b": [vit_config(c, a) for c in a.configs.split(",")]}
     print(json.dumps(out))
