@@ -219,6 +219,31 @@ P4V_API int p4v_attention_frozen_forward_long(const p4v_attention_desc* a, const
                                       const p4v_matmul_desc* mm2, const void* pack2, size_t pack2_bytes,
                                       const float* bias, const float* mask, float* out, void* stream);
 
+/* Fused frozen MLP: one call of a transformer block's MLP (utils/models.py Mlp: fc2(act(fc1(x))), act = nn.GELU()) whose
+ * fc1 and fc2 Linears are frozen (p4v_linear_pack).  Replaces the unfrozen sequence of quant_forward(fc1) (linear.py:62-67),
+ * torch's GELU and quant_forward(fc2), whose activation quantiser (linear.py:62-67, post-GELU: :601-607) reads the GELU
+ * output, with two launches:
+ *   A. fc1 on the fused kernel (csrc/forward_tc.cu) with an epilogue that applies torch's fp32 GELU (approximate='none')
+ *      to each output element and quantises it with fc2's activation quantiser into fc2's int8 activation image, the
+ *      image of fc2's streamed path (p4v_linear_frozen_forward): the hidden activations reach HBM only as those bytes;
+ *   B. fc2's sweep forward on that image.
+ * Every byte of the image and every output bit equal those of p4v_linear_frozen_forward(fc1), torch.nn.functional.gelu
+ * and p4v_linear_frozen_forward(fc2).  The descriptors are those fc1 and fc2 were packed with, their rows the rows of x.
+ * p4v_mlp_fused_ok is the shape rule, a pure function of the descriptors without their rows: fc1.out_features ==
+ * fc2.in_features, fc1 plain (not post-GELU) with the fused kernel as its frozen path, and the fused kernel's shared-memory
+ * plan with the epilogue fits.  p4v_mlp_frozen_workspace_bytes: the size of fc2's image for the rows (the caller's
+ * workspace).  p4v_mlp_frozen_forward validates every argument before it launches anything (null pointers, equal rows,
+ * the shape rule, pack sizes, alignment: x 16 bytes, out 8 bytes, workspace 16 bytes; workspace size), then enqueues the
+ * two kernels: no allocation, no copy, no synchronisation, so it can be captured in a CUDA graph. */
+P4V_API int p4v_mlp_fused_ok(const p4v_linear_desc* fc1, const p4v_linear_desc* fc2, int* ok);
+P4V_API int p4v_mlp_frozen_workspace_bytes(const p4v_linear_desc* fc1, const p4v_linear_desc* fc2, size_t* bytes);
+P4V_API int p4v_mlp_frozen_forward(const p4v_linear_desc* fc1, const float* x, const float* bias1, const void* pack1,
+                                   size_t pack1_bytes, const p4v_linear_desc* fc2, const float* bias2, const void* pack2,
+                                   size_t pack2_bytes, void* workspace, size_t workspace_bytes, float* out, void* stream);
+/* Diagnostic: y[i] = the GELU of the fused MLP's epilogue applied to x[i], for i < n (one launch on `stream`), so that it
+ * can be compared with torch.nn.functional.gelu over every fp32 bit pattern. */
+P4V_API int p4v_gelu_probe(const float* x, float* y, long long n, void* stream);
+
 /* The patch-embedding convolution: ChannelwiseBatchingQuantConv2d with a_bit >= 32 (quant_layers/conv.py:444-614, wired
  * by configs/PTQ4ViT.py:52-54): one weight step size per output channel, activations left in FP32.  The caller passes
  * the im2col matrix of the FP32 input (torch.nn.functional.unfold, [images, positions, K], K = in_channels*kh*kw in the

@@ -69,6 +69,11 @@ _SIGNATURES = {
     "p4v_attention_long_ok": [C.c_int32, C.c_int32, C.POINTER(C.c_int)],
     "p4v_attention_frozen_forward_long": [C.POINTER(AttentionDesc), _P, C.POINTER(C.c_longlong), C.POINTER(MatMulDesc), _P,
                                           C.c_size_t, C.POINTER(MatMulDesc), _P, C.c_size_t, _P, _P, _P, _P],
+    "p4v_mlp_fused_ok": [C.POINTER(LinearDesc), C.POINTER(LinearDesc), C.POINTER(C.c_int)],
+    "p4v_mlp_frozen_workspace_bytes": [C.POINTER(LinearDesc), C.POINTER(LinearDesc), C.POINTER(C.c_size_t)],
+    "p4v_mlp_frozen_forward": [C.POINTER(LinearDesc), _P, _P, _P, C.c_size_t, C.POINTER(LinearDesc), _P, _P, C.c_size_t, _P,
+                               C.c_size_t, _P, _P],
+    "p4v_gelu_probe": [_P, _P, C.c_longlong, _P],
     "p4v_conv_workspace_bytes": [C.POINTER(ConvDesc), C.POINTER(C.c_size_t)],
     "p4v_conv_calibrate": [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P],
     "p4v_export_quantized": [_P, C.c_longlong, C.c_longlong, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,

@@ -16,8 +16,13 @@
 //      segment group, folded into r after its last job exactly as the sweep's forward branch does (sweep_tc.cu):
 //      r = -bias, r = fmaf(-scale[g][col / 16], (float)acc, r) in the step's group order, out = -r.  Same integers, same
 //      fp32 operations in the same order: the output is bit-identical to p4v_linear_quant_forward.
+// With FwdMlpParams the same kernel is fc1 of a fused frozen MLP: step 2's epilogue applies torch's GELU and fc2's
+// activation quantiser and writes fc2's int8 activation image instead of FP32 (see the epilogue below, DESIGN §4.8).
 // 288 threads leave 224 registers per thread without setmaxnreg; the bounded mbarrier wait is inline, and the k32 steps of
 // a stage are one straight-line batch selected by a warp-uniform count (ptxas C7520, see sm90.cuh).
+#include <type_traits>
+
+#include "../../include/ptq4vit_b200.h"
 #include "forward.cuh"
 #include "sm90.cuh"
 
@@ -43,13 +48,123 @@ __device__ __forceinline__ void pack16(uint32_t (&w)[4], int e, float q) {
   w[e >> 2] |= (uint32_t)((int)q & 0xff) << ((e & 3) * 8);
 }
 
-__global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_constant__ FwdParams P) {
+// ---- the epilogue of mlp_fc1_kernel: GELU, fc2's activation quantiser, fc2's image --------------------------------
+// Shared memory: [staged tile: planes2 x 128 rows x P4V_MLP_STAGE_LD][step size, reciprocal of the 128 columns][chunk table]
+// The bytes of a 16-byte chunk of fc2's image have source columns that need not lie in one 128-column tile of fc1 (a
+// segment of fc2 may start anywhere), and the column tiles of a row tile may belong to different CTAs.  A byte belongs
+// to the column tile of its source column; a padding byte to that of its segment's last column.  Every byte of the image
+// then has exactly one owner, and a CTA stores whole chunks it owns as one 16-byte store and the owned bytes of a chunk
+// that straddles two column tiles one by one.
+__device__ __forceinline__ unsigned mlp_epi_bytes(const FwdParams&) { return 0u; }
+__device__ __forceinline__ unsigned mlp_epi_bytes(const FwdMlpParams& P) { return P.epi_bytes; }
+
+__device__ __forceinline__ uint8_t* mlp_epi(const FwdMlpParams& P, uint8_t* smem) {
+  return smem + P.a_bytes + (size_t)P.n_stages * P.stage_bytes;
+}
+__device__ __forceinline__ float* mlp_steps(const FwdMlpParams& P, uint8_t* epi) {
+  return reinterpret_cast<float*>(epi + P.planes2 * P4V_TILE * P4V_MLP_STAGE_LD);
+}
+__device__ __forceinline__ P4VMlpChunk* mlp_chunks(const FwdMlpParams& P, uint8_t* epi) {
+  return reinterpret_cast<P4VMlpChunk*>(mlp_steps(P, epi) + 2 * P4V_TILE);
+}
+
+// fc2's chunk table (one plane of a row of its image), by the whole CTA before the setup barrier
+__device__ __forceinline__ void mlp_chunk_table(const FwdMlpParams& P, uint8_t* epi) {
+  P4VMlpChunk* tab = mlp_chunks(P, epi);
+  for (int s = threadIdx.x; s < P.nseg2; s += kThreads) {
+    const P4VSeg sg = P.segs2[s];
+    const int c0 = sg.dst_off / (P4V_TILE * 16), nch = ((sg.klen + 31) / 32) * 2, last = sg.k0 + sg.klen - 1;
+    for (int c = 0; c < nch; ++c) tab[c0 + c] = P4VMlpChunk{min(sg.k0 + 16 * c, last), max(0, min(16, sg.klen - 16 * c))};
+  }
+}
+
+// fc2's step size of each column of tile tn and its reciprocal (0 where p4v_rint_div_ok fails: the exact division), by
+// the consumers between the barriers that open a column tile
+__device__ __forceinline__ void mlp_column_steps(const FwdMlpParams& P, uint8_t* epi, int tn, int et) {
+  float* d = mlp_steps(P, epi);
+  for (int lc = et; lc < P4V_TILE; lc += kConsumers) {
+    const int col = tn * P4V_TILE + lc;
+    const float delta = col < P.N ? __ldg(P.dX2 + col / P.crb_acts2) : 1.f;
+    d[lc] = delta;
+    d[P4V_TILE + lc] = p4v_rint_div_ok(delta) ? __frcp_rn(delta) : 0.f;
+  }
+}
+
+// The thread's 64 fc1 values (r = -value, fragment layout of forward_tc_body) -> GELU -> fc2's bytes, staged by column
+// (quant_image_kernel's sequence for fc2's segments: p4v_quant_plain, the negative plane with d_neg, NaN -> 0)
+__device__ __forceinline__ void mlp_stage_tile(const FwdMlpParams& P, uint8_t* epi, const float (&r)[64], int frow, int fcol) {
+  const float* d = mlp_steps(P, epi);
+  const float rcp_neg = __frcp_rn(P.d_neg2), rcp_neg_scalar = __fdiv_rn(1.f, P.d_neg2);
+  const bool fast_neg = p4v_rint_div_ok(P.d_neg2), twin = P.planes2 == 2;
+#pragma unroll
+  for (int v = 0; v < 64; v += 2) {
+    const int row = frow + 8 * ((v >> 1) & 1), lc = fcol + 8 * (v >> 2);
+    uint32_t bp = 0u, bn = 0u;
+#pragma unroll
+    for (int t = 0; t < 2; ++t) {
+      const float g = p4v_gelu(-r[v + t]);
+      const float rcp = d[P4V_TILE + lc + t];
+      bp |= p4v_qbyte(p4v_quant_plain(g, d[lc + t], rcp != 0.f, rcp, false, 0.f, P.lo2, P.hi2)) << (8 * t);
+      if (twin) bn |= p4v_qbyte(p4v_quant_plain(g, P.d_neg2, fast_neg, rcp_neg, !P.ieee_div, rcp_neg_scalar, P.neg_lo2, 0.f)) << (8 * t);
+    }
+    uint8_t* st = epi + row * P4V_MLP_STAGE_LD + lc;
+    *reinterpret_cast<uint16_t*>(st) = (uint16_t)bp;
+    if (twin) *reinterpret_cast<uint16_t*>(st + P4V_TILE * P4V_MLP_STAGE_LD) = (uint16_t)bn;
+  }
+}
+
+// The bytes of fc2's image that column tile tn of row tile tm owns, from the staged tile; rows past M are zeros
+__device__ __forceinline__ void mlp_store_tile(const FwdMlpParams& P, uint8_t* epi, int tm, int tn, int et) {
+  const P4VMlpChunk* tab = mlp_chunks(P, epi);
+  const int c0 = tn * P4V_TILE, c1 = min(c0 + P4V_TILE, P.N);
+  // the chunks with a byte in [c0, c1): kf and the owner of the last byte grow with the chunk index
+  int lo = 0, hi = P.n_chunks2;
+  while (lo < hi) { const int m = (lo + hi) >> 1; const P4VMlpChunk c = tab[m]; if (c.kf + max(c.n - 1, 0) >= c0) hi = m; else lo = m + 1; }
+  const int cb = lo;
+  hi = P.n_chunks2;
+  while (lo < hi) { const int m = (lo + hi) >> 1; if (tab[m].kf >= c1) hi = m; else lo = m + 1; }
+  const int nc = lo - cb;
+  for (int u = et; u < P.planes2 * nc * P4V_TILE; u += kConsumers) {
+    const int r = u & (P4V_TILE - 1), pc = u >> 7, plane = pc / nc, c = cb + pc % nc;
+    const P4VMlpChunk ch = tab[c];
+    const bool in = tm * P4V_TILE + r < P.M;
+    const uint8_t* srow = epi + (plane * P4V_TILE + r) * P4V_MLP_STAGE_LD - c0;   // indexed by source column
+    uint8_t* dst = P.X2 + (size_t)tm * P.X2_tile_bytes + (size_t)plane * P.X2_plane_bytes + ((size_t)c * P4V_TILE + r) * 16;
+    if (ch.n == 16 && ch.kf >= c0 && ch.kf + 16 <= c1 && ((ch.kf - c0) & 15) == 0) {
+      *reinterpret_cast<uint4*>(dst) = in ? *reinterpret_cast<const uint4*>(srow + ch.kf) : make_uint4(0u, 0u, 0u, 0u);
+      continue;
+    }
+    const int kl = ch.kf + max(ch.n - 1, 0);
+    uint32_t w[4] = {0u, 0u, 0u, 0u}, own = 0u;
+#pragma unroll
+    for (int e = 0; e < 16; ++e) {
+      const int k = e < ch.n ? ch.kf + e : kl;
+      if (k >= c0 && k < c1) {
+        own |= 1u << e;
+        if (e < ch.n && in) w[e >> 2] |= (uint32_t)srow[k] << ((e & 3) * 8);
+      }
+    }
+    if (own == 0xffffu) {
+      *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
+    } else {
+#pragma unroll
+      for (int e = 0; e < 16; ++e)
+        if ((own >> e) & 1u) dst[e] = (uint8_t)(w[e >> 2] >> ((e & 3) * 8));
+    }
+  }
+}
+
+// Par = FwdParams: the frozen Linear forward, FP32 output.  Par = FwdMlpParams: fc1 of a frozen MLP, GELU-and-quantise
+// epilogue into fc2's image.
+template <class Par>
+__global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_constant__ Par P) {
+  constexpr bool kMlp = std::is_same<Par, FwdMlpParams>::value;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
-  // carve: [resident activation tile][weight ring][control]
+  // carve: [resident activation tile][weight ring][MLP epilogue][control]
   const uint32_t nst = P.n_stages, sC = P.stage_bytes;
   const uint32_t resA = smem_u32(smem), ring = resA + P.a_bytes;
-  FwdCtl& S = *reinterpret_cast<FwdCtl*>(smem + P.a_bytes + (size_t)nst * sC);
+  FwdCtl& S = *reinterpret_cast<FwdCtl*>(smem + P.a_bytes + (size_t)nst * sC + mlp_epi_bytes(P));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // the CTA's row tile and its share of the column tiles
@@ -65,6 +180,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
     for (int c = 0; c < nch; ++c)
       S.chunks[c0 + c] = Chunk{sg.k0 + 16 * c, (short)max(0, min(16, sg.klen - 16 * c)), (short)sg.didx};
   }
+  if constexpr (kMlp) mlp_chunk_table(P, mlp_epi(P, smem));
   if (threadIdx.x == 0) {
     for (uint32_t i = 0; i < nst; ++i) { mbar_init(&S.full[i], 1); mbar_init(&S.empty[i], kConsumerWarps); }
     fence_mbarrier_init();
@@ -154,6 +270,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
     asm volatile("bar.sync 1, %0;" ::"n"(kConsumers));   // previous column tile done with the scale rows
     for (int i = et; i < P.n_groups * P4V_TILE_CG; i += kConsumers)
       S.scale[i >> 3][i & 7] = P.scale[(size_t)(i >> 3) * P.nsg + tn * P4V_TILE_CG + (i & 7)];
+    if constexpr (kMlp) mlp_column_steps(P, mlp_epi(P, smem), tn, et);
     const int gc = tn * P4V_TILE + fcol;               // global columns gc + 8 * i + {0, 1}
 #pragma unroll
     for (int v = 0; v < 64; ++v) {
@@ -183,35 +300,67 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
       }
       if (++stage == nst) { stage = 0; phase ^= 1; }
     }
-    const bool pairs = (P.N & 1) == 0;       // even row stride: the fragment's column pairs are 8-byte aligned
+    if constexpr (kMlp) {
+      mlp_stage_tile(P, mlp_epi(P, smem), r, frow, fcol);
+      asm volatile("bar.sync 1, %0;" ::"n"(kConsumers));   // staged tile complete
+      // the next column tile's first barrier orders these reads of the staging before it is written again
+      mlp_store_tile(P, mlp_epi(P, smem), tm, tn, et);
+    } else {
+      const bool pairs = (P.N & 1) == 0;       // even row stride: the fragment's column pairs are 8-byte aligned
 #pragma unroll
-    for (int v = 0; v < 64; v += 2) {
-      const int row = gm + 8 * ((v >> 1) & 1), col = gc + 8 * (v >> 2);
-      if (row < P.M) {
-        float* o = P.out + (size_t)row * P.N + col;
-        if (pairs) { if (col < P.N) *reinterpret_cast<float2*>(o) = make_float2(-r[v], -r[v + 1]); }
-        else { if (col < P.N) o[0] = -r[v]; if (col + 1 < P.N) o[1] = -r[v + 1]; }
+      for (int v = 0; v < 64; v += 2) {
+        const int row = gm + 8 * ((v >> 1) & 1), col = gc + 8 * (v >> 2);
+        if (row < P.M) {
+          float* o = P.out + (size_t)row * P.N + col;
+          if (pairs) { if (col < P.N) *reinterpret_cast<float2*>(o) = make_float2(-r[v], -r[v + 1]); }
+          else { if (col < P.N) o[0] = -r[v]; if (col + 1 < P.N) o[1] = -r[v + 1]; }
+        }
       }
     }
   }
 }
 
-}  // namespace
+__global__ void gelu_probe_kernel(const float* __restrict__ x, float* __restrict__ y, long long n) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    y[i] = p4v_gelu(x[i]);
+}
 
-int p4v_launch_forward_tc(const FwdParams& p, int num_sms, cudaStream_t st) {
+template <class Par>
+int launch(void (*kernel)(Par), const Par& p, unsigned epi_bytes, int num_sms, cudaStream_t st) {
   P4V_REQUIRE(p.n_jobs >= 1 && p.n_jobs <= P4V_MAX_JOBS && p.n_groups <= P4V_MAX_GROUPS, "forward: too many K segments");
   P4V_REQUIRE(p.n_stages >= 2 && p.n_stages <= P4V_FWD_MAX_STAGES && p.n_chunks <= P4V_FWD_MAX_CHUNKS &&
-              p.stage_bytes % 128 == 0 && p.a_bytes % 128 == 0, "forward: bad shared-memory plan");
+              p.stage_bytes % 128 == 0 && p.a_bytes % 128 == 0 && epi_bytes % 128 == 0, "forward: bad shared-memory plan");
   P4V_REQUIRE((reinterpret_cast<uintptr_t>(p.out) & 7) == 0 && (reinterpret_cast<uintptr_t>(p.x) & 15) == 0,
               "forward: x must be 16-byte and out 8-byte aligned");
-  const size_t smem = (size_t)p.a_bytes + (size_t)p.n_stages * p.stage_bytes + sizeof(FwdCtl) + 128;
+  const size_t smem = (size_t)p.a_bytes + (size_t)p.n_stages * p.stage_bytes + epi_bytes + sizeof(FwdCtl) + 128;
   P4V_REQUIRE(smem <= P4V_FWD_SMEM, "forward: shared-memory plan too large (%zu bytes)", smem);
   // Fewer row tiles than SMs: split the column tiles of a row tile over several CTAs (each quantises the row tile again,
   // from L2) so that the whole GPU writes output.
   int csplit = num_sms / p.tiles_m;
   csplit = csplit < 1 ? 1 : (csplit > p.tiles_n ? p.tiles_n : csplit);
-  P4V_CUDA_OK(cudaFuncSetAttribute(forward_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  forward_tc_kernel<<<p.tiles_m * csplit, kThreads, smem, st>>>(p);
+  P4V_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<p.tiles_m * csplit, kThreads, smem, st>>>(p);
+  p4v_count_launch();
+  P4V_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+}  // namespace
+
+int p4v_launch_forward_tc(const FwdParams& p, int num_sms, cudaStream_t st) { return launch(forward_tc_kernel<FwdParams>, p, 0u, num_sms, st); }
+
+int p4v_launch_mlp_fc1_tc(const FwdMlpParams& p, int num_sms, cudaStream_t st) {
+  P4V_REQUIRE(!p.twin && (p.planes2 == 1 || p.planes2 == 2) && p.epi_bytes == p4v_mlp_epi_bytes(p.planes2, p.n_chunks2) &&
+              (reinterpret_cast<uintptr_t>(p.X2) & 15) == 0, "mlp forward: bad epilogue plan");
+  return launch(forward_tc_kernel<FwdMlpParams>, p, p.epi_bytes, num_sms, st);
+}
+
+// Diagnostic: y = p4v_gelu(x) elementwise (the GELU of mlp_fc1_kernel's epilogue)
+extern "C" int p4v_gelu_probe(const float* x, float* y, long long n, void* stream) {
+  P4V_REQUIRE(x && y && n >= 0, "gelu_probe: null pointer or negative count");
+  if (n == 0) return 0;
+  const long long blocks = (n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096;
+  gelu_probe_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, y, n);
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   return 0;

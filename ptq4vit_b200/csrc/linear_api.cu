@@ -783,6 +783,36 @@ extern "C" int p4v_linear_frozen_workspace_bytes(const p4v_linear_desc* d, size_
   return 0;
 }
 
+namespace {
+
+// The fused kernel's parameters of a frozen layer whose path is the fused kernel
+void fill_fwd(const FrozenPlan& f, const float* x, const float* bias, void* packed, float* out, FwdParams& q) {
+  const LinPlan& p = f.p;
+  q.x = x; q.ld = p.K; q.M = p.M; q.N = p.O; q.bias = p.d.has_bias ? bias : nullptr; q.out = out;
+  q.W = p.Wcur.ptr(packed); q.W_tile_bytes = p.Wcur.tile_bytes(); q.tiles_m = p.tiles_m; q.tiles_n = p.tiles_o;
+  q.scale = at<float>(packed, p.o_fix); q.nsg = p.nsg; q.n_groups = p.fwd.nfg;
+  q.jobs = p.jobs.dev(packed) + p.fwd.job_off; q.n_jobs = p.fwd.nfj;
+  q.segs = p.segsX.dev(packed); q.nseg = (int)p.segs.size();
+  q.dX = at<float>(packed, f.o_dX);
+  q.twin = p.twin; q.d_neg = p.d_neg; q.lo = p.twin ? 0.f : (float)-p.a_qmax; q.hi = (float)(p.a_qmax - 1);
+  q.neg_lo = (float)-p.a_qmax; q.ieee_div = p4v_scalar_div_ieee();
+  q.plane_bytes = (unsigned)p.Wcur.tile_bytes(); q.a_bytes = (unsigned)f.X.tile_bytes();
+  q.stage_bytes = (unsigned)f.stage_kb * P4V_TILE; q.n_stages = (unsigned)f.stages; q.n_chunks = (unsigned)p.Wcur.kb / 16;
+}
+
+// The second half of the streamed path: the sweep forward of the layer's int8 activation image in the workspace
+int streamed_sweep(const FrozenPlan& f, void* packed, void* workspace, const float* bias, float* out, cudaStream_t st) {
+  const LinPlan& p = f.p;
+  SweepParams sp; fill_sweep(p, packed, p.fwd, sp, all_rows(p));
+  sp.R_cur = f.X.ptr(workspace);
+  sp.bias = p.d.has_bias ? bias : nullptr;
+  sp.out = out; sp.n_cand = 1; sp.order = 0;
+  sp.R_cand = nullptr; sp.C_cand = nullptr;
+  return run_sweep(p, p.fwd, sp, st);
+}
+
+}  // namespace
+
 extern "C" int p4v_linear_frozen_forward(const p4v_linear_desc* d, const float* x, const float* bias, const void* packed_in,
                                          void* workspace, size_t workspace_bytes, float* out, void* stream) {
   FrozenPlan f; int rc = build_frozen(d, f, false);
@@ -792,19 +822,9 @@ extern "C" int p4v_linear_frozen_forward(const p4v_linear_desc* d, const float* 
   P4V_REQUIRE(x && packed && out, "linear_frozen_forward: null pointer");
   P4V_REQUIRE(!d->has_bias || bias, "linear_frozen_forward: has_bias set but bias is null");
   cudaStream_t st = (cudaStream_t)stream;
-  const P4VJob* host_jobs = p.jobs.host.data() + p.fwd.job_off;
   if (f.stages >= 2) {
     FwdParams q{};
-    q.x = x; q.ld = p.K; q.M = p.M; q.N = p.O; q.bias = d->has_bias ? bias : nullptr; q.out = out;
-    q.W = p.Wcur.ptr(packed); q.W_tile_bytes = p.Wcur.tile_bytes(); q.tiles_m = p.tiles_m; q.tiles_n = p.tiles_o;
-    q.scale = at<float>(packed, p.o_fix); q.nsg = p.nsg; q.n_groups = p.fwd.nfg;
-    q.jobs = p.jobs.dev(packed) + p.fwd.job_off; q.n_jobs = p.fwd.nfj;
-    q.segs = p.segsX.dev(packed); q.nseg = (int)p.segs.size();
-    q.dX = at<float>(packed, f.o_dX);
-    q.twin = p.twin; q.d_neg = p.d_neg; q.lo = p.twin ? 0.f : (float)-p.a_qmax; q.hi = (float)(p.a_qmax - 1);
-    q.neg_lo = (float)-p.a_qmax; q.ieee_div = p4v_scalar_div_ieee();
-    q.plane_bytes = (unsigned)p.Wcur.tile_bytes(); q.a_bytes = (unsigned)f.X.tile_bytes();
-    q.stage_bytes = (unsigned)f.stage_kb * P4V_TILE; q.n_stages = (unsigned)f.stages; q.n_chunks = (unsigned)p.Wcur.kb / 16;
+    fill_fwd(f, x, bias, packed, out, q);
     return p4v_launch_forward_tc(q, p4v_num_sms(), st);
   }
   P4V_REQUIRE(workspace && workspace_bytes >= f.X.bytes(), "linear_frozen_forward: workspace too small (%zu < %zu)",
@@ -814,10 +834,80 @@ extern "C" int p4v_linear_frozen_forward(const p4v_linear_desc* d, const float* 
   qa.src = x; qa.ld = p.K; qa.rows = p.M; qa.delta = at<float>(packed, f.o_dX); qa.d_mod = 1;
   qa.rows_per_block = p.M + P4V_TILE; qa.segs = p.segsX.dev(packed); qa.nseg = (int)p.segsX.host.size();
   if ((rc = p4v_quant_image(qa, st))) return rc;
-  SweepParams sp; fill_sweep(p, packed, p.fwd, sp, all_rows(p));
-  sp.R_cur = f.X.ptr(workspace);
-  sp.bias = d->has_bias ? bias : nullptr;
-  sp.out = out; sp.n_cand = 1; sp.order = 0;
-  sp.R_cand = nullptr; sp.C_cand = nullptr;
-  return run_sweep(p, p.fwd, sp, st);
+  return streamed_sweep(f, packed, workspace, bias, out, st);
+}
+
+// ---- fused frozen MLP: fc1 + GELU + fc2's activation quantiser in one kernel, then fc2's sweep forward -----------
+namespace {
+
+struct MlpPlan {
+  FrozenPlan f1, f2;
+  int stages;         // ring stages of fc1's kernel with the epilogue; 0: the MLP does not fuse
+  int planes2, chunks2;
+};
+
+// for_rule: the rows of the descriptors are ignored (p4v_mlp_fused_ok)
+int build_mlp(const p4v_linear_desc* d1, const p4v_linear_desc* d2, MlpPlan& m, bool for_rule) {
+  P4V_REQUIRE(d1 && d2, "mlp: null desc");
+  int rc;
+  if ((rc = build_frozen(d1, m.f1, for_rule)) || (rc = build_frozen(d2, m.f2, for_rule))) return rc;
+  const LinPlan &p1 = m.f1.p, &p2 = m.f2.p;
+  m.planes2 = p2.twin ? 2 : 1;
+  m.chunks2 = p2.Wcur.kb / 16;      // a plane of fc2's activation image has the K layout of its weight image
+  m.stages = 0;
+  if (p1.O == p2.K && !p1.twin && m.f1.stages >= 2)
+    m.stages = mlp_ring_stages(m.f1.X.tile_bytes(), (size_t)m.f1.stage_kb * P4V_TILE, p1.Wcur.kb / 16, m.planes2, m.chunks2);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int p4v_mlp_fused_ok(const p4v_linear_desc* fc1, const p4v_linear_desc* fc2, int* ok) {
+  MlpPlan m; int rc = build_mlp(fc1, fc2, m, true);
+  if (rc) return rc;
+  P4V_REQUIRE(ok != nullptr, "null output");
+  *ok = m.stages >= 2 ? 1 : 0;
+  return 0;
+}
+
+extern "C" int p4v_mlp_frozen_workspace_bytes(const p4v_linear_desc* fc1, const p4v_linear_desc* fc2, size_t* bytes) {
+  MlpPlan m; int rc = build_mlp(fc1, fc2, m, false);
+  if (rc) return rc;
+  P4V_REQUIRE(fc1->rows == fc2->rows, "mlp: fc1 and fc2 must have the same rows (%d != %d)", fc1->rows, fc2->rows);
+  P4V_REQUIRE(bytes != nullptr, "null output");
+  *bytes = m.f2.X.bytes();
+  return 0;
+}
+
+extern "C" int p4v_mlp_frozen_forward(const p4v_linear_desc* fc1, const float* x, const float* bias1, const void* pack1,
+                                      size_t pack1_bytes, const p4v_linear_desc* fc2, const float* bias2, const void* pack2,
+                                      size_t pack2_bytes, void* workspace, size_t workspace_bytes, float* out, void* stream) {
+  MlpPlan m; int rc = build_mlp(fc1, fc2, m, false);
+  if (rc) return rc;
+  P4V_REQUIRE(fc1->rows == fc2->rows, "mlp_frozen_forward: fc1 and fc2 must have the same rows (%d != %d)", fc1->rows, fc2->rows);
+  P4V_REQUIRE(x && pack1 && pack2 && workspace && out, "mlp_frozen_forward: null pointer");
+  P4V_REQUIRE((!fc1->has_bias || bias1) && (!fc2->has_bias || bias2), "mlp_frozen_forward: has_bias set but bias is null");
+  P4V_REQUIRE(m.stages >= 2, "mlp_frozen_forward: these layers do not fuse (p4v_mlp_fused_ok)");
+  P4V_REQUIRE(pack1_bytes >= m.f1.bytes && pack2_bytes >= m.f2.bytes, "mlp_frozen_forward: packed buffer too small "
+              "(fc1 %zu < %zu or fc2 %zu < %zu)", pack1_bytes, m.f1.bytes, pack2_bytes, m.f2.bytes);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0 &&
+              (reinterpret_cast<uintptr_t>(workspace) & 15) == 0,
+              "mlp_frozen_forward: x and workspace must be 16-byte and out 8-byte aligned");
+  P4V_REQUIRE(workspace_bytes >= m.f2.X.bytes(), "mlp_frozen_forward: workspace too small (%zu < %zu)", workspace_bytes,
+              m.f2.X.bytes());
+  cudaStream_t st = (cudaStream_t)stream;
+  void* p1 = const_cast<void*>(pack1);
+  void* p2 = const_cast<void*>(pack2);
+  const LinPlan& l2 = m.f2.p;
+  FwdMlpParams q{};
+  fill_fwd(m.f1, x, bias1, p1, nullptr, q);
+  q.n_stages = (unsigned)m.stages;
+  q.X2 = m.f2.X.ptr(workspace); q.X2_tile_bytes = m.f2.X.tile_bytes(); q.X2_plane_bytes = (unsigned)l2.Wcur.tile_bytes();
+  q.segs2 = l2.segsX.dev(p2); q.nseg2 = (int)l2.segs.size();
+  q.n_chunks2 = m.chunks2; q.planes2 = m.planes2;
+  q.dX2 = at<float>(p2, m.f2.o_dX); q.crb_acts2 = l2.crb_acts;
+  q.d_neg2 = l2.d_neg; q.lo2 = l2.twin ? 0.f : (float)-l2.a_qmax; q.hi2 = (float)(l2.a_qmax - 1); q.neg_lo2 = (float)-l2.a_qmax;
+  q.epi_bytes = p4v_mlp_epi_bytes(m.planes2, m.chunks2);
+  if ((rc = p4v_launch_mlp_fc1_tc(q, p4v_num_sms(), st))) return rc;
+  return streamed_sweep(m.f2, p2, workspace, bias2, out, st);
 }

@@ -106,6 +106,13 @@ inline int frozen_ring_stages(size_t a_bytes, size_t stage_bytes, size_t plane_c
   return (int)std::min<size_t>((usable - a_bytes) / stage_bytes, P4V_FWD_MAX_STAGES);
 }
 
+// fc1 of a fused frozen MLP (forward_tc.cu with FwdMlpParams): the ring stages of fc1's fused kernel when the
+// GELU-and-quantise epilogue (the staged tile in fc2's planes, fc2's column steps and chunk table) takes its share of
+// shared memory.  0: the MLP does not fuse.
+inline int mlp_ring_stages(size_t a_bytes1, size_t stage_bytes1, size_t plane_chunks1, int planes2, int plane_chunks2) {
+  return frozen_ring_stages(a_bytes1 + p4v_mlp_epi_bytes(planes2, plane_chunks2), stage_bytes1, plane_chunks1);
+}
+
 // A commit copies the chosen candidate's slabs from the planes of cand into cur
 inline void fill_images(CommitArgs& c, void* ws, const Image& cand, const Image& cur) {
   c.cand = cand.ptr(ws); c.cand_tile_bytes = cand.tile_bytes(); c.cand_plane_stride = cand.plane_stride();

@@ -154,11 +154,14 @@ class MinMaxQuantLinear(nn.Linear):
     def frozen(self):
         return self._packed is not None
 
-    def _frozen_forward(self, x):
+    def _check_frozen_intervals(self):
         w0, a0, v0 = self._frozen_intervals
         if self.w_interval is not w0 or self.a_interval is not a0 or self._interval_versions() != v0:
             raise RuntimeError(f"{self}: the step sizes changed after freeze(); call unfreeze() (and freeze() again) "
                                "before running the layer")
+
+    def _frozen_forward(self, x):
+        self._check_frozen_intervals()
         dev = self._packed.device
         x2 = _flat2d(x.to(dev))
         d = self._desc(x2.shape[0], 1)
@@ -241,6 +244,51 @@ class MinMaxQuantLinear(nn.Linear):
         self.calibrated = True
         out = self._bias_correction_quant_forward(x)
         return out
+
+
+def frozen_mlp_applies(fc1, fc2, act, x):
+    """Whether one call of an MLP block fc2(act(fc1(x))) can run as the fused frozen MLP (frozen_mlp): fc1 and fc2 frozen
+    Linear layers in quant_forward mode, act exactly torch's exact GELU (nn.GELU(approximate='none')), under grad mode
+    no input and no parameter of the layers that requires grad (the unfused call then carries a grad_fn), and a shape the
+    kernel holds (p4v_mlp_fused_ok: fc1.out_features == fc2.in_features, fc1 not post-GELU and on its fused kernel, the
+    shared-memory plan fits)."""
+    if not all(isinstance(m, MinMaxQuantLinear) and m.frozen and m.mode == "quant_forward" for m in (fc1, fc2)):
+        return False
+    if type(act) is not nn.GELU or act.approximate != "none":
+        return False
+    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in (fc1, fc2) for p in m.parameters())):
+        return False
+    ok = ctypes.c_int()
+    _lib.check(_lib.lib().p4v_mlp_fused_ok(ctypes.byref(fc1._desc(1, 1)), ctypes.byref(fc2._desc(1, 1)), ctypes.byref(ok)),
+               "p4v_mlp_fused_ok")
+    return bool(ok.value)
+
+
+def frozen_mlp(fc1, fc2, x):
+    """fc2(gelu(fc1(x))) of two frozen layers in two launches (csrc/forward_tc.cu: fc1 with a GELU-and-quantise
+    epilogue writing fc2's int8 activation image; fc2's sweep forward), for a call where frozen_mlp_applies holds.  The
+    bits are those of the unfused sequence.  fc2's image is kept between calls in fc2's frozen workspace."""
+    fc1._check_frozen_intervals()
+    fc2._check_frozen_intervals()
+    dev = fc1._packed.device
+    x2 = _flat2d(x.to(dev))
+    d1, d2 = fc1._desc(x2.shape[0], 1), fc2._desc(x2.shape[0], 1)
+    lib = _lib.lib()
+    nbytes = ctypes.c_size_t()
+    _lib.check(lib.p4v_mlp_frozen_workspace_bytes(ctypes.byref(d1), ctypes.byref(d2), ctypes.byref(nbytes)),
+               "p4v_mlp_frozen_workspace_bytes")
+    if fc2._frozen_ws is None or fc2._frozen_ws.numel() < nbytes.value or fc2._frozen_ws.device != dev:
+        fc2._frozen_ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    ws = fc2._frozen_ws
+    out = torch.empty(x2.shape[0], fc2.out_features, dtype=torch.float32, device=dev)
+    b1 = None if fc1.bias is None else fc1.bias.detach().contiguous().float()
+    b2 = None if fc2.bias is None else fc2.bias.detach().contiguous().float()
+    _lib.check(lib.p4v_mlp_frozen_forward(ctypes.byref(d1), _lib.ptr(x2), _lib.ptr(b1), _lib.ptr(fc1._packed), fc1._packed.numel(),
+                                          ctypes.byref(d2), _lib.ptr(b2), _lib.ptr(fc2._packed), fc2._packed.numel(),
+                                          _lib.ptr(ws), ws.numel(), _lib.ptr(out),
+                                          ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+               "p4v_mlp_frozen_forward")
+    return out.reshape(*x.shape[:-1], fc2.out_features)
 
 
 class PTQSLQuantLinear(MinMaxQuantLinear):

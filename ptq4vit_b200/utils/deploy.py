@@ -24,13 +24,18 @@ between the qkv and proj Linears -- matmul1, the scale, bias and mask, the softm
 never reaches HBM.  It is opt-in; `unfuse_attention(net)` undoes it.  `fuse_attention(net, max_tokens=1024)` also fuses
 the ViT / DeiT attention calls of 257 to 1024 tokens (384-pixel models: 577), with a kernel that quantises the keys and
 values of a head once and recomputes the scores instead of storing them (csrc/forward_attn_long_tc.cu).
+
+`fuse_mlp(net)` does the same for the MLP blocks whose fc1 and fc2 are frozen: fc1's kernel applies the GELU and fc2's
+activation quantiser in its epilogue and writes fc2's int8 activation image, which fc2's sweep forward reads -- two
+launches instead of four, bit-identical, and the FP32 hidden activations never reach HBM.  Opt-in as well;
+`unfuse_mlp(net)` undoes it.
 """
 import torch
 
 from ..quant_layers.linear import MinMaxQuantLinear
 from ..quant_layers.matmul import LONG_ATTENTION_TOKENS, SHORT_ATTENTION_TOKENS, MinMaxQuantMatMul
 from . import integer
-from .models import Attention, WindowAttention
+from .models import Attention, Mlp, WindowAttention
 
 INTERVALS = ("w_interval", "a_interval", "A_interval", "B_interval", "split")
 
@@ -86,6 +91,28 @@ def unfuse_attention(net):
             m.fused = False
         if isinstance(m, Attention):
             m.fused_max_tokens = SHORT_ATTENTION_TOKENS
+
+
+def fuse_mlp(net):
+    """Mark every `Mlp` module of `net` whose fc1 and fc2 are frozen Linear layers as fused: each call that qualifies
+    (quant_layers.linear.frozen_mlp_applies: exact GELU, no gradient wanted, a shape the kernel holds) runs fc1, the
+    GELU and fc2's activation quantiser as one kernel that writes fc2's int8 activation image, then fc2's sweep forward,
+    with the bits of the unfused sequence; the FP32 hidden activations never reach HBM.  A fused call skips the forward
+    hooks of fc1, act and fc2, so the fusion is opt-in; any other call runs the modules as before.  Returns the names of
+    the Mlp modules left unfused because a Linear is not frozen."""
+    left = []
+    for name, m in net.named_modules():
+        if isinstance(m, Mlp):
+            m.fused = all(isinstance(l, MinMaxQuantLinear) and l.frozen for l in (m.fc1, m.fc2))
+            if not m.fused:
+                left.append(name)
+    return left
+
+
+def unfuse_mlp(net):
+    for m in net.modules():
+        if isinstance(m, Mlp):
+            m.fused = False
 
 
 def _to(v, device):

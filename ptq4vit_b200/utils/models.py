@@ -5,6 +5,7 @@ available offline, so weights are synthetic (trunc-normal 0.02) -- this is harne
 import torch
 import torch.nn as nn
 
+from ..quant_layers.linear import frozen_mlp, frozen_mlp_applies
 from ..quant_layers.matmul import frozen_attention, frozen_attention_applies
 
 
@@ -50,7 +51,11 @@ class Mlp(nn.Module):
         self.act = nn.GELU()
         self.fc2 = nn.Linear(hidden, dim)
 
+    fused = False      # set by utils.deploy.fuse_mlp: run fc1, GELU and fc2 as the fused frozen MLP when it applies
+
     def forward(self, x):
+        if self.fused and frozen_mlp_applies(self.fc1, self.fc2, self.act, x):
+            return frozen_mlp(self.fc1, self.fc2, x)
         return self.fc2(self.act(self.fc1(x)))
 
 
