@@ -271,6 +271,42 @@ P4V_API int p4v_conv_calibrate(const p4v_conv_desc* d, const float* cols, const 
                        const float* raw_out, const float* raw_grad, void* workspace, size_t workspace_bytes,
                        float* w_interval, float* score_log, void* stream);
 
+/* Frozen patch-embedding convolution: the integer weights of a calibrated conv module with a_bit >= 32 packed once, and
+ * a forward that reads no FP32 weight.  Replaces, per call of quant_forward (quant_layers/conv.py:69-74 with
+ * quant_weight_bias :53-62; the activation quantiser :64-67 is off), the re-quantisation of the weight and
+ * F.conv2d(x, fl(q * delta), bias) for kernel == stride, padding 0, dilation 1, groups 1 (the patch embedding of
+ * ViT, DeiT and Swin; the Python layer checks stride, padding, dilation and groups, which the descriptor does not carry):
+ *   out[b, o, py, px] = fmaf(delta[o], S, bias[o])      (delta[o] * S rounded once without a bias)
+ *   S = sum_k (x_hi + x_mid + x_lo)[b, k at (py, px)] * q[o, k],   k = (c, i, j) in weight.reshape(O, K) order
+ * q: the integers of the export quantiser (p4v_export_quantized mode 0) for this weight and w_interval; x_hi/mid/lo: the
+ * exact three-term bf16 split of the FP32 pixel; bf16 wgmma products chained into one fp32 accumulator.  Not
+ * bit-identical to cuDNN's convolution; the bound against fp64 (ref = fp64(sum_k x_k * fl(q * delta)[o, k] + bias[o])):
+ *   |out - ref| <= (3K + 2) * 2^-23 * sum_k |x_k * fl(q * delta)[o, k]|  +  2^-23 * |ref|
+ * Repeated calls give the same bits (fixed summation order). */
+typedef struct p4v_conv_frozen_desc {
+  int32_t images, in_channels, height, width;   /* x [images, in_channels, height, width], contiguous fp32        */
+  int32_t out_channels, kernel_h, kernel_w;     /* stride = kernel; out [images, out_channels, height / kernel_h,
+                                                   width / kernel_w], contiguous fp32 (what F.conv2d returns)      */
+  int32_t w_bit;
+  int32_t layerwise;                            /* 1: w_interval holds one step size (BatchingEasyQuantConv2d),
+                                                   0: one per output channel (ChannelwiseBatchingQuantConv2d)      */
+  int32_t has_bias;
+} p4v_conv_frozen_desc;
+/* The shape rule, a pure function of the descriptor's module geometry (images, height and width are not consulted):
+ * 1 <= out_channels <= 4096, 1 <= K = in_channels * kernel_h * kernel_w <= 4096, 2 <= w_bit <= 8, flags 0 or 1. */
+P4V_API int p4v_conv_frozen_ok(const p4v_conv_frozen_desc* d, int* ok);
+/* `packed` (p4v_conv_pack_bytes bytes, independent of images, height and width; 16-byte aligned): the step size of every
+ * output channel (one repeated when layer-wise) and the bf16 image of q in 128-channel tiles and 32-element K slabs.
+ * p4v_conv_pack quantises weight [out_channels, K] fp32 with w_interval ([out_channels], or [1] when layer-wise). */
+P4V_API int p4v_conv_pack_bytes(const p4v_conv_frozen_desc* d, size_t* bytes);
+P4V_API int p4v_conv_pack(const p4v_conv_frozen_desc* d, const float* weight, const float* w_interval, void* packed,
+                          size_t packed_bytes, void* stream);
+/* One launch (csrc/forward_conv_tc.cu); every argument is validated first: null pointers, the shape rule, geometry
+ * (images >= 1, height >= kernel_h, width >= kernel_w), packed_bytes, alignment (packed 16 bytes; x, bias, out 4 bytes).
+ * No allocation, no copy, no synchronisation: it can be captured in a CUDA graph. */
+P4V_API int p4v_conv_frozen_forward(const p4v_conv_frozen_desc* d, const float* x, const float* bias, const void* packed,
+                                    size_t packed_bytes, float* out, void* stream);
+
 /* Integer export of a calibrated module (utils/integer.py:8-129): src [rows, cols] fp32 -> dst one byte per element.
  * mode 0: int8 = clamp(rne(x / delta), -q, q-1) (quantize_int_weight :8-18, quantize_matmul_input :27-42, plain
  * activations :64-69); mode 1: the post-GELU twin uint8 layout (:51-62); mode 2: the split-of-softmax twin uint8 layout

@@ -39,6 +39,12 @@ class ConvDesc(C.Structure):
                 ("has_bias", C.c_int32), ("kernel", C.c_int32), ("layerwise", C.c_int32)]
 
 
+class ConvFrozenDesc(C.Structure):
+    _fields_ = [("images", C.c_int32), ("in_channels", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
+                ("out_channels", C.c_int32), ("kernel_h", C.c_int32), ("kernel_w", C.c_int32), ("w_bit", C.c_int32),
+                ("layerwise", C.c_int32), ("has_bias", C.c_int32)]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     "p4v_linear_workspace_bytes": [C.POINTER(LinearDesc), C.POINTER(C.c_size_t)],
@@ -76,6 +82,10 @@ _SIGNATURES = {
     "p4v_gelu_probe": [_P, _P, C.c_longlong, _P],
     "p4v_conv_workspace_bytes": [C.POINTER(ConvDesc), C.POINTER(C.c_size_t)],
     "p4v_conv_calibrate": [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P],
+    "p4v_conv_frozen_ok": [C.POINTER(ConvFrozenDesc), C.POINTER(C.c_int)],
+    "p4v_conv_pack_bytes": [C.POINTER(ConvFrozenDesc), C.POINTER(C.c_size_t)],
+    "p4v_conv_pack": [C.POINTER(ConvFrozenDesc), _P, _P, _P, C.c_size_t, _P],
+    "p4v_conv_frozen_forward": [C.POINTER(ConvFrozenDesc), _P, _P, _P, C.c_size_t, _P, _P],
     "p4v_export_quantized": [_P, C.c_longlong, C.c_longlong, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                              _P, _P, _P],
 }

@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libptq4vit_b200.so")
-SOURCES = ["sweep_tc.cu", "forward_tc.cu", "forward_mm_tc.cu", "forward_attn_tc.cu", "forward_attn_long_tc.cu", "sweep_simt.cu", "prep.cu", "gram.cu", "gram_gemm.cu", "linear_api.cu", "matmul_api.cu", "conv_api.cu",
+SOURCES = ["sweep_tc.cu", "forward_tc.cu", "forward_mm_tc.cu", "forward_attn_tc.cu", "forward_attn_long_tc.cu", "forward_conv_tc.cu", "sweep_simt.cu", "prep.cu", "gram.cu", "gram_gemm.cu", "linear_api.cu", "matmul_api.cu", "conv_api.cu",
            "export.cu", "runtime.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",

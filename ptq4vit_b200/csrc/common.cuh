@@ -119,6 +119,12 @@ __device__ __forceinline__ float p4v_quant_sos(float v, float split, float qm1, 
   return fminf(fmaxf(rintf(__fdiv_rn(fminf(fmaxf(v, 0.f), split), __fdiv_rn(split, qm1))), 0.f), qm1);
 }
 
+// The export quantiser of a weight element (export.cu mode 0, utils/integer.py:15-17): clamp(rne(x / delta), -q, q-1)
+// with q = 2^(bit-1).  Shared by the export and the frozen convolution's pack, whose integers must be the same.
+__device__ __forceinline__ float p4v_quant_export(float x, float delta, float q) {
+  return fminf(fmaxf(rintf(__fdiv_rn(x, delta)), -q), q - 1.f);
+}
+
 // The int8 operand byte of a quantised value q (p4v_quant_plain / p4v_quant_sos): the integer's low byte.  NaN (0/0)
 // cannot be represented in the integer operand and becomes 0.
 __device__ __forceinline__ uint32_t p4v_qbyte(float q) {

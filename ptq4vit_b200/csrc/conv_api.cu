@@ -18,6 +18,10 @@
 //     score_c = -sum_images mean_positions mean_channels (g * (y - yhat_c))^2                 (conv.py:387-394)
 #include "../../include/ptq4vit_b200.h"
 #include "plan.cuh"
+#include <climits>
+
+#define P4V_XSTR(x) #x
+#define P4V_STR(x) P4V_XSTR(x)
 
 namespace {
 
@@ -181,4 +185,87 @@ extern "C" int p4v_conv_calibrate(const p4v_conv_desc* d, const float* cols, con
   if ((rc = p4v_select_step(f, st))) return rc;
   P4V_CUDA_OK(cudaMemcpyAsync(w_interval, at<float>(ws, p.o_d), (size_t)p.n_d * 4, cudaMemcpyDeviceToDevice, st));
   return 0;
+}
+
+// ---- frozen patch-embedding convolution: integer weights packed once, forward on csrc/forward_conv_tc.cu -----------
+namespace {
+
+// The shape rule on the module's geometry (images, height and width are the forward's): nullptr when it qualifies, else
+// the reason.
+const char* conv_frozen_reason(const p4v_conv_frozen_desc* d) {
+  if (d->in_channels < 1 || d->out_channels < 1 || d->kernel_h < 1 || d->kernel_w < 1) return "empty channel or kernel dimension";
+  if (d->out_channels > P4V_CONV_MAX_O) return "out_channels above " P4V_STR(P4V_CONV_MAX_O);
+  if ((long long)d->in_channels * d->kernel_h * d->kernel_w > P4V_CONV_MAX_K) return "K = in_channels * kh * kw above " P4V_STR(P4V_CONV_MAX_K);
+  if (d->w_bit < 2 || d->w_bit > 8) return "w_bit must be in [2,8] (bf16 holds the integers exactly)";
+  if ((d->layerwise != 0 && d->layerwise != 1) || (d->has_bias != 0 && d->has_bias != 1)) return "layerwise and has_bias must be 0 or 1";
+  return nullptr;
+}
+
+struct ConvFrozen { int O, K, tiles_n, n_slabs; size_t delta_bytes, total; };
+
+int build_conv_frozen(const p4v_conv_frozen_desc* d, ConvFrozen& f, const char* who) {
+  P4V_REQUIRE(d != nullptr, "%s: null desc", who);
+  const char* why = conv_frozen_reason(d);
+  P4V_REQUIRE(why == nullptr, "%s: %s", who, why);
+  f.O = d->out_channels; f.K = d->in_channels * d->kernel_h * d->kernel_w;
+  f.tiles_n = p4v_cdiv(f.O, P4V_TILE); f.n_slabs = p4v_cdiv(f.K, P4V_CONV_SLAB);
+  f.delta_bytes = p4v_conv_delta_bytes(f.O);
+  f.total = f.delta_bytes + (size_t)f.tiles_n * f.n_slabs * p4v_conv_slab_bytes();
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int p4v_conv_frozen_ok(const p4v_conv_frozen_desc* d, int* ok) {
+  P4V_REQUIRE(d && ok, "conv_frozen_ok: null pointer");
+  *ok = conv_frozen_reason(d) == nullptr;
+  return 0;
+}
+
+extern "C" int p4v_conv_pack_bytes(const p4v_conv_frozen_desc* d, size_t* bytes) {
+  ConvFrozen f; int rc = build_conv_frozen(d, f, "conv_pack_bytes");
+  if (rc) return rc;
+  P4V_REQUIRE(bytes != nullptr, "conv_pack_bytes: null output");
+  *bytes = f.total;
+  return 0;
+}
+
+extern "C" int p4v_conv_pack(const p4v_conv_frozen_desc* d, const float* weight, const float* w_interval, void* packed,
+                             size_t packed_bytes, void* stream) {
+  ConvFrozen f; int rc = build_conv_frozen(d, f, "conv_pack");
+  if (rc) return rc;
+  P4V_REQUIRE(weight && w_interval && packed, "conv_pack: null pointer");
+  P4V_REQUIRE(packed_bytes >= f.total, "conv_pack: packed buffer too small (%zu < %zu)", packed_bytes, f.total);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(packed) & 15) == 0, "conv_pack: packed must be 16-byte aligned");
+  uint8_t* base = static_cast<uint8_t*>(packed);
+  return p4v_launch_conv_pack(weight, w_interval, d->layerwise, f.O, f.K, d->w_bit, f.tiles_n, f.n_slabs,
+                              reinterpret_cast<float*>(base), base + f.delta_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int p4v_conv_frozen_forward(const p4v_conv_frozen_desc* d, const float* x, const float* bias, const void* packed,
+                                       size_t packed_bytes, float* out, void* stream) {
+  ConvFrozen f; int rc = build_conv_frozen(d, f, "conv_frozen_forward");
+  if (rc) return rc;
+  P4V_REQUIRE(x && packed && out, "conv_frozen_forward: null pointer");
+  P4V_REQUIRE(!d->has_bias || bias, "conv_frozen_forward: has_bias set but bias is null");
+  P4V_REQUIRE(d->images >= 1 && d->height >= d->kernel_h && d->width >= d->kernel_w,
+              "conv_frozen_forward: bad geometry (images %d, input %dx%d, kernel %dx%d): need at least one image and one "
+              "output position", d->images, d->height, d->width, d->kernel_h, d->kernel_w);
+  const long long chw = (long long)d->in_channels * d->height * d->width;
+  const int Ph = d->height / d->kernel_h, Pw = d->width / d->kernel_w;
+  const long long M = (long long)d->images * Ph * Pw;
+  P4V_REQUIRE(chw <= INT_MAX && M <= INT_MAX - P4V_TILE && (long long)p4v_cdiv((int)M, P4V_TILE) * f.tiles_n <= INT_MAX,
+              "conv_frozen_forward: input too large (in_channels*height*width %lld, positions %lld)", chw, M);
+  P4V_REQUIRE(packed_bytes >= f.total, "conv_frozen_forward: packed buffer too small (%zu < %zu)", packed_bytes, f.total);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(packed) & 15) == 0 && (reinterpret_cast<uintptr_t>(x) & 3) == 0 &&
+              (reinterpret_cast<uintptr_t>(out) & 3) == 0 && (reinterpret_cast<uintptr_t>(bias) & 3) == 0,
+              "conv_frozen_forward: packed must be 16-byte, x, bias and out 4-byte aligned");
+  FwdConvParams p{};
+  p.x = x; p.bias = d->has_bias ? bias : nullptr; p.out = out;
+  p.delta = static_cast<const float*>(packed);
+  p.Wq = static_cast<const uint8_t*>(packed) + f.delta_bytes;
+  p.B = d->images; p.C = d->in_channels; p.H = d->height; p.W = d->width; p.O = f.O; p.kh = d->kernel_h; p.kw = d->kernel_w;
+  p.Ph = Ph; p.Pw = Pw; p.K = f.K; p.M = (int)M;
+  p.tiles_m = p4v_cdiv(p.M, P4V_TILE); p.tiles_n = f.tiles_n; p.n_slabs = f.n_slabs;
+  return p4v_launch_forward_conv_tc(p, (cudaStream_t)stream);
 }

@@ -21,8 +21,7 @@ struct ExportArgs {
 __device__ __forceinline__ uint8_t encode(const ExportArgs& a, float x, float delta, float split, float rcp_neg) {
   const float q = a.qmax;
   if (a.mode == 0) {
-    const float v = fminf(fmaxf(rintf(__fdiv_rn(x, delta)), -q), q - 1.f);
-    return (uint8_t)(int8_t)(int)v;
+    return (uint8_t)(int8_t)(int)p4v_quant_export(x, delta, q);
   }
   if (a.mode == 1) {
     const float p = fminf(fmaxf(rintf(__fdiv_rn(x, delta)), 0.f), q - 1.f);

@@ -9,6 +9,12 @@ positions (im2col of the FP32 input, split exactly into three bf16 terms), one s
 BasePTQ wraps it with `BatchingEasyQuantConv2d(..., a_bit=32)` (configs/BasePTQ.py:48-50): one weight
 step size for the whole kernel.  The library runs the same search with every channel given that step
 size and sums the per-channel scores of a candidate into one (`p4v_conv_desc.layerwise`).
+
+After calibration a module can be frozen (`freeze()`): its integer weights are packed once as a bf16 image, and every
+quant_forward call that wants no gradient runs one kernel that gathers the patches from the image, splits the FP32
+pixels exactly into three bf16 terms and multiplies them with the integers on the tensor cores
+(csrc/forward_conv_tc.cu).  It reads no FP32 weight and does not depend on torch's TF32 setting.  Not bit-identical to
+cuDNN's F.conv2d: the contract is a bound against fp64 (DESIGN.md section 4.9).
 """
 import ctypes
 
@@ -41,6 +47,7 @@ class MinMaxQuantConv2d(nn.Conv2d):
         self.next_nodes = []
         self.w_qmax = 2 ** (self.w_bit - 1)
         self.a_qmax = 2 ** (self.a_bit - 1)
+        self._packed = None                  # freeze(): packed bf16 integer weights and step sizes (torch.uint8, device)
 
     def forward(self, x):
         if self.mode == "raw":
@@ -67,11 +74,107 @@ class MinMaxQuantConv2d(nn.Conv2d):
         return (x / ai).round_().clamp_(-self.a_qmax, self.a_qmax - 1).mul_(ai)
 
     def quant_forward(self, x):
-        """reference: conv.py:69-74"""
+        """reference: conv.py:69-74.  A frozen module runs the packed forward for calls that want no gradient (under grad
+        mode no input and no parameter requires grad); every other call runs the torch operations below."""
         assert self.calibrated is not None, f"You should run calibrate_forward before run quant_forward for {self}"
+        if self._packed is not None and not (torch.is_grad_enabled() and
+                                             (x.requires_grad or any(p.requires_grad for p in self.parameters()))):
+            return self._frozen_forward(x)
         w_sim, bias_sim = self.quant_weight_bias()
         x_sim = self.quant_input(x) if self.a_bit < 32 else x
         return F.conv2d(x_sim, w_sim, bias_sim, self.stride, self.padding, self.dilation, self.groups)
+
+    # ---- frozen module: integer weights packed once (csrc/forward_conv_tc.cu) ----
+    def _frozen_desc(self, x=None):
+        d = _lib.ConvFrozenDesc()
+        if x is not None:
+            d.images, d.in_channels, d.height, d.width = (int(s) for s in x.shape)
+        else:
+            d.in_channels = self.in_channels
+        d.out_channels = self.out_channels
+        d.kernel_h, d.kernel_w = (int(k) for k in self.kernel_size)
+        d.w_bit = int(self.w_bit)
+        d.layerwise = 1 if self.w_interval is not None and torch.as_tensor(self.w_interval).numel() == 1 else 0
+        d.has_bias = 0 if self.bias is None else 1
+        return d
+
+    def frozen_unsupported(self):
+        """Why freeze() cannot pack this module (None when it can): the frozen forward implements a_bit >= 32 and the
+        patch-embedding geometry -- kernel == stride, no padding, dilation 1, groups 1 -- within the library's shape rule
+        (p4v_conv_frozen_ok: K = in_channels * kh * kw and out_channels at most 4096, w_bit in [2, 8])."""
+        if self.a_bit < 32:
+            return f"a_bit = {self.a_bit}: the frozen convolution keeps the activations in FP32 (a_bit >= 32)"
+        if tuple(self.stride) != tuple(self.kernel_size):
+            return f"stride {tuple(self.stride)} != kernel_size {tuple(self.kernel_size)}"
+        if isinstance(self.padding, str) or any(p != 0 for p in self.padding):
+            return f"padding {self.padding!r}: only padding 0"
+        if any(dl != 1 for dl in self.dilation):
+            return f"dilation {tuple(self.dilation)}: only dilation 1"
+        if self.groups != 1:
+            return f"groups = {self.groups}: only groups 1"
+        if self.w_interval is not None and torch.as_tensor(self.w_interval).numel() not in (1, self.out_channels):
+            return f"w_interval has {torch.as_tensor(self.w_interval).numel()} entries: one per output channel or one"
+        ok = ctypes.c_int()
+        d = self._frozen_desc()
+        _lib.check(_lib.lib().p4v_conv_frozen_ok(ctypes.byref(d), ctypes.byref(ok)), "p4v_conv_frozen_ok")
+        if not ok.value:
+            return (f"K = {d.in_channels * d.kernel_h * d.kernel_w}, out_channels = {d.out_channels}, w_bit = {d.w_bit}: "
+                    "outside the shape rule of p4v_conv_frozen_ok")
+        return None
+
+    def freeze(self, weight=None):
+        """Pack the module's integers (the export quantiser's, utils.integer) as bf16 and its step sizes once; until
+        unfreeze(), quant_forward calls that want no gradient run the frozen forward, which reads no FP32 weight.
+        `weight`: quantise this [out, in, kh, kw] tensor instead of self.weight (utils/deploy.py passes the dequantised
+        integers of a saved model)."""
+        if not getattr(self, "calibrated", None):
+            raise RuntimeError(f"freeze() needs a calibrated module: {self}")
+        why = self.frozen_unsupported()
+        if why is not None:
+            raise NotImplementedError(f"{type(self).__name__}.freeze(): {why}")
+        dev = self.weight.device
+        if dev.type != "cuda":
+            raise RuntimeError("ptq4vit_b200 quant layers need their parameters on a CUDA device (no CPU path)")
+        d = self._frozen_desc()
+        lib = _lib.lib()
+        nbytes = ctypes.c_size_t()
+        _lib.check(lib.p4v_conv_pack_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "p4v_conv_pack_bytes")
+        packed = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        w = (self.weight if weight is None else weight).detach().to(dev).reshape(self.out_channels, -1).contiguous().float()
+        wi = torch.as_tensor(self.w_interval, dtype=torch.float32, device=dev).reshape(-1).contiguous()
+        _lib.check(lib.p4v_conv_pack(ctypes.byref(d), _lib.ptr(w), _lib.ptr(wi), _lib.ptr(packed), nbytes.value,
+                                     ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "p4v_conv_pack")
+        self._packed = packed
+        # the step sizes that were packed: the object (kept, so its identity cannot be reused) and its version
+        self._frozen_interval = (self.w_interval, getattr(self.w_interval, "_version", None))
+        return self
+
+    def unfreeze(self):
+        self._packed = self._frozen_interval = None
+        return self
+
+    @property
+    def frozen(self):
+        return self._packed is not None
+
+    def _frozen_forward(self, x):
+        w0, v0 = self._frozen_interval
+        if self.w_interval is not w0 or getattr(self.w_interval, "_version", None) != v0:
+            raise RuntimeError(f"{self}: the step sizes changed after freeze(); call unfreeze() (and freeze() again) "
+                               "before running the layer")
+        dev = self._packed.device
+        x4 = x.to(dev).contiguous().float()
+        if x4.dim() != 4 or x4.shape[1] != self.in_channels:
+            raise ValueError(f"{self}: expected input [images, {self.in_channels}, height, width], got {tuple(x.shape)}")
+        d = self._frozen_desc(x4)
+        out = torch.empty(d.images, self.out_channels, d.height // d.kernel_h, d.width // d.kernel_w, dtype=torch.float32,
+                          device=dev)
+        b = None if self.bias is None else self.bias.detach().contiguous().float()
+        _lib.check(_lib.lib().p4v_conv_frozen_forward(ctypes.byref(d), _lib.ptr(x4), _lib.ptr(b), _lib.ptr(self._packed),
+                                                      self._packed.numel(), _lib.ptr(out),
+                                                      ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                   "p4v_conv_frozen_forward")
+        return out
 
     def calibration_step1(self, x):
         """reference: conv.py:76-81"""

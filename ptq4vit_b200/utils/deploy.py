@@ -1,22 +1,31 @@
 """After calibration: freeze a wrapped model's Linear layers into packed integer weights (and, on request, its MatMul
-modules into packed step sizes), save the quantised model and load it back.  What the reference does right after calibrating (example/test_all.py:31-36 evaluates with quant_forward,
+modules into packed step sizes and its patch-embedding convolution into packed integer weights), save the quantised
+model and load it back.  What the reference does right after calibrating (example/test_all.py:31-36 evaluates with quant_forward,
 example/get_int.py exports the integer weights) as one deployable state.
 
 File format (`torch.save`): {"format": 1, "modules": {name: entry}} with, per wrapped module, its step sizes
 (`w_interval`, `a_interval`, `A_interval`, `B_interval`, `split` -- whichever it has, stored as they are) and, for Linear
-layers on a CUDA device, `w_int`: the int8 weight as `utils.integer.quantize_int_weight` exports it, and `w_bit`.  The
-`w_int` entries alone are what the reference's get_model_int_weight returns.
+layers and conv modules on a CUDA device, `w_int`: the int8 weight as `utils.integer.quantize_int_weight` exports it
+(through the same export quantiser at any w_bit; conv: [out, in, kh, kw]), and `w_bit`.  At W8 the `w_int` entries alone
+are what the reference's get_model_int_weight returns.
 
 Loading freezes every Linear from the integers in the file: the pack kernel is fed with `w_int * step_W` (the block's
 step size) and quantises it again.  That returns the same integers exactly: fl(q * s) = q s (1 + e) with |e| <= 2^-24,
 and the IEEE quotient by s is within |q| * 2^-23 <= 2^-16 of q, far from a rounding tie, so rne gives q.  No FP32
-weight of the module is read, and the frozen forward reads none either.
+weight of the module is read, and the frozen forward reads none either.  The argument holds per step size, so it holds
+for the per-channel step sizes of a conv module as well.
 
 With `matmul=True` the MatMul modules are frozen as well: their step sizes and scale tables are packed once and every
 call runs one fused kernel that quantises both activation operands in shared memory (csrc/forward_mm_tc.cu), with the
 same bits.  A model frozen that way runs its whole quantised forward without host work between kernels, so it can be
-captured in one CUDA graph.  The default leaves the MatMul modules as they are.  The Conv module is never frozen: its
-quant_forward is torch operations on the device and already capturable.
+captured in one CUDA graph.  The default leaves the MatMul modules as they are.
+
+With `conv=True` the patch-embedding convolution is frozen too (a_bit >= 32, kernel == stride, no padding, dilation 1,
+groups 1: every model here): its integers are packed once as bf16 and each call runs one kernel that gathers the patches
+from the image and multiplies the exact three-term bf16 split of the FP32 pixels with them (csrc/forward_conv_tc.cu).
+Unlike the other frozen modules it is not bit-identical to the unfrozen quant_forward, which is cuDNN's F.conv2d (and,
+under torch's default allow_tf32, rounds its operands to TF32): its contract is a bound against fp64 (DESIGN.md section
+4.9).  Loading with `conv=True` freezes the conv from the file's integers; the default leaves it as it is.
 
 `fuse_attention(net)` goes one step further for attention blocks whose two MatMul modules are frozen: the whole core
 between the qkv and proj Linears -- matmul1, the scale, bias and mask, the softmax, matmul2 and the transpose to
@@ -32,6 +41,7 @@ launches instead of four, bit-identical, and the FP32 hidden activations never r
 """
 import torch
 
+from ..quant_layers.conv import MinMaxQuantConv2d
 from ..quant_layers.linear import MinMaxQuantLinear
 from ..quant_layers.matmul import LONG_ATTENTION_TOKENS, SHORT_ATTENTION_TOKENS, MinMaxQuantMatMul
 from . import integer
@@ -40,17 +50,20 @@ from .models import Attention, Mlp, WindowAttention
 INTERVALS = ("w_interval", "a_interval", "A_interval", "B_interval", "split")
 
 
-def _freezes(m, matmul):
+def _freezes(m, matmul, conv=False):
+    if isinstance(m, MinMaxQuantConv2d):
+        return conv and m.weight.device.type == "cuda" and m.frozen_unsupported() is None
     return isinstance(m, MinMaxQuantLinear) or (matmul and isinstance(m, MinMaxQuantMatMul))
 
 
-def freeze_model(wrapped_modules, matmul=False):
-    """Freeze every calibrated Linear and, with matmul=True, every calibrated MatMul; returns the names of the modules
-    left as they are.  By default (matmul=False) the MatMul modules keep their quant_forward and are among the names
-    returned, as before the MatMul modules could be frozen."""
+def freeze_model(wrapped_modules, matmul=False, conv=False):
+    """Freeze every calibrated Linear, with matmul=True every calibrated MatMul and with conv=True every calibrated conv
+    module the frozen convolution implements (MinMaxQuantConv2d.frozen_unsupported() is None, on a CUDA device); returns
+    the names of the modules left as they are.  By default (matmul=False, conv=False) the MatMul and conv modules keep
+    their quant_forward and are among the names returned, as before they could be frozen."""
     left = []
     for name, m in wrapped_modules.items():
-        if _freezes(m, matmul) and getattr(m, "calibrated", None):
+        if getattr(m, "calibrated", None) and _freezes(m, matmul, conv):
             m.freeze()
         else:
             left.append(name)
@@ -59,7 +72,7 @@ def freeze_model(wrapped_modules, matmul=False):
 
 def unfreeze_model(wrapped_modules):
     for m in wrapped_modules.values():
-        if isinstance(m, (MinMaxQuantLinear, MinMaxQuantMatMul)):
+        if isinstance(m, (MinMaxQuantLinear, MinMaxQuantMatMul, MinMaxQuantConv2d)):
             m.unfreeze()
 
 
@@ -133,14 +146,21 @@ def save_quantized(wrapped_modules, path):
             entry["w_int"] = integer._export(m.weight.detach().reshape(O, K), m.w_interval, O // m.n_V, m.n_V, K // m.n_H,
                                              m.n_H, integer.MODE_INT8, m.w_bit).cpu()
             entry["w_bit"] = int(m.w_bit)
+        elif isinstance(m, MinMaxQuantConv2d) and getattr(m, "calibrated", None) and m.weight.device.type == "cuda":
+            O = m.out_channels
+            n_d = torch.as_tensor(m.w_interval).numel()          # one step size per output channel, or one
+            entry["w_int"] = integer._export(m.weight.detach().reshape(O, -1), m.w_interval, O // n_d, n_d, m.weight[0].numel(),
+                                             1, integer.MODE_INT8, m.w_bit).view(m.weight.shape).cpu()
+            entry["w_bit"] = int(m.w_bit)
         modules[name] = entry
     torch.save({"format": 1, "modules": modules}, path)
 
 
-def load_quantized(wrapped_modules, path, matmul=False):
+def load_quantized(wrapped_modules, path, matmul=False, conv=False):
     """Restore the step sizes of every module in the file, mark the modules calibrated and freeze the Linear layers from
-    the file's int8 weights (and, with matmul=True, the MatMul modules from their step sizes).  Returns the names of the
-    modules that were not frozen."""
+    the file's int8 weights (with matmul=True also the MatMul modules from their step sizes, with conv=True also the conv
+    modules from their int8 weights; a conv entry without them stays unfrozen).  Returns the names of the modules that
+    were not frozen."""
     state = torch.load(path, map_location="cpu", weights_only=True)
     if state.get("format") != 1:
         raise RuntimeError(f"{path}: not a ptq4vit_b200 quantised-model file")
@@ -156,7 +176,9 @@ def load_quantized(wrapped_modules, path, matmul=False):
             if k in entry:
                 setattr(m, k, _to(entry[k], device))
         m.calibrated = True
-        if isinstance(m, MinMaxQuantLinear) and "w_int" in entry and m.weight.device.type == "cuda":
+        int_weights = isinstance(m, MinMaxQuantLinear) or \
+            (conv and isinstance(m, MinMaxQuantConv2d) and m.frozen_unsupported() is None)
+        if int_weights and "w_int" in entry and m.weight.device.type == "cuda":
             if entry["w_bit"] != m.w_bit:
                 raise RuntimeError(f"{path}: {name} was saved with w_bit {entry['w_bit']}, the module has {m.w_bit}")
             m.freeze(weight=integer.dequantize_int_weight(m, entry["w_int"].to(device)))

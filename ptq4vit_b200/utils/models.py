@@ -268,6 +268,7 @@ class SwinTransformer(nn.Module):
 
 _SWIN_ZOO = {
     "swin_tiny_patch4_window7_224": dict(img_size=224, dim=96, depths=(2, 2, 6, 2), num_heads=(3, 6, 12, 24), window_size=7),
+    "swin_small_patch4_window7_224": dict(img_size=224, dim=96, depths=(2, 2, 18, 2), num_heads=(3, 6, 12, 24), window_size=7),
     "swin_base_patch4_window7_224": dict(img_size=224, dim=128, depths=(2, 2, 18, 2), num_heads=(4, 8, 16, 32), window_size=7),
     "swin_base_patch4_window12_384": dict(img_size=384, dim=128, depths=(2, 2, 18, 2), num_heads=(4, 8, 16, 32), window_size=12),
 }
@@ -275,9 +276,11 @@ _SWIN_ZOO = {
 
 _ZOO = {
     "vit_tiny_patch16_224": dict(img_size=224, patch=16, dim=192, depth=12, num_heads=3),
+    "vit_small_patch32_224": dict(img_size=224, patch=32, dim=384, depth=12, num_heads=6),
     "vit_small_patch16_224": dict(img_size=224, patch=16, dim=384, depth=12, num_heads=6),
     "vit_base_patch16_224": dict(img_size=224, patch=16, dim=768, depth=12, num_heads=12),
     "vit_base_patch16_384": dict(img_size=384, patch=16, dim=768, depth=12, num_heads=12),
+    "deit_tiny_patch16_224": dict(img_size=224, patch=16, dim=192, depth=12, num_heads=3),
     "deit_small_patch16_224": dict(img_size=224, patch=16, dim=384, depth=12, num_heads=6),
     "deit_base_patch16_224": dict(img_size=224, patch=16, dim=768, depth=12, num_heads=12),
     "deit_base_patch16_384": dict(img_size=384, patch=16, dim=768, depth=12, num_heads=12),
