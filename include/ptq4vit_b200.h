@@ -244,6 +244,31 @@ P4V_API int p4v_mlp_frozen_forward(const p4v_linear_desc* fc1, const float* x, c
  * can be compared with torch.nn.functional.gelu over every fp32 bit pattern. */
 P4V_API int p4v_gelu_probe(const float* x, float* y, long long n, void* stream);
 
+/* A LayerNorm folded into the frozen Linear that consumes it: out = layer(LayerNorm(x)) with torch's exact fp32 LayerNorm
+ * (its vectorised kernel: weight and bias present, in_features % 4 == 0) computed in the fused kernel's activation
+ * quantiser, so the normalised activations never reach HBM.  Bit-identical to torch's F.layer_norm followed by
+ * p4v_linear_frozen_forward.
+ * p4v_linear_norm_ok is the shape rule, a pure function of the descriptor without its rows: the layer is on the fused
+ * path (p4v_linear_frozen_path), not post-GELU, in_features % 4 == 0, and the shared-memory plan with the per-row
+ * statistics fits.  p4v_mlp_norm_ok: the same for fc1 of a fused MLP (p4v_mlp_fused_ok and the plan with the epilogue and
+ * the statistics fits).
+ * p4v_linear_frozen_forward_norm / p4v_mlp_frozen_forward_norm mirror p4v_linear_frozen_forward / p4v_mlp_frozen_forward
+ * with the pre-norm x [rows][in_features] and the LayerNorm's gamma and beta [in_features] (contiguous, 16-byte aligned)
+ * and eps (finite, >= 0).  Every argument is validated before the one launch of the folded layer (the MLP adds fc2's sweep);
+ * nothing is allocated or copied, so both can be captured in a CUDA graph. */
+P4V_API int p4v_linear_norm_ok(const p4v_linear_desc* d, int* ok);
+P4V_API int p4v_mlp_norm_ok(const p4v_linear_desc* fc1, const p4v_linear_desc* fc2, int* ok);
+P4V_API int p4v_linear_frozen_forward_norm(const p4v_linear_desc* d, const float* x, const float* gamma, const float* beta,
+                                           float eps, const float* bias, const void* packed, float* out, void* stream);
+P4V_API int p4v_mlp_frozen_forward_norm(const p4v_linear_desc* fc1, const float* x, const float* gamma, const float* beta,
+                                        float eps, const float* bias1, const void* pack1, size_t pack1_bytes,
+                                        const p4v_linear_desc* fc2, const float* bias2, const void* pack2, size_t pack2_bytes,
+                                        void* workspace, size_t workspace_bytes, float* out, void* stream);
+/* Diagnostic: y = the LayerNorm of the folded kernels applied to each row of x [M][N] (N % 4 == 0, x 16-byte aligned),
+ * so that it can be compared with torch.nn.functional.layer_norm bit for bit. */
+P4V_API int p4v_layer_norm_probe(const float* x, const float* gamma, const float* beta, float eps, long long M, int N, float* y,
+                                 void* stream);
+
 /* The patch-embedding convolution: ChannelwiseBatchingQuantConv2d with a_bit >= 32 (quant_layers/conv.py:444-614, wired
  * by configs/PTQ4ViT.py:52-54): one weight step size per output channel, activations left in FP32.  The caller passes
  * the im2col matrix of the FP32 input (torch.nn.functional.unfold, [images, positions, K], K = in_channels*kh*kw in the

@@ -80,6 +80,12 @@ _SIGNATURES = {
     "p4v_mlp_frozen_forward": [C.POINTER(LinearDesc), _P, _P, _P, C.c_size_t, C.POINTER(LinearDesc), _P, _P, C.c_size_t, _P,
                                C.c_size_t, _P, _P],
     "p4v_gelu_probe": [_P, _P, C.c_longlong, _P],
+    "p4v_linear_norm_ok": [C.POINTER(LinearDesc), C.POINTER(C.c_int)],
+    "p4v_mlp_norm_ok": [C.POINTER(LinearDesc), C.POINTER(LinearDesc), C.POINTER(C.c_int)],
+    "p4v_linear_frozen_forward_norm": [C.POINTER(LinearDesc), _P, _P, _P, C.c_float, _P, _P, _P, _P],
+    "p4v_mlp_frozen_forward_norm": [C.POINTER(LinearDesc), _P, _P, _P, C.c_float, _P, _P, C.c_size_t, C.POINTER(LinearDesc), _P,
+                                    _P, C.c_size_t, _P, C.c_size_t, _P, _P],
+    "p4v_layer_norm_probe": [_P, _P, _P, C.c_float, C.c_longlong, C.c_int, _P, _P],
     "p4v_conv_workspace_bytes": [C.POINTER(ConvDesc), C.POINTER(C.c_size_t)],
     "p4v_conv_calibrate": [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P],
     "p4v_conv_frozen_ok": [C.POINTER(ConvFrozenDesc), C.POINTER(C.c_int)],

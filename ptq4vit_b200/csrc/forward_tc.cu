@@ -18,6 +18,9 @@
 //      fp32 operations in the same order: the output is bit-identical to p4v_linear_quant_forward.
 // With FwdMlpParams the same kernel is fc1 of a fused frozen MLP: step 2's epilogue applies torch's GELU and fc2's
 // activation quantiser and writes fc2's int8 activation image instead of FP32 (see the epilogue below, DESIGN §4.8).
+// With FwdNormParams / FwdMlpNormParams a LayerNorm is folded into step 1: the CTA first computes each row's mean and
+// rstd with torch's exact reduction (forward.cuh, p4v_ln_row_stats) and the quantise loop normalises every value before
+// quantising it (DESIGN §4.10).
 // 288 threads leave 224 registers per thread without setmaxnreg; the bounded mbarrier wait is inline, and the k32 steps of
 // a stage are one straight-line batch selected by a warp-uniform count (ptxas C7520, see sm90.cuh).
 #include <type_traits>
@@ -57,6 +60,12 @@ __device__ __forceinline__ void pack16(uint32_t (&w)[4], int e, float q) {
 // that straddles two column tiles one by one.
 __device__ __forceinline__ unsigned mlp_epi_bytes(const FwdParams&) { return 0u; }
 __device__ __forceinline__ unsigned mlp_epi_bytes(const FwdMlpParams& P) { return P.epi_bytes; }
+
+// shared memory between the weight ring and the control block: the MLP epilogue's, then the LayerNorm row stats
+__device__ __forceinline__ unsigned extra_bytes(const FwdParams&) { return 0u; }
+__device__ __forceinline__ unsigned extra_bytes(const FwdMlpParams& P) { return P.epi_bytes; }
+__device__ __forceinline__ unsigned extra_bytes(const FwdNormParams&) { return P4V_NORM_STATS_BYTES; }
+__device__ __forceinline__ unsigned extra_bytes(const FwdMlpNormParams& P) { return P.epi_bytes + P4V_NORM_STATS_BYTES; }
 
 __device__ __forceinline__ uint8_t* mlp_epi(const FwdMlpParams& P, uint8_t* smem) {
   return smem + P.a_bytes + (size_t)P.n_stages * P.stage_bytes;
@@ -154,23 +163,44 @@ __device__ __forceinline__ void mlp_store_tile(const FwdMlpParams& P, uint8_t* e
   }
 }
 
+template <class Par> constexpr bool kIsMlp = std::is_same<Par, FwdMlpParams>::value || std::is_same<Par, FwdMlpNormParams>::value;
+template <class Par> constexpr bool kIsNorm = std::is_same<Par, FwdNormParams>::value || std::is_same<Par, FwdMlpNormParams>::value;
+
+// The LayerNorm prologue's row stats: mean [128], then rstd [128]
+template <class Par>
+__device__ __forceinline__ float* ln_stats(const Par& P, uint8_t* smem) {
+  return reinterpret_cast<float*>(smem + P.a_bytes + (size_t)P.n_stages * P.stage_bytes + mlp_epi_bytes(P));
+}
+
 // Par = FwdParams: the frozen Linear forward, FP32 output.  Par = FwdMlpParams: fc1 of a frozen MLP, GELU-and-quantise
-// epilogue into fc2's image.
+// epilogue into fc2's image.  FwdNormParams / FwdMlpNormParams: the same with a LayerNorm prologue.
 template <class Par>
 __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_constant__ Par P) {
-  constexpr bool kMlp = std::is_same<Par, FwdMlpParams>::value;
+  constexpr bool kMlp = kIsMlp<Par>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
-  // carve: [resident activation tile][weight ring][MLP epilogue][control]
+  // carve: [resident activation tile][weight ring][MLP epilogue][LayerNorm row stats][control]
   const uint32_t nst = P.n_stages, sC = P.stage_bytes;
   const uint32_t resA = smem_u32(smem), ring = resA + P.a_bytes;
-  FwdCtl& S = *reinterpret_cast<FwdCtl*>(smem + P.a_bytes + (size_t)nst * sC + mlp_epi_bytes(P));
+  FwdCtl& S = *reinterpret_cast<FwdCtl*>(smem + P.a_bytes + (size_t)nst * sC + extra_bytes(P));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // the CTA's row tile and its share of the column tiles
   const int csplit = gridDim.x / P.tiles_m;
   const int tm = blockIdx.x / csplit, cs = blockIdx.x % csplit;
   const int tn0 = cs * P.tiles_n / csplit, tn1 = (cs + 1) * P.tiles_n / csplit;
+
+  // ---- LayerNorm prologue: mean and rstd of every row of the tile, one warp per row (released by the setup barrier) ----
+  if constexpr (kIsNorm<Par>) {
+    float* ln_mean = ln_stats(P, smem);
+    for (int r = warp; r < P4V_TILE; r += kThreads / 32) {
+      const int row = tm * P4V_TILE + r;
+      if (row >= P.M) break;
+      float mean, rstd;
+      p4v_ln_row_stats(P.x + (size_t)row * P.ld, (int)P.ld, P.ln.eps, lane, mean, rstd);
+      if (lane == 0) { ln_mean[r] = mean; ln_mean[P4V_TILE + r] = rstd; }
+    }
+  }
 
   // ---- setup: jobs, chunk table, barriers ----
   for (int i = threadIdx.x; i < P.n_jobs; i += kThreads) S.jobs[i] = P.jobs[i];
@@ -206,6 +236,26 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
         } else {
 #pragma unroll
           for (int e = 0; e < 16; ++e) vals[e] = e < ch.n ? src[e] : 0.f;
+        }
+        if constexpr (kIsNorm<Par>) {
+          const float* ln_mean = ln_stats(P, smem);
+          const float mean = ln_mean[r], rstd = ln_mean[P4V_TILE + r];
+          float g[16], b[16];
+          if (ch.n == 16 && (ch.k0 & 3) == 0) {          // gamma and beta are 16-byte aligned at a multiple of 4
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float4 g4 = __ldg(reinterpret_cast<const float4*>(P.ln.gamma + ch.k0) + e);
+              const float4 b4 = __ldg(reinterpret_cast<const float4*>(P.ln.beta + ch.k0) + e);
+              g[4 * e] = g4.x; g[4 * e + 1] = g4.y; g[4 * e + 2] = g4.z; g[4 * e + 3] = g4.w;
+              b[4 * e] = b4.x; b[4 * e + 1] = b4.y; b[4 * e + 2] = b4.z; b[4 * e + 3] = b4.w;
+            }
+          } else {
+#pragma unroll
+            for (int e = 0; e < 16; ++e) { g[e] = e < ch.n ? __ldg(P.ln.gamma + ch.k0 + e) : 0.f; b[e] = e < ch.n ? __ldg(P.ln.beta + ch.k0 + e) : 0.f; }
+          }
+#pragma unroll
+          for (int e = 0; e < 16; ++e)
+            if (e < ch.n) vals[e] = p4v_ln_apply(vals[e], mean, rstd, g[e], b[e]);
         }
         const float delta = P.dX[ch.a];
         const bool fast = p4v_rint_div_ok(delta);
@@ -355,12 +405,57 @@ int p4v_launch_mlp_fc1_tc(const FwdMlpParams& p, int num_sms, cudaStream_t st) {
   return launch(forward_tc_kernel<FwdMlpParams>, p, p.epi_bytes, num_sms, st);
 }
 
+// The LayerNorm variants: the row stats take P4V_NORM_STATS_BYTES after the (MLP epilogue's) shared memory
+int p4v_launch_forward_norm_tc(const FwdNormParams& p, int num_sms, cudaStream_t st) {
+  P4V_REQUIRE(!p.twin && p.ld % 4 == 0 && p.ln.gamma && p.ln.beta, "forward: bad LayerNorm plan");
+  return launch(forward_tc_kernel<FwdNormParams>, p, P4V_NORM_STATS_BYTES, num_sms, st);
+}
+
+int p4v_launch_mlp_fc1_norm_tc(const FwdMlpNormParams& p, int num_sms, cudaStream_t st) {
+  P4V_REQUIRE(!p.twin && (p.planes2 == 1 || p.planes2 == 2) && p.epi_bytes == p4v_mlp_epi_bytes(p.planes2, p.n_chunks2) &&
+              (reinterpret_cast<uintptr_t>(p.X2) & 15) == 0 && p.ld % 4 == 0 && p.ln.gamma && p.ln.beta,
+              "mlp forward: bad epilogue or LayerNorm plan");
+  return launch(forward_tc_kernel<FwdMlpNormParams>, p, p.epi_bytes + P4V_NORM_STATS_BYTES, num_sms, st);
+}
+
 // Diagnostic: y = p4v_gelu(x) elementwise (the GELU of mlp_fc1_kernel's epilogue)
 extern "C" int p4v_gelu_probe(const float* x, float* y, long long n, void* stream) {
   P4V_REQUIRE(x && y && n >= 0, "gelu_probe: null pointer or negative count");
   if (n == 0) return 0;
   const long long blocks = (n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096;
   gelu_probe_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, y, n);
+  p4v_count_launch();
+  P4V_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+namespace {
+
+// one warp per row
+__global__ void layer_norm_probe_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
+                                        const float* __restrict__ beta, float eps, long long M, int N, float* __restrict__ y) {
+  const int lane = threadIdx.x & 31;
+  for (long long row = blockIdx.x * (long long)(blockDim.x / 32) + (threadIdx.x >> 5); row < M;
+       row += (long long)gridDim.x * (blockDim.x / 32)) {
+    const float* xr = x + row * N;
+    float mean, rstd;
+    p4v_ln_row_stats(xr, N, eps, lane, mean, rstd);
+    for (int k = lane; k < N; k += 32) y[row * N + k] = p4v_ln_apply(xr[k], mean, rstd, gamma[k], beta[k]);
+  }
+}
+
+}  // namespace
+
+// Diagnostic: y = LayerNorm(x) row by row for [M][N] x (the LayerNorm of the fused kernel's prologue)
+extern "C" int p4v_layer_norm_probe(const float* x, const float* gamma, const float* beta, float eps, long long M, int N, float* y,
+                                    void* stream) {
+  P4V_REQUIRE(x && gamma && beta && y && M >= 0, "layer_norm_probe: null pointer or negative count");
+  P4V_REQUIRE(N > 0 && N % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0, "layer_norm_probe: N must be a positive "
+              "multiple of 4 and x 16-byte aligned");
+  P4V_REQUIRE(eps >= 0.f && eps <= 3.4e38f, "layer_norm_probe: eps must be finite and non-negative");
+  if (M == 0) return 0;
+  const long long blocks = (M + 7) / 8 < 4096 ? (M + 7) / 8 : 4096;
+  layer_norm_probe_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, gamma, beta, eps, M, N, y);
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   return 0;

@@ -843,6 +843,7 @@ namespace {
 struct MlpPlan {
   FrozenPlan f1, f2;
   int stages;         // ring stages of fc1's kernel with the epilogue; 0: the MLP does not fuse
+  int stages_norm;    // the same with a LayerNorm folded into fc1 (norm_ring_stages); 0: the LayerNorm does not fold
   int planes2, chunks2;
 };
 
@@ -854,9 +855,13 @@ int build_mlp(const p4v_linear_desc* d1, const p4v_linear_desc* d2, MlpPlan& m, 
   const LinPlan &p1 = m.f1.p, &p2 = m.f2.p;
   m.planes2 = p2.twin ? 2 : 1;
   m.chunks2 = p2.Wcur.kb / 16;      // a plane of fc2's activation image has the K layout of its weight image
-  m.stages = 0;
-  if (p1.O == p2.K && !p1.twin && m.f1.stages >= 2)
+  m.stages = m.stages_norm = 0;
+  if (p1.O == p2.K && !p1.twin && m.f1.stages >= 2) {
     m.stages = mlp_ring_stages(m.f1.X.tile_bytes(), (size_t)m.f1.stage_kb * P4V_TILE, p1.Wcur.kb / 16, m.planes2, m.chunks2);
+    if (m.stages >= 2 && p1.K % 4 == 0)
+      m.stages_norm = mlp_ring_stages(m.f1.X.tile_bytes() + P4V_NORM_STATS_BYTES, (size_t)m.f1.stage_kb * P4V_TILE,
+                                      p1.Wcur.kb / 16, m.planes2, m.chunks2);
+  }
   return 0;
 }
 
@@ -909,5 +914,94 @@ extern "C" int p4v_mlp_frozen_forward(const p4v_linear_desc* fc1, const float* x
   q.d_neg2 = l2.d_neg; q.lo2 = l2.twin ? 0.f : (float)-l2.a_qmax; q.hi2 = (float)(l2.a_qmax - 1); q.neg_lo2 = (float)-l2.a_qmax;
   q.epi_bytes = p4v_mlp_epi_bytes(m.planes2, m.chunks2);
   if ((rc = p4v_launch_mlp_fc1_tc(q, p4v_num_sms(), st))) return rc;
+  return streamed_sweep(m.f2, p2, workspace, bias2, out, st);
+}
+
+// ---- LayerNorm folded into the activation quantiser of the fused kernel (forward_tc.cu, DESIGN §4.10) -------------
+namespace {
+
+// Ring stages of the fused kernel with the LayerNorm prologue; 0: the LayerNorm does not fold into this layer
+int norm_stages(const FrozenPlan& f) {
+  const LinPlan& p = f.p;
+  if (f.stages < 2 || p.twin || p.K % 4 != 0) return 0;
+  return norm_ring_stages(f.X.tile_bytes(), (size_t)f.stage_kb * P4V_TILE, p.Wcur.kb / 16);
+}
+
+// The arguments of the LayerNorm shared by both entry points
+int check_norm(const char* what, const float* x, const float* gamma, const float* beta, float eps) {
+  P4V_REQUIRE(x && gamma && beta, "%s: null pointer", what);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(gamma) & 15) == 0 &&
+              (reinterpret_cast<uintptr_t>(beta) & 15) == 0, "%s: x, gamma and beta must be 16-byte aligned", what);
+  P4V_REQUIRE(eps >= 0.f && eps <= 3.4028234663852886e38f, "%s: eps must be finite and non-negative (got %g)", what, (double)eps);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int p4v_linear_norm_ok(const p4v_linear_desc* d, int* ok) {
+  FrozenPlan f; int rc = build_frozen(d, f, true);
+  if (rc) return rc;
+  P4V_REQUIRE(ok != nullptr, "null output");
+  *ok = norm_stages(f) >= 2 ? 1 : 0;
+  return 0;
+}
+
+extern "C" int p4v_mlp_norm_ok(const p4v_linear_desc* fc1, const p4v_linear_desc* fc2, int* ok) {
+  MlpPlan m; int rc = build_mlp(fc1, fc2, m, true);
+  if (rc) return rc;
+  P4V_REQUIRE(ok != nullptr, "null output");
+  *ok = m.stages_norm >= 2 ? 1 : 0;
+  return 0;
+}
+
+extern "C" int p4v_linear_frozen_forward_norm(const p4v_linear_desc* d, const float* x, const float* gamma, const float* beta,
+                                              float eps, const float* bias, const void* packed_in, float* out, void* stream) {
+  FrozenPlan f; int rc = build_frozen(d, f, false);
+  if (rc) return rc;
+  if ((rc = check_norm("linear_frozen_forward_norm", x, gamma, beta, eps))) return rc;
+  P4V_REQUIRE(packed_in && out, "linear_frozen_forward_norm: null pointer");
+  P4V_REQUIRE(!d->has_bias || bias, "linear_frozen_forward_norm: has_bias set but bias is null");
+  const int stages = norm_stages(f);
+  P4V_REQUIRE(stages >= 2, "linear_frozen_forward_norm: the LayerNorm does not fold into this layer (p4v_linear_norm_ok)");
+  FwdNormParams q{};
+  fill_fwd(f, x, bias, const_cast<void*>(packed_in), out, q);
+  q.n_stages = (unsigned)stages;
+  q.ln = FwdNorm{gamma, beta, eps};
+  return p4v_launch_forward_norm_tc(q, p4v_num_sms(), (cudaStream_t)stream);
+}
+
+extern "C" int p4v_mlp_frozen_forward_norm(const p4v_linear_desc* fc1, const float* x, const float* gamma, const float* beta,
+                                           float eps, const float* bias1, const void* pack1, size_t pack1_bytes,
+                                           const p4v_linear_desc* fc2, const float* bias2, const void* pack2, size_t pack2_bytes,
+                                           void* workspace, size_t workspace_bytes, float* out, void* stream) {
+  MlpPlan m; int rc = build_mlp(fc1, fc2, m, false);
+  if (rc) return rc;
+  if ((rc = check_norm("mlp_frozen_forward_norm", x, gamma, beta, eps))) return rc;
+  P4V_REQUIRE(fc1->rows == fc2->rows, "mlp_frozen_forward_norm: fc1 and fc2 must have the same rows (%d != %d)", fc1->rows,
+              fc2->rows);
+  P4V_REQUIRE(pack1 && pack2 && workspace && out, "mlp_frozen_forward_norm: null pointer");
+  P4V_REQUIRE((!fc1->has_bias || bias1) && (!fc2->has_bias || bias2), "mlp_frozen_forward_norm: has_bias set but bias is null");
+  P4V_REQUIRE(m.stages_norm >= 2, "mlp_frozen_forward_norm: these layers do not fuse with the LayerNorm (p4v_mlp_norm_ok)");
+  P4V_REQUIRE(pack1_bytes >= m.f1.bytes && pack2_bytes >= m.f2.bytes, "mlp_frozen_forward_norm: packed buffer too small "
+              "(fc1 %zu < %zu or fc2 %zu < %zu)", pack1_bytes, m.f1.bytes, pack2_bytes, m.f2.bytes);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(out) & 7) == 0 && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0,
+              "mlp_frozen_forward_norm: workspace must be 16-byte and out 8-byte aligned");
+  P4V_REQUIRE(workspace_bytes >= m.f2.X.bytes(), "mlp_frozen_forward_norm: workspace too small (%zu < %zu)", workspace_bytes,
+              m.f2.X.bytes());
+  cudaStream_t st = (cudaStream_t)stream;
+  void* p1 = const_cast<void*>(pack1);
+  void* p2 = const_cast<void*>(pack2);
+  const LinPlan& l2 = m.f2.p;
+  FwdMlpNormParams q{};
+  fill_fwd(m.f1, x, bias1, p1, nullptr, q);
+  q.n_stages = (unsigned)m.stages_norm;
+  q.X2 = m.f2.X.ptr(workspace); q.X2_tile_bytes = m.f2.X.tile_bytes(); q.X2_plane_bytes = (unsigned)l2.Wcur.tile_bytes();
+  q.segs2 = l2.segsX.dev(p2); q.nseg2 = (int)l2.segs.size();
+  q.n_chunks2 = m.chunks2; q.planes2 = m.planes2;
+  q.dX2 = at<float>(p2, m.f2.o_dX); q.crb_acts2 = l2.crb_acts;
+  q.d_neg2 = l2.d_neg; q.lo2 = l2.twin ? 0.f : (float)-l2.a_qmax; q.hi2 = (float)(l2.a_qmax - 1); q.neg_lo2 = (float)-l2.a_qmax;
+  q.epi_bytes = p4v_mlp_epi_bytes(m.planes2, m.chunks2);
+  q.ln = FwdNorm{gamma, beta, eps};
+  if ((rc = p4v_launch_mlp_fc1_norm_tc(q, p4v_num_sms(), st))) return rc;
   return streamed_sweep(m.f2, p2, workspace, bias2, out, st);
 }

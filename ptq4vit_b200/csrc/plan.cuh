@@ -113,6 +113,13 @@ inline int mlp_ring_stages(size_t a_bytes1, size_t stage_bytes1, size_t plane_ch
   return frozen_ring_stages(a_bytes1 + p4v_mlp_epi_bytes(planes2, plane_chunks2), stage_bytes1, plane_chunks1);
 }
 
+// A frozen layer with a LayerNorm folded into its fused kernel (forward_tc.cu with FwdNormParams): the ring stages when
+// the per-row mean and rstd of the tile take their share of shared memory.  0: the LayerNorm does not fold.  The plain
+// layer's own stage count (frozen_ring_stages) is not changed by this.
+inline int norm_ring_stages(size_t a_bytes, size_t stage_bytes, size_t plane_chunks) {
+  return frozen_ring_stages(a_bytes + P4V_NORM_STATS_BYTES, stage_bytes, plane_chunks);
+}
+
 // A commit copies the chosen candidate's slabs from the planes of cand into cur
 inline void fill_images(CommitArgs& c, void* ws, const Image& cand, const Image& cur) {
   c.cand = cand.ptr(ws); c.cand_tile_bytes = cand.tile_bytes(); c.cand_plane_stride = cand.plane_stride();

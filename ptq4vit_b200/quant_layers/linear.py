@@ -264,10 +264,12 @@ def frozen_mlp_applies(fc1, fc2, act, x):
     return bool(ok.value)
 
 
-def frozen_mlp(fc1, fc2, x):
+def frozen_mlp(fc1, fc2, x, norm=None):
     """fc2(gelu(fc1(x))) of two frozen layers in two launches (csrc/forward_tc.cu: fc1 with a GELU-and-quantise
     epilogue writing fc2's int8 activation image; fc2's sweep forward), for a call where frozen_mlp_applies holds.  The
-    bits are those of the unfused sequence.  fc2's image is kept between calls in fc2's frozen workspace."""
+    bits are those of the unfused sequence.  fc2's image is kept between calls in fc2's frozen workspace.
+    With `norm` (an nn.LayerNorm for which frozen_norm_applies(norm, fc1, x) and frozen_mlp_norm_ok(fc1, fc2) hold):
+    fc2(gelu(fc1(norm(x)))), the LayerNorm folded into fc1's activation quantiser, still two launches."""
     fc1._check_frozen_intervals()
     fc2._check_frozen_intervals()
     dev = fc1._packed.device
@@ -283,12 +285,73 @@ def frozen_mlp(fc1, fc2, x):
     out = torch.empty(x2.shape[0], fc2.out_features, dtype=torch.float32, device=dev)
     b1 = None if fc1.bias is None else fc1.bias.detach().contiguous().float()
     b2 = None if fc2.bias is None else fc2.bias.detach().contiguous().float()
+    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    if norm is not None:
+        _lib.check(lib.p4v_mlp_frozen_forward_norm(ctypes.byref(d1), _lib.ptr(x2), _lib.ptr(norm.weight), _lib.ptr(norm.bias),
+                                                   float(norm.eps), _lib.ptr(b1), _lib.ptr(fc1._packed), fc1._packed.numel(),
+                                                   ctypes.byref(d2), _lib.ptr(b2), _lib.ptr(fc2._packed), fc2._packed.numel(),
+                                                   _lib.ptr(ws), ws.numel(), _lib.ptr(out), stream),
+                   "p4v_mlp_frozen_forward_norm")
+        return out.reshape(*x.shape[:-1], fc2.out_features)
     _lib.check(lib.p4v_mlp_frozen_forward(ctypes.byref(d1), _lib.ptr(x2), _lib.ptr(b1), _lib.ptr(fc1._packed), fc1._packed.numel(),
                                           ctypes.byref(d2), _lib.ptr(b2), _lib.ptr(fc2._packed), fc2._packed.numel(),
                                           _lib.ptr(ws), ws.numel(), _lib.ptr(out),
                                           ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
                "p4v_mlp_frozen_forward")
     return out.reshape(*x.shape[:-1], fc2.out_features)
+
+
+def frozen_norm_applies(norm, lin, x):
+    """Whether lin(norm(x)) can run as one folded call (frozen_norm_linear): `norm` exactly an nn.LayerNorm with weight and
+    bias over lin.in_features, `lin` a frozen Linear layer in quant_forward mode whose shape holds the fold
+    (p4v_linear_norm_ok: on the fused kernel, not post-GELU, in_features % 4 == 0, the shared-memory plan fits), x FP32 on
+    lin's device, under grad mode no input and no parameter of norm or lin that requires grad, and the case in which torch
+    itself runs its vectorised LayerNorm kernel (FP32 weight and bias, 16-byte aligned data) -- the kernel whose bits the
+    fold reproduces (DESIGN.md section 4.10)."""
+    if type(norm) is not nn.LayerNorm or norm.weight is None or norm.bias is None:
+        return False
+    if not (isinstance(lin, MinMaxQuantLinear) and lin.frozen and lin.mode == "quant_forward"):
+        return False
+    if tuple(norm.normalized_shape) != (lin.in_features,) or lin.in_features % 4 != 0:
+        return False
+    dev = lin._packed.device
+    if x.dtype != torch.float32 or x.device != dev or x.numel() == 0:
+        return False
+    if any(p.dtype != torch.float32 or p.device != dev or not p.is_contiguous() or p.data_ptr() % 16 for p in (norm.weight, norm.bias)):
+        return False
+    if x.is_contiguous() and x.data_ptr() % 16:       # torch normalises a non-contiguous x from an aligned copy
+        return False
+    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in (norm, lin) for p in m.parameters())):
+        return False
+    ok = ctypes.c_int()
+    _lib.check(_lib.lib().p4v_linear_norm_ok(ctypes.byref(lin._desc(1, 1)), ctypes.byref(ok)), "p4v_linear_norm_ok")
+    return bool(ok.value)
+
+
+def frozen_mlp_norm_ok(fc1, fc2):
+    """The shape rule of frozen_mlp(..., norm=): fc1 and fc2 fuse (p4v_mlp_fused_ok) and the plan with the LayerNorm's
+    row statistics still fits (p4v_mlp_norm_ok)."""
+    ok = ctypes.c_int()
+    _lib.check(_lib.lib().p4v_mlp_norm_ok(ctypes.byref(fc1._desc(1, 1)), ctypes.byref(fc2._desc(1, 1)), ctypes.byref(ok)),
+               "p4v_mlp_norm_ok")
+    return bool(ok.value)
+
+
+def frozen_norm_linear(norm, lin, x):
+    """lin(norm(x)) in one launch, for a call where frozen_norm_applies(norm, lin, x) holds: torch's exact LayerNorm
+    computed in the activation quantiser of lin's fused kernel (csrc/forward_tc.cu), bit-identical to the unfolded call;
+    the normalised activations never reach HBM.  Only the output is allocated."""
+    lin._check_frozen_intervals()
+    dev = lin._packed.device
+    x2 = _flat2d(x.to(dev))
+    d = lin._desc(x2.shape[0], 1)
+    out = torch.empty(x2.shape[0], lin.out_features, dtype=torch.float32, device=dev)
+    b = None if lin.bias is None else lin.bias.detach().contiguous().float()
+    _lib.check(_lib.lib().p4v_linear_frozen_forward_norm(ctypes.byref(d), _lib.ptr(x2), _lib.ptr(norm.weight), _lib.ptr(norm.bias),
+                                                         float(norm.eps), _lib.ptr(b), _lib.ptr(lin._packed), _lib.ptr(out),
+                                                         ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+               "p4v_linear_frozen_forward_norm")
+    return out.reshape(*x.shape[:-1], lin.out_features)
 
 
 class PTQSLQuantLinear(MinMaxQuantLinear):

@@ -38,6 +38,13 @@ values of a head once and recomputes the scores instead of storing them (csrc/fo
 activation quantiser in its epilogue and writes fc2's int8 activation image, which fc2's sweep forward reads -- two
 launches instead of four, bit-identical, and the FP32 hidden activations never reach HBM.  Opt-in as well;
 `unfuse_mlp(net)` undoes it.
+
+`fuse_norm(net)` folds a LayerNorm into the frozen Linear that consumes it (a pre-norm block's norm1 -> attn.qkv and
+norm2 -> mlp.fc1, Swin's norm2 -> fc1, PatchMerging's norm -> reduction, a ViT's final norm -> head, of which only the cls
+rows are normalised): torch's exact LayerNorm runs in the Linear's activation quantiser, one launch instead of two and
+no normalised tensor in HBM, bit-identical.  It composes with fuse_attention and fuse_mlp (norm2, fc1, GELU and fc2's
+quantiser in one kernel).  A folded call skips the LayerNorm's forward hooks, so it is opt-in; `unfuse_norm(net)` undoes
+it.  None of the fusions is recorded by save_quantized: apply them again after load_quantized.
 """
 import torch
 
@@ -45,7 +52,7 @@ from ..quant_layers.conv import MinMaxQuantConv2d
 from ..quant_layers.linear import MinMaxQuantLinear
 from ..quant_layers.matmul import LONG_ATTENTION_TOKENS, SHORT_ATTENTION_TOKENS, MinMaxQuantMatMul
 from . import integer
-from .models import Attention, Mlp, WindowAttention
+from .models import Attention, Block, Mlp, PatchMerging, SwinBlock, VisionTransformer, WindowAttention
 
 INTERVALS = ("w_interval", "a_interval", "A_interval", "B_interval", "split")
 
@@ -126,6 +133,44 @@ def unfuse_mlp(net):
     for m in net.modules():
         if isinstance(m, Mlp):
             m.fused = False
+
+
+def _norm_sites(m):
+    """The (flag, LayerNorm, consuming Linear) fold sites of module m"""
+    if isinstance(m, Block):
+        return [("fold_norm1", m.norm1, m.attn.qkv), ("fold_norm2", m.norm2, m.mlp.fc1)]
+    if isinstance(m, SwinBlock):
+        return [("fold_norm2", m.norm2, m.mlp.fc1)]
+    if isinstance(m, PatchMerging):
+        return [("fold_norm", m.norm, m.reduction)]
+    if isinstance(m, VisionTransformer):
+        return [("fold_norm", m.norm, m.head)]
+    return []
+
+
+def fuse_norm(net):
+    """Mark every LayerNorm fold site of `net` whose consumer is a frozen Linear layer: Block.norm1 -> attn.qkv,
+    Block.norm2 -> mlp.fc1, SwinBlock.norm2 -> mlp.fc1, PatchMerging.norm -> reduction and VisionTransformer.norm -> head.
+    Each call that qualifies (quant_layers.linear.frozen_norm_applies: an affine nn.LayerNorm over in_features, torch's
+    vectorised case, no gradient wanted, a shape the fused kernel holds) normalises its input inside the Linear's
+    activation quantiser, with the bits of the unfolded call; any other call runs the LayerNorm and the Linear as before.
+    A folded call skips the LayerNorm's forward hooks, which is why the fold is opt-in.  It composes with fuse_attention
+    and fuse_mlp; save_quantized / load_quantized do not record it.  Returns the names of the LayerNorm modules left
+    unfolded (Swin's norm1, final norm and patch_norm always are)."""
+    folded = set()
+    for m in net.modules():
+        for flag, norm, lin in _norm_sites(m):
+            on = isinstance(lin, MinMaxQuantLinear) and lin.frozen
+            setattr(m, flag, on)
+            if on:
+                folded.add(id(norm))
+    return [name for name, m in net.named_modules() if isinstance(m, torch.nn.LayerNorm) and id(m) not in folded]
+
+
+def unfuse_norm(net):
+    for m in net.modules():
+        for flag, _norm, _lin in _norm_sites(m):
+            setattr(m, flag, False)
 
 
 def _to(v, device):

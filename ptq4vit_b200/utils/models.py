@@ -5,8 +5,16 @@ available offline, so weights are synthetic (trunc-normal 0.02) -- this is harne
 import torch
 import torch.nn as nn
 
-from ..quant_layers.linear import frozen_mlp, frozen_mlp_applies
+from ..quant_layers.linear import (frozen_mlp, frozen_mlp_applies, frozen_mlp_norm_ok, frozen_norm_applies,
+                                   frozen_norm_linear)
 from ..quant_layers.matmul import frozen_attention, frozen_attention_applies
+
+
+def _norm_linear(norm, lin, x):
+    """lin(norm(x)): folded into one call when frozen_norm_applies holds, else the two modules as they are."""
+    if frozen_norm_applies(norm, lin, x):
+        return frozen_norm_linear(norm, lin, x)
+    return lin(norm(x))
 
 
 class MatMul(nn.Module):
@@ -28,9 +36,10 @@ class Attention(nn.Module):
     fused_max_tokens = 256   # set by utils.deploy.fuse_attention: sequences up to this length run fused (the long
                              # kernel above 256 tokens)
 
-    def forward(self, x):
+    def forward(self, x, norm=None):
+        """norm: a LayerNorm to apply to x first (Block with fold_norm1), folded into qkv when it applies."""
         B, N, C = x.shape
-        y = self.qkv(x)
+        y = self.qkv(x) if norm is None else _norm_linear(norm, self.qkv, x)
         if self.fused and frozen_attention_applies(self.matmul1, self.matmul2, N, C // self.num_heads, y,
                                                    max_tokens=self.fused_max_tokens):
             qkv5 = y.reshape(B, N, 3, self.num_heads, C // self.num_heads)
@@ -53,7 +62,15 @@ class Mlp(nn.Module):
 
     fused = False      # set by utils.deploy.fuse_mlp: run fc1, GELU and fc2 as the fused frozen MLP when it applies
 
-    def forward(self, x):
+    def forward(self, x, norm=None):
+        """norm: a LayerNorm to apply to x first (Block / SwinBlock with fold_norm2), folded into fc1 when it applies."""
+        if norm is not None:
+            if frozen_norm_applies(norm, self.fc1, x):
+                if not (self.fused and frozen_mlp_applies(self.fc1, self.fc2, self.act, x)):
+                    return self.fc2(self.act(frozen_norm_linear(norm, self.fc1, x)))
+                if frozen_mlp_norm_ok(self.fc1, self.fc2):
+                    return frozen_mlp(self.fc1, self.fc2, x, norm=norm)
+            x = norm(x)
         if self.fused and frozen_mlp_applies(self.fc1, self.fc2, self.act, x):
             return frozen_mlp(self.fc1, self.fc2, x)
         return self.fc2(self.act(self.fc1(x)))
@@ -67,9 +84,15 @@ class Block(nn.Module):
         self.norm2 = nn.LayerNorm(dim, eps=1e-6)
         self.mlp = Mlp(dim, int(dim * mlp_ratio))
 
+    fold_norm1 = False     # set by utils.deploy.fuse_norm: hand norm1 to attn, which folds it into qkv when it applies
+    fold_norm2 = False     # set by utils.deploy.fuse_norm: hand norm2 to mlp, which folds it into fc1 when it applies
+
     def forward(self, x):
-        x = x + self.attn(self.norm1(x))
-        return x + self.mlp(self.norm2(x))
+        if not (self.fold_norm1 or self.fold_norm2):
+            x = x + self.attn(self.norm1(x))
+            return x + self.mlp(self.norm2(x))
+        x = x + (self.attn(x, norm=self.norm1) if self.fold_norm1 else self.attn(self.norm1(x)))
+        return x + (self.mlp(x, norm=self.norm2) if self.fold_norm2 else self.mlp(self.norm2(x)))
 
 
 class PatchEmbed(nn.Module):
@@ -106,10 +129,16 @@ class VisionTransformer(nn.Module):
             self.head.weight.mul_(8.0)
             self.pos_embed.copy_(torch.nn.init.trunc_normal_(torch.empty_like(self.pos_embed), std=0.02, generator=gen))
 
+    fold_norm = False      # set by utils.deploy.fuse_norm: fold norm into head, normalising only the cls rows
+
     def forward(self, x):
         x = self.patch_embed(x)
         x = torch.cat([self.cls_token.expand(x.shape[0], -1, -1), x], dim=1) + self.pos_embed
-        x = self.norm(self.blocks(x))
+        x = self.blocks(x)
+        # LayerNorm is per row: the cls rows normalised alone have the bits of the whole tensor's cls rows
+        if self.fold_norm and frozen_norm_applies(self.norm, self.head, x):
+            return frozen_norm_linear(self.norm, self.head, x[:, 0])
+        x = self.norm(x)
         return self.head(x[:, 0])
 
 
@@ -195,6 +224,8 @@ class SwinBlock(nn.Module):
             mask = mask.masked_fill(mask != 0, -100.0).masked_fill(mask == 0, 0.0)
         self.register_buffer("attn_mask", mask)
 
+    fold_norm2 = False     # set by utils.deploy.fuse_norm, as Block.fold_norm2
+
     def forward(self, x):
         B, L, C = x.shape
         H = W = self.res
@@ -206,6 +237,8 @@ class SwinBlock(nn.Module):
         if self.shift > 0:
             h = torch.roll(h, shifts=(self.shift, self.shift), dims=(1, 2))
         x = x + h.view(B, L, C)
+        if self.fold_norm2:
+            return x + self.mlp(x, norm=self.norm2)
         return x + self.mlp(self.norm2(x))
 
 
@@ -216,10 +249,14 @@ class PatchMerging(nn.Module):
         self.norm = nn.LayerNorm(4 * dim)
         self.reduction = nn.Linear(4 * dim, 2 * dim, bias=False)
 
+    fold_norm = False      # set by utils.deploy.fuse_norm: fold norm into reduction when it applies
+
     def forward(self, x):
         B, L, C = x.shape
         x = x.view(B, self.res, self.res, C)
         x = torch.cat([x[:, 0::2, 0::2], x[:, 1::2, 0::2], x[:, 0::2, 1::2], x[:, 1::2, 1::2]], -1).view(B, -1, 4 * C)
+        if self.fold_norm:
+            return _norm_linear(self.norm, self.reduction, x)
         return self.reduction(self.norm(x))
 
 
