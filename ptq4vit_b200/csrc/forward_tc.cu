@@ -23,8 +23,6 @@
 // quantising it (DESIGN §4.10).
 // 288 threads leave 224 registers per thread without setmaxnreg; the bounded mbarrier wait is inline, and the k32 steps of
 // a stage are one straight-line batch selected by a warp-uniform count (ptxas C7520, see sm90.cuh).
-#include <type_traits>
-
 #include "../../include/ptq4vit_b200.h"
 #include "forward.cuh"
 #include "sm90.cuh"
@@ -58,15 +56,6 @@ __device__ __forceinline__ void pack16(uint32_t (&w)[4], int e, float q) {
 // to the column tile of its source column; a padding byte to that of its segment's last column.  Every byte of the image
 // then has exactly one owner, and a CTA stores whole chunks it owns as one 16-byte store and the owned bytes of a chunk
 // that straddles two column tiles one by one.
-__device__ __forceinline__ unsigned mlp_epi_bytes(const FwdParams&) { return 0u; }
-__device__ __forceinline__ unsigned mlp_epi_bytes(const FwdMlpParams& P) { return P.epi_bytes; }
-
-// shared memory between the weight ring and the control block: the MLP epilogue's, then the LayerNorm row stats
-__device__ __forceinline__ unsigned extra_bytes(const FwdParams&) { return 0u; }
-__device__ __forceinline__ unsigned extra_bytes(const FwdMlpParams& P) { return P.epi_bytes; }
-__device__ __forceinline__ unsigned extra_bytes(const FwdNormParams&) { return P4V_NORM_STATS_BYTES; }
-__device__ __forceinline__ unsigned extra_bytes(const FwdMlpNormParams& P) { return P.epi_bytes + P4V_NORM_STATS_BYTES; }
-
 __device__ __forceinline__ uint8_t* mlp_epi(const FwdMlpParams& P, uint8_t* smem) {
   return smem + P.a_bytes + (size_t)P.n_stages * P.stage_bytes;
 }
@@ -163,13 +152,11 @@ __device__ __forceinline__ void mlp_store_tile(const FwdMlpParams& P, uint8_t* e
   }
 }
 
-template <class Par> constexpr bool kIsMlp = std::is_same<Par, FwdMlpParams>::value || std::is_same<Par, FwdMlpNormParams>::value;
-template <class Par> constexpr bool kIsNorm = std::is_same<Par, FwdNormParams>::value || std::is_same<Par, FwdMlpNormParams>::value;
-
-// The LayerNorm prologue's row stats: mean [128], then rstd [128]
+// The LayerNorm prologue's row stats, the last P4V_NORM_STATS_BYTES before the control block: mean [128], then rstd [128]
 template <class Par>
 __device__ __forceinline__ float* ln_stats(const Par& P, uint8_t* smem) {
-  return reinterpret_cast<float*>(smem + P.a_bytes + (size_t)P.n_stages * P.stage_bytes + mlp_epi_bytes(P));
+  return reinterpret_cast<float*>(smem + P.a_bytes + (size_t)P.n_stages * P.stage_bytes +
+                                  (p4v_fwd_extra_bytes(P) - P4V_NORM_STATS_BYTES));
 }
 
 // Par = FwdParams: the frozen Linear forward, FP32 output.  Par = FwdMlpParams: fc1 of a frozen MLP, GELU-and-quantise
@@ -182,7 +169,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
   // carve: [resident activation tile][weight ring][MLP epilogue][LayerNorm row stats][control]
   const uint32_t nst = P.n_stages, sC = P.stage_bytes;
   const uint32_t resA = smem_u32(smem), ring = resA + P.a_bytes;
-  FwdCtl& S = *reinterpret_cast<FwdCtl*>(smem + P.a_bytes + (size_t)nst * sC + extra_bytes(P));
+  FwdCtl& S = *reinterpret_cast<FwdCtl*>(smem + P.a_bytes + (size_t)nst * sC + p4v_fwd_extra_bytes(P));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // the CTA's row tile and its share of the column tiles
@@ -375,48 +362,35 @@ __global__ void gelu_probe_kernel(const float* __restrict__ x, float* __restrict
     y[i] = p4v_gelu(x[i]);
 }
 
-template <class Par>
-int launch(void (*kernel)(Par), const Par& p, unsigned epi_bytes, int num_sms, cudaStream_t st) {
+}  // namespace
+
+template <class Par> int p4v_launch_forward_tc(const Par& p, int num_sms, cudaStream_t st) {
+  if constexpr (kIsMlp<Par>)
+    P4V_REQUIRE(!p.twin && (p.planes2 == 1 || p.planes2 == 2) && p.epi_bytes == p4v_mlp_epi_bytes(p.planes2, p.n_chunks2) &&
+                (reinterpret_cast<uintptr_t>(p.X2) & 15) == 0, "mlp forward: bad epilogue plan");
+  if constexpr (kIsNorm<Par>) P4V_REQUIRE(!p.twin && p.ld % 4 == 0 && p.ln.gamma && p.ln.beta, "forward: bad LayerNorm plan");
+  const unsigned extra = p4v_fwd_extra_bytes(p);
   P4V_REQUIRE(p.n_jobs >= 1 && p.n_jobs <= P4V_MAX_JOBS && p.n_groups <= P4V_MAX_GROUPS, "forward: too many K segments");
   P4V_REQUIRE(p.n_stages >= 2 && p.n_stages <= P4V_FWD_MAX_STAGES && p.n_chunks <= P4V_FWD_MAX_CHUNKS &&
-              p.stage_bytes % 128 == 0 && p.a_bytes % 128 == 0 && epi_bytes % 128 == 0, "forward: bad shared-memory plan");
+              p.stage_bytes % 128 == 0 && p.a_bytes % 128 == 0 && extra % 128 == 0, "forward: bad shared-memory plan");
   P4V_REQUIRE((reinterpret_cast<uintptr_t>(p.out) & 7) == 0 && (reinterpret_cast<uintptr_t>(p.x) & 15) == 0,
               "forward: x must be 16-byte and out 8-byte aligned");
-  const size_t smem = (size_t)p.a_bytes + (size_t)p.n_stages * p.stage_bytes + epi_bytes + sizeof(FwdCtl) + 128;
+  const size_t smem = (size_t)p.a_bytes + (size_t)p.n_stages * p.stage_bytes + extra + sizeof(FwdCtl) + 128;
   P4V_REQUIRE(smem <= P4V_FWD_SMEM, "forward: shared-memory plan too large (%zu bytes)", smem);
   // Fewer row tiles than SMs: split the column tiles of a row tile over several CTAs (each quantises the row tile again,
   // from L2) so that the whole GPU writes output.
   int csplit = num_sms / p.tiles_m;
   csplit = csplit < 1 ? 1 : (csplit > p.tiles_n ? p.tiles_n : csplit);
-  P4V_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kernel<<<p.tiles_m * csplit, kThreads, smem, st>>>(p);
+  P4V_CUDA_OK(cudaFuncSetAttribute(forward_tc_kernel<Par>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  forward_tc_kernel<Par><<<p.tiles_m * csplit, kThreads, smem, st>>>(p);
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   return 0;
 }
-
-}  // namespace
-
-int p4v_launch_forward_tc(const FwdParams& p, int num_sms, cudaStream_t st) { return launch(forward_tc_kernel<FwdParams>, p, 0u, num_sms, st); }
-
-int p4v_launch_mlp_fc1_tc(const FwdMlpParams& p, int num_sms, cudaStream_t st) {
-  P4V_REQUIRE(!p.twin && (p.planes2 == 1 || p.planes2 == 2) && p.epi_bytes == p4v_mlp_epi_bytes(p.planes2, p.n_chunks2) &&
-              (reinterpret_cast<uintptr_t>(p.X2) & 15) == 0, "mlp forward: bad epilogue plan");
-  return launch(forward_tc_kernel<FwdMlpParams>, p, p.epi_bytes, num_sms, st);
-}
-
-// The LayerNorm variants: the row stats take P4V_NORM_STATS_BYTES after the (MLP epilogue's) shared memory
-int p4v_launch_forward_norm_tc(const FwdNormParams& p, int num_sms, cudaStream_t st) {
-  P4V_REQUIRE(!p.twin && p.ld % 4 == 0 && p.ln.gamma && p.ln.beta, "forward: bad LayerNorm plan");
-  return launch(forward_tc_kernel<FwdNormParams>, p, P4V_NORM_STATS_BYTES, num_sms, st);
-}
-
-int p4v_launch_mlp_fc1_norm_tc(const FwdMlpNormParams& p, int num_sms, cudaStream_t st) {
-  P4V_REQUIRE(!p.twin && (p.planes2 == 1 || p.planes2 == 2) && p.epi_bytes == p4v_mlp_epi_bytes(p.planes2, p.n_chunks2) &&
-              (reinterpret_cast<uintptr_t>(p.X2) & 15) == 0 && p.ld % 4 == 0 && p.ln.gamma && p.ln.beta,
-              "mlp forward: bad epilogue or LayerNorm plan");
-  return launch(forward_tc_kernel<FwdMlpNormParams>, p, p.epi_bytes + P4V_NORM_STATS_BYTES, num_sms, st);
-}
+template int p4v_launch_forward_tc(const FwdParams&, int, cudaStream_t);
+template int p4v_launch_forward_tc(const FwdMlpParams&, int, cudaStream_t);
+template int p4v_launch_forward_tc(const FwdNormParams&, int, cudaStream_t);
+template int p4v_launch_forward_tc(const FwdMlpNormParams&, int, cudaStream_t);
 
 // Diagnostic: y = p4v_gelu(x) elementwise (the GELU of mlp_fc1_kernel's epilogue)
 extern "C" int p4v_gelu_probe(const float* x, float* y, long long n, void* stream) {

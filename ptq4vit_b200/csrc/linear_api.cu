@@ -740,6 +740,19 @@ int build_frozen(const p4v_linear_desc* d, FrozenPlan& f, bool for_pack) {
   return 0;
 }
 
+// The ring stages the fused kernel gets for a call of the layer f1 -- as fc1 of a fused MLP whose fc2 is f2, with a
+// LayerNorm folded into its activation quantiser (norm) -- or 0 when the call does not take the fused kernel.  f1 must
+// be on it itself; an MLP needs fc1's outputs to be fc2's inputs and a plain fc1, a LayerNorm a plain layer with K % 4 == 0.
+// The epilogue and the row stats take their share of shared memory, which can only lower the count.
+int fused_stages(const FrozenPlan& f1, const FrozenPlan* f2, bool norm) {
+  const LinPlan& p1 = f1.p;
+  if (f1.stages < 2 || (f2 && (p1.O != f2->p.K || p1.twin)) || (norm && (p1.twin || p1.K % 4 != 0))) return 0;
+  // a plane of fc2's activation image has the K layout of its weight image; a post-GELU fc2 has two
+  const unsigned epi = f2 ? p4v_mlp_epi_bytes(f2->p.twin ? 2 : 1, f2->p.Wcur.kb / 16) : 0u;
+  return frozen_ring_stages(f1.X.tile_bytes() + p4v_fwd_extra_bytes(epi, norm), (size_t)f1.stage_kb * P4V_TILE,
+                            p1.Wcur.kb / 16);
+}
+
 }  // namespace
 
 extern "C" int p4v_linear_pack_bytes(const p4v_linear_desc* d, size_t* bytes) {
@@ -771,7 +784,7 @@ extern "C" int p4v_linear_frozen_path(const p4v_linear_desc* d, int* path) {
   FrozenPlan f; int rc = build_frozen(d, f, true);
   if (rc) return rc;
   P4V_REQUIRE(path != nullptr, "null output");
-  *path = f.stages >= 2 ? 1 : 0;
+  *path = fused_stages(f, nullptr, false) ? 1 : 0;
   return 0;
 }
 
@@ -779,7 +792,7 @@ extern "C" int p4v_linear_frozen_workspace_bytes(const p4v_linear_desc* d, size_
   FrozenPlan f; int rc = build_frozen(d, f, false);
   if (rc) return rc;
   P4V_REQUIRE(bytes != nullptr, "null output");
-  *bytes = f.stages >= 2 ? 0 : f.X.bytes();
+  *bytes = fused_stages(f, nullptr, false) ? 0 : f.X.bytes();
   return 0;
 }
 
@@ -800,6 +813,17 @@ void fill_fwd(const FrozenPlan& f, const float* x, const float* bias, void* pack
   q.stage_bytes = (unsigned)f.stage_kb * P4V_TILE; q.n_stages = (unsigned)f.stages; q.n_chunks = (unsigned)p.Wcur.kb / 16;
 }
 
+// fc2's part of a fused MLP's parameters: the epilogue writes fc2's activation image into the workspace
+void fill_mlp(const FrozenPlan& f2, void* pack2, void* workspace, FwdMlpParams& q) {
+  const LinPlan& p2 = f2.p;
+  q.X2 = f2.X.ptr(workspace); q.X2_tile_bytes = f2.X.tile_bytes(); q.X2_plane_bytes = (unsigned)p2.Wcur.tile_bytes();
+  q.segs2 = p2.segsX.dev(pack2); q.nseg2 = (int)p2.segs.size();
+  q.n_chunks2 = p2.Wcur.kb / 16; q.planes2 = p2.twin ? 2 : 1;
+  q.dX2 = at<float>(pack2, f2.o_dX); q.crb_acts2 = p2.crb_acts;
+  q.d_neg2 = p2.d_neg; q.lo2 = p2.twin ? 0.f : (float)-p2.a_qmax; q.hi2 = (float)(p2.a_qmax - 1); q.neg_lo2 = (float)-p2.a_qmax;
+  q.epi_bytes = p4v_mlp_epi_bytes(q.planes2, q.n_chunks2);
+}
+
 // The second half of the streamed path: the sweep forward of the layer's int8 activation image in the workspace
 int streamed_sweep(const FrozenPlan& f, void* packed, void* workspace, const float* bias, float* out, cudaStream_t st) {
   const LinPlan& p = f.p;
@@ -809,6 +833,58 @@ int streamed_sweep(const FrozenPlan& f, void* packed, void* workspace, const flo
   sp.out = out; sp.n_cand = 1; sp.order = 0;
   sp.R_cand = nullptr; sp.C_cand = nullptr;
   return run_sweep(p, p.fwd, sp, st);
+}
+
+// The arguments of a folded LayerNorm
+int check_norm(const char* what, const float* x, const float* gamma, const float* beta, float eps) {
+  P4V_REQUIRE(x && gamma && beta, "%s: null pointer", what);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(gamma) & 15) == 0 &&
+              (reinterpret_cast<uintptr_t>(beta) & 15) == 0, "%s: x, gamma and beta must be 16-byte aligned", what);
+  P4V_REQUIRE(eps >= 0.f && eps <= 3.4028234663852886e38f, "%s: eps must be finite and non-negative (got %g)", what, (double)eps);
+  return 0;
+}
+
+// A call of the fused kernel on the frozen layer f1: validates every argument of the entry point fn (in its order, with
+// its name in the messages), fills the kernel's parameters and launches it.  Par selects the variant: with a LayerNorm
+// (ln) folded into the activation quantiser, and as fc1 of a fused MLP whose epilogue writes the image of its fc2 (f2)
+// into the workspace, which fc2's sweep forward then reads.  The arguments of fc2, the packed sizes and the workspace
+// are read by the MLP only.
+template <class Par>
+int fused_forward(const char* fn, const FrozenPlan& f1, const float* x, const FwdNorm& ln, const float* bias1,
+                  const void* pack1, size_t pack1_bytes, const FrozenPlan* f2, const float* bias2, const void* pack2,
+                  size_t pack2_bytes, void* workspace, size_t workspace_bytes, float* out, cudaStream_t st) {
+  constexpr bool mlp = kIsMlp<Par>, norm = kIsNorm<Par>;
+  if constexpr (norm) {
+    if (int rc = check_norm(fn, x, ln.gamma, ln.beta, ln.eps)) return rc;
+  }
+  if constexpr (mlp)
+    P4V_REQUIRE(f1.p.d.rows == f2->p.d.rows, "%s: fc1 and fc2 must have the same rows (%d != %d)", fn, f1.p.d.rows,
+                f2->p.d.rows);
+  P4V_REQUIRE(x && pack1 && (!mlp || (pack2 && workspace)) && out, "%s: null pointer", fn);
+  P4V_REQUIRE((!f1.p.d.has_bias || bias1) && (!mlp || !f2->p.d.has_bias || bias2), "%s: has_bias set but bias is null", fn);
+  const int stages = fused_stages(f1, f2, norm);
+  P4V_REQUIRE(stages, "%s: %s", fn, mlp ? (norm ? "these layers do not fuse with the LayerNorm (p4v_mlp_norm_ok)"
+                                                : "these layers do not fuse (p4v_mlp_fused_ok)")
+                                        : "the LayerNorm does not fold into this layer (p4v_linear_norm_ok)");
+  if constexpr (mlp) {
+    P4V_REQUIRE(pack1_bytes >= f1.bytes && pack2_bytes >= f2->bytes, "%s: packed buffer too small "
+                "(fc1 %zu < %zu or fc2 %zu < %zu)", fn, pack1_bytes, f1.bytes, pack2_bytes, f2->bytes);
+    P4V_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0 &&
+                (reinterpret_cast<uintptr_t>(workspace) & 15) == 0,
+                "%s: %sworkspace must be 16-byte and out 8-byte aligned", fn, norm ? "" : "x and ");   // check_norm took x
+    P4V_REQUIRE(workspace_bytes >= f2->X.bytes(), "%s: workspace too small (%zu < %zu)", fn, workspace_bytes, f2->X.bytes());
+  }
+  // the plan's accessors take the buffers they index; nothing writes them
+  void* p1 = const_cast<void*>(pack1);
+  void* p2 = const_cast<void*>(pack2);
+  Par q{};
+  fill_fwd(f1, x, bias1, p1, mlp ? nullptr : out, q);
+  q.n_stages = (unsigned)stages;
+  if constexpr (norm) q.ln = ln;
+  if constexpr (mlp) fill_mlp(*f2, p2, workspace, q);
+  const int rc = p4v_launch_forward_tc(q, p4v_num_sms(), st);
+  if (rc || !mlp) return rc;
+  return streamed_sweep(*f2, p2, workspace, bias2, out, st);
 }
 
 }  // namespace
@@ -822,11 +898,9 @@ extern "C" int p4v_linear_frozen_forward(const p4v_linear_desc* d, const float* 
   P4V_REQUIRE(x && packed && out, "linear_frozen_forward: null pointer");
   P4V_REQUIRE(!d->has_bias || bias, "linear_frozen_forward: has_bias set but bias is null");
   cudaStream_t st = (cudaStream_t)stream;
-  if (f.stages >= 2) {
-    FwdParams q{};
-    fill_fwd(f, x, bias, packed, out, q);
-    return p4v_launch_forward_tc(q, p4v_num_sms(), st);
-  }
+  if (fused_stages(f, nullptr, false))
+    return fused_forward<FwdParams>("linear_frozen_forward", f, x, FwdNorm{}, bias, packed, 0, nullptr, nullptr, nullptr, 0,
+                                    nullptr, 0, out, st);
   P4V_REQUIRE(workspace && workspace_bytes >= f.X.bytes(), "linear_frozen_forward: workspace too small (%zu < %zu)",
               workspace ? workspace_bytes : (size_t)0, f.X.bytes());
   QuantImageArgs qa{};
@@ -840,117 +914,55 @@ extern "C" int p4v_linear_frozen_forward(const p4v_linear_desc* d, const float* 
 // ---- fused frozen MLP: fc1 + GELU + fc2's activation quantiser in one kernel, then fc2's sweep forward -----------
 namespace {
 
-struct MlpPlan {
-  FrozenPlan f1, f2;
-  int stages;         // ring stages of fc1's kernel with the epilogue; 0: the MLP does not fuse
-  int stages_norm;    // the same with a LayerNorm folded into fc1 (norm_ring_stages); 0: the LayerNorm does not fold
-  int planes2, chunks2;
-};
-
-// for_rule: the rows of the descriptors are ignored (p4v_mlp_fused_ok)
-int build_mlp(const p4v_linear_desc* d1, const p4v_linear_desc* d2, MlpPlan& m, bool for_rule) {
+// for_rule: the rows of the descriptors are ignored (p4v_mlp_fused_ok, p4v_mlp_norm_ok)
+int build_mlp(const p4v_linear_desc* d1, const p4v_linear_desc* d2, FrozenPlan& f1, FrozenPlan& f2, bool for_rule) {
   P4V_REQUIRE(d1 && d2, "mlp: null desc");
-  int rc;
-  if ((rc = build_frozen(d1, m.f1, for_rule)) || (rc = build_frozen(d2, m.f2, for_rule))) return rc;
-  const LinPlan &p1 = m.f1.p, &p2 = m.f2.p;
-  m.planes2 = p2.twin ? 2 : 1;
-  m.chunks2 = p2.Wcur.kb / 16;      // a plane of fc2's activation image has the K layout of its weight image
-  m.stages = m.stages_norm = 0;
-  if (p1.O == p2.K && !p1.twin && m.f1.stages >= 2) {
-    m.stages = mlp_ring_stages(m.f1.X.tile_bytes(), (size_t)m.f1.stage_kb * P4V_TILE, p1.Wcur.kb / 16, m.planes2, m.chunks2);
-    if (m.stages >= 2 && p1.K % 4 == 0)
-      m.stages_norm = mlp_ring_stages(m.f1.X.tile_bytes() + P4V_NORM_STATS_BYTES, (size_t)m.f1.stage_kb * P4V_TILE,
-                                      p1.Wcur.kb / 16, m.planes2, m.chunks2);
-  }
-  return 0;
+  if (int rc = build_frozen(d1, f1, for_rule)) return rc;
+  return build_frozen(d2, f2, for_rule);
 }
 
 }  // namespace
 
 extern "C" int p4v_mlp_fused_ok(const p4v_linear_desc* fc1, const p4v_linear_desc* fc2, int* ok) {
-  MlpPlan m; int rc = build_mlp(fc1, fc2, m, true);
+  FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, true);
   if (rc) return rc;
   P4V_REQUIRE(ok != nullptr, "null output");
-  *ok = m.stages >= 2 ? 1 : 0;
+  *ok = fused_stages(f1, &f2, false) ? 1 : 0;
   return 0;
 }
 
 extern "C" int p4v_mlp_frozen_workspace_bytes(const p4v_linear_desc* fc1, const p4v_linear_desc* fc2, size_t* bytes) {
-  MlpPlan m; int rc = build_mlp(fc1, fc2, m, false);
+  FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
   P4V_REQUIRE(fc1->rows == fc2->rows, "mlp: fc1 and fc2 must have the same rows (%d != %d)", fc1->rows, fc2->rows);
   P4V_REQUIRE(bytes != nullptr, "null output");
-  *bytes = m.f2.X.bytes();
+  *bytes = f2.X.bytes();
   return 0;
 }
 
 extern "C" int p4v_mlp_frozen_forward(const p4v_linear_desc* fc1, const float* x, const float* bias1, const void* pack1,
                                       size_t pack1_bytes, const p4v_linear_desc* fc2, const float* bias2, const void* pack2,
                                       size_t pack2_bytes, void* workspace, size_t workspace_bytes, float* out, void* stream) {
-  MlpPlan m; int rc = build_mlp(fc1, fc2, m, false);
+  FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
-  P4V_REQUIRE(fc1->rows == fc2->rows, "mlp_frozen_forward: fc1 and fc2 must have the same rows (%d != %d)", fc1->rows, fc2->rows);
-  P4V_REQUIRE(x && pack1 && pack2 && workspace && out, "mlp_frozen_forward: null pointer");
-  P4V_REQUIRE((!fc1->has_bias || bias1) && (!fc2->has_bias || bias2), "mlp_frozen_forward: has_bias set but bias is null");
-  P4V_REQUIRE(m.stages >= 2, "mlp_frozen_forward: these layers do not fuse (p4v_mlp_fused_ok)");
-  P4V_REQUIRE(pack1_bytes >= m.f1.bytes && pack2_bytes >= m.f2.bytes, "mlp_frozen_forward: packed buffer too small "
-              "(fc1 %zu < %zu or fc2 %zu < %zu)", pack1_bytes, m.f1.bytes, pack2_bytes, m.f2.bytes);
-  P4V_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0 &&
-              (reinterpret_cast<uintptr_t>(workspace) & 15) == 0,
-              "mlp_frozen_forward: x and workspace must be 16-byte and out 8-byte aligned");
-  P4V_REQUIRE(workspace_bytes >= m.f2.X.bytes(), "mlp_frozen_forward: workspace too small (%zu < %zu)", workspace_bytes,
-              m.f2.X.bytes());
-  cudaStream_t st = (cudaStream_t)stream;
-  void* p1 = const_cast<void*>(pack1);
-  void* p2 = const_cast<void*>(pack2);
-  const LinPlan& l2 = m.f2.p;
-  FwdMlpParams q{};
-  fill_fwd(m.f1, x, bias1, p1, nullptr, q);
-  q.n_stages = (unsigned)m.stages;
-  q.X2 = m.f2.X.ptr(workspace); q.X2_tile_bytes = m.f2.X.tile_bytes(); q.X2_plane_bytes = (unsigned)l2.Wcur.tile_bytes();
-  q.segs2 = l2.segsX.dev(p2); q.nseg2 = (int)l2.segs.size();
-  q.n_chunks2 = m.chunks2; q.planes2 = m.planes2;
-  q.dX2 = at<float>(p2, m.f2.o_dX); q.crb_acts2 = l2.crb_acts;
-  q.d_neg2 = l2.d_neg; q.lo2 = l2.twin ? 0.f : (float)-l2.a_qmax; q.hi2 = (float)(l2.a_qmax - 1); q.neg_lo2 = (float)-l2.a_qmax;
-  q.epi_bytes = p4v_mlp_epi_bytes(m.planes2, m.chunks2);
-  if ((rc = p4v_launch_mlp_fc1_tc(q, p4v_num_sms(), st))) return rc;
-  return streamed_sweep(m.f2, p2, workspace, bias2, out, st);
+  return fused_forward<FwdMlpParams>("mlp_frozen_forward", f1, x, FwdNorm{}, bias1, pack1, pack1_bytes, &f2, bias2, pack2,
+                                     pack2_bytes, workspace, workspace_bytes, out, (cudaStream_t)stream);
 }
 
 // ---- LayerNorm folded into the activation quantiser of the fused kernel (forward_tc.cu, DESIGN §4.10) -------------
-namespace {
-
-// Ring stages of the fused kernel with the LayerNorm prologue; 0: the LayerNorm does not fold into this layer
-int norm_stages(const FrozenPlan& f) {
-  const LinPlan& p = f.p;
-  if (f.stages < 2 || p.twin || p.K % 4 != 0) return 0;
-  return norm_ring_stages(f.X.tile_bytes(), (size_t)f.stage_kb * P4V_TILE, p.Wcur.kb / 16);
-}
-
-// The arguments of the LayerNorm shared by both entry points
-int check_norm(const char* what, const float* x, const float* gamma, const float* beta, float eps) {
-  P4V_REQUIRE(x && gamma && beta, "%s: null pointer", what);
-  P4V_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(gamma) & 15) == 0 &&
-              (reinterpret_cast<uintptr_t>(beta) & 15) == 0, "%s: x, gamma and beta must be 16-byte aligned", what);
-  P4V_REQUIRE(eps >= 0.f && eps <= 3.4028234663852886e38f, "%s: eps must be finite and non-negative (got %g)", what, (double)eps);
-  return 0;
-}
-
-}  // namespace
-
 extern "C" int p4v_linear_norm_ok(const p4v_linear_desc* d, int* ok) {
   FrozenPlan f; int rc = build_frozen(d, f, true);
   if (rc) return rc;
   P4V_REQUIRE(ok != nullptr, "null output");
-  *ok = norm_stages(f) >= 2 ? 1 : 0;
+  *ok = fused_stages(f, nullptr, true) ? 1 : 0;
   return 0;
 }
 
 extern "C" int p4v_mlp_norm_ok(const p4v_linear_desc* fc1, const p4v_linear_desc* fc2, int* ok) {
-  MlpPlan m; int rc = build_mlp(fc1, fc2, m, true);
+  FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, true);
   if (rc) return rc;
   P4V_REQUIRE(ok != nullptr, "null output");
-  *ok = m.stages_norm >= 2 ? 1 : 0;
+  *ok = fused_stages(f1, &f2, true) ? 1 : 0;
   return 0;
 }
 
@@ -958,50 +970,17 @@ extern "C" int p4v_linear_frozen_forward_norm(const p4v_linear_desc* d, const fl
                                               float eps, const float* bias, const void* packed_in, float* out, void* stream) {
   FrozenPlan f; int rc = build_frozen(d, f, false);
   if (rc) return rc;
-  if ((rc = check_norm("linear_frozen_forward_norm", x, gamma, beta, eps))) return rc;
-  P4V_REQUIRE(packed_in && out, "linear_frozen_forward_norm: null pointer");
-  P4V_REQUIRE(!d->has_bias || bias, "linear_frozen_forward_norm: has_bias set but bias is null");
-  const int stages = norm_stages(f);
-  P4V_REQUIRE(stages >= 2, "linear_frozen_forward_norm: the LayerNorm does not fold into this layer (p4v_linear_norm_ok)");
-  FwdNormParams q{};
-  fill_fwd(f, x, bias, const_cast<void*>(packed_in), out, q);
-  q.n_stages = (unsigned)stages;
-  q.ln = FwdNorm{gamma, beta, eps};
-  return p4v_launch_forward_norm_tc(q, p4v_num_sms(), (cudaStream_t)stream);
+  return fused_forward<FwdNormParams>("linear_frozen_forward_norm", f, x, FwdNorm{gamma, beta, eps}, bias, packed_in, 0,
+                                      nullptr, nullptr, nullptr, 0, nullptr, 0, out, (cudaStream_t)stream);
 }
 
 extern "C" int p4v_mlp_frozen_forward_norm(const p4v_linear_desc* fc1, const float* x, const float* gamma, const float* beta,
                                            float eps, const float* bias1, const void* pack1, size_t pack1_bytes,
                                            const p4v_linear_desc* fc2, const float* bias2, const void* pack2, size_t pack2_bytes,
                                            void* workspace, size_t workspace_bytes, float* out, void* stream) {
-  MlpPlan m; int rc = build_mlp(fc1, fc2, m, false);
+  FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
-  if ((rc = check_norm("mlp_frozen_forward_norm", x, gamma, beta, eps))) return rc;
-  P4V_REQUIRE(fc1->rows == fc2->rows, "mlp_frozen_forward_norm: fc1 and fc2 must have the same rows (%d != %d)", fc1->rows,
-              fc2->rows);
-  P4V_REQUIRE(pack1 && pack2 && workspace && out, "mlp_frozen_forward_norm: null pointer");
-  P4V_REQUIRE((!fc1->has_bias || bias1) && (!fc2->has_bias || bias2), "mlp_frozen_forward_norm: has_bias set but bias is null");
-  P4V_REQUIRE(m.stages_norm >= 2, "mlp_frozen_forward_norm: these layers do not fuse with the LayerNorm (p4v_mlp_norm_ok)");
-  P4V_REQUIRE(pack1_bytes >= m.f1.bytes && pack2_bytes >= m.f2.bytes, "mlp_frozen_forward_norm: packed buffer too small "
-              "(fc1 %zu < %zu or fc2 %zu < %zu)", pack1_bytes, m.f1.bytes, pack2_bytes, m.f2.bytes);
-  P4V_REQUIRE((reinterpret_cast<uintptr_t>(out) & 7) == 0 && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0,
-              "mlp_frozen_forward_norm: workspace must be 16-byte and out 8-byte aligned");
-  P4V_REQUIRE(workspace_bytes >= m.f2.X.bytes(), "mlp_frozen_forward_norm: workspace too small (%zu < %zu)", workspace_bytes,
-              m.f2.X.bytes());
-  cudaStream_t st = (cudaStream_t)stream;
-  void* p1 = const_cast<void*>(pack1);
-  void* p2 = const_cast<void*>(pack2);
-  const LinPlan& l2 = m.f2.p;
-  FwdMlpNormParams q{};
-  fill_fwd(m.f1, x, bias1, p1, nullptr, q);
-  q.n_stages = (unsigned)m.stages_norm;
-  q.X2 = m.f2.X.ptr(workspace); q.X2_tile_bytes = m.f2.X.tile_bytes(); q.X2_plane_bytes = (unsigned)l2.Wcur.tile_bytes();
-  q.segs2 = l2.segsX.dev(p2); q.nseg2 = (int)l2.segs.size();
-  q.n_chunks2 = m.chunks2; q.planes2 = m.planes2;
-  q.dX2 = at<float>(p2, m.f2.o_dX); q.crb_acts2 = l2.crb_acts;
-  q.d_neg2 = l2.d_neg; q.lo2 = l2.twin ? 0.f : (float)-l2.a_qmax; q.hi2 = (float)(l2.a_qmax - 1); q.neg_lo2 = (float)-l2.a_qmax;
-  q.epi_bytes = p4v_mlp_epi_bytes(m.planes2, m.chunks2);
-  q.ln = FwdNorm{gamma, beta, eps};
-  if ((rc = p4v_launch_mlp_fc1_norm_tc(q, p4v_num_sms(), st))) return rc;
-  return streamed_sweep(m.f2, p2, workspace, bias2, out, st);
+  return fused_forward<FwdMlpNormParams>("mlp_frozen_forward_norm", f1, x, FwdNorm{gamma, beta, eps}, bias1, pack1,
+                                         pack1_bytes, &f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out,
+                                         (cudaStream_t)stream);
 }

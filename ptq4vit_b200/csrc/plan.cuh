@@ -97,27 +97,14 @@ inline void fill_images(SweepParams& sp, void* ws, const Image& Rcur, const Imag
 }
 
 // Forward of a frozen Linear layer: weight-ring stages of stage_bytes that fit in shared memory beside the resident
-// quantised activation tile of a_bytes (all segments; both parts of a post-GELU layer).  At least two, and a plane whose
-// 16-byte chunks fit the kernel's chunk table: the fused kernel (forward_tc.cu).  0: the layer streams an int8 activation
-// image through the sweep kernel instead.
+// quantised activation tile and whatever else the kernel keeps there, a_bytes in all (the tile of all segments, both
+// parts of a post-GELU layer, plus p4v_fwd_extra_bytes of an MLP epilogue or a LayerNorm).  At least two, and a plane
+// whose 16-byte chunks fit the kernel's chunk table: the fused kernel (forward_tc.cu).  0: the call does not take it
+// (a plain layer streams an int8 activation image through the sweep kernel instead).
 inline int frozen_ring_stages(size_t a_bytes, size_t stage_bytes, size_t plane_chunks) {
   const size_t usable = P4V_FWD_SMEM - P4V_FWD_CTL_BYTES;
   if (plane_chunks > P4V_FWD_MAX_CHUNKS || a_bytes + 2 * stage_bytes > usable) return 0;
   return (int)std::min<size_t>((usable - a_bytes) / stage_bytes, P4V_FWD_MAX_STAGES);
-}
-
-// fc1 of a fused frozen MLP (forward_tc.cu with FwdMlpParams): the ring stages of fc1's fused kernel when the
-// GELU-and-quantise epilogue (the staged tile in fc2's planes, fc2's column steps and chunk table) takes its share of
-// shared memory.  0: the MLP does not fuse.
-inline int mlp_ring_stages(size_t a_bytes1, size_t stage_bytes1, size_t plane_chunks1, int planes2, int plane_chunks2) {
-  return frozen_ring_stages(a_bytes1 + p4v_mlp_epi_bytes(planes2, plane_chunks2), stage_bytes1, plane_chunks1);
-}
-
-// A frozen layer with a LayerNorm folded into its fused kernel (forward_tc.cu with FwdNormParams): the ring stages when
-// the per-row mean and rstd of the tile take their share of shared memory.  0: the LayerNorm does not fold.  The plain
-// layer's own stage count (frozen_ring_stages) is not changed by this.
-inline int norm_ring_stages(size_t a_bytes, size_t stage_bytes, size_t plane_chunks) {
-  return frozen_ring_stages(a_bytes + P4V_NORM_STATS_BYTES, stage_bytes, plane_chunks);
 }
 
 // A commit copies the chosen candidate's slabs from the planes of cand into cur

@@ -133,15 +133,15 @@ class MinMaxQuantLinear(nn.Linear):
         dev = self._device()
         d = self._desc(1, 1)
         lib = _lib.lib()
-        nbytes, path = ctypes.c_size_t(), ctypes.c_int()
+        nbytes = ctypes.c_size_t()
         _lib.check(lib.p4v_linear_pack_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "p4v_linear_pack_bytes")
-        _lib.check(lib.p4v_linear_frozen_path(ctypes.byref(d), ctypes.byref(path)), "p4v_linear_frozen_path")
+        fused = _rule("p4v_linear_frozen_path", self)
         packed = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
         w = (self.weight if weight is None else weight).detach().to(dev).reshape(self.out_features, self.in_features).contiguous().float()
         wi, ai = self._w_flat(), self._a_flat()
         _lib.check(lib.p4v_linear_pack(ctypes.byref(d), _lib.ptr(w), _lib.ptr(wi), _lib.ptr(ai), _lib.ptr(packed), nbytes.value,
                                        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "p4v_linear_pack")
-        self._packed, self._frozen_fused, self._frozen_ws = packed, bool(path.value), None
+        self._packed, self._frozen_fused, self._frozen_ws = packed, fused, None
         # the step sizes that were packed: the objects (kept, so their identity cannot be reused) and their versions
         self._frozen_intervals = (self.w_interval, self.a_interval, self._interval_versions())
         return self
@@ -160,30 +160,9 @@ class MinMaxQuantLinear(nn.Linear):
             raise RuntimeError(f"{self}: the step sizes changed after freeze(); call unfreeze() (and freeze() again) "
                                "before running the layer")
 
-    def _frozen_forward(self, x):
-        self._check_frozen_intervals()
-        dev = self._packed.device
-        x2 = _flat2d(x.to(dev))
-        d = self._desc(x2.shape[0], 1)
-        lib = _lib.lib()
-        ws, ws_bytes = None, 0
-        if not self._frozen_fused:           # streamed path: one int8 activation image, kept between calls
-            nbytes = ctypes.c_size_t()
-            _lib.check(lib.p4v_linear_frozen_workspace_bytes(ctypes.byref(d), ctypes.byref(nbytes)), "frozen_workspace")
-            if self._frozen_ws is None or self._frozen_ws.numel() < nbytes.value:
-                self._frozen_ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
-            ws, ws_bytes = self._frozen_ws, self._frozen_ws.numel()
-        out = torch.empty(x2.shape[0], self.out_features, dtype=torch.float32, device=dev)
-        b = None if self.bias is None else self.bias.detach().contiguous().float()
-        _lib.check(lib.p4v_linear_frozen_forward(ctypes.byref(d), _lib.ptr(x2), _lib.ptr(b), _lib.ptr(self._packed), _lib.ptr(ws),
-                                                 ws_bytes, _lib.ptr(out),
-                                                 ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-                   "p4v_linear_frozen_forward")
-        return out.reshape(*x.shape[:-1], self.out_features)
-
     def _quant_forward_native(self, x):
         if self._packed is not None:
-            return self._frozen_forward(x)
+            return _frozen_call(self, x)
         dev = self._device()
         x2 = _flat2d(x.to(dev))
         d = self._desc(x2.shape[0], 1)
@@ -246,6 +225,56 @@ class MinMaxQuantLinear(nn.Linear):
         return out
 
 
+def _rule(fn, *layers):
+    """A shape rule of the library (an int written through its last argument) over the layers' descriptors; the rules
+    ignore the rows."""
+    ok = ctypes.c_int()
+    _lib.check(getattr(_lib.lib(), fn)(*[ctypes.byref(m._desc(1, 1)) for m in layers], ctypes.byref(ok)), fn)
+    return bool(ok.value)
+
+
+def _streamed_image(lin, dev, fn, *descs):
+    """lin's int8 activation image of a streamed call (fn: the library call that sizes it), kept in lin between calls
+    and allocated again when it is too small or on another device."""
+    nbytes = ctypes.c_size_t()
+    _lib.check(getattr(_lib.lib(), fn)(*[ctypes.byref(d) for d in descs], ctypes.byref(nbytes)), fn)
+    if lin._frozen_ws is None or lin._frozen_ws.numel() < nbytes.value or lin._frozen_ws.device != dev:
+        lin._frozen_ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    return lin._frozen_ws
+
+
+def _frozen_call(lin, x, norm=None, fc2=None):
+    """One library call of frozen layers: lin(x), on lin's fused kernel or its streamed path; with `norm`, lin(norm(x))
+    with the LayerNorm folded into lin's fused kernel; with `fc2`, fc2(gelu(lin(...))) as the fused MLP.  The callers'
+    rules say which applies; the library validates the call.  Only the output (and a missing streamed image) is
+    allocated."""
+    for m in (lin, fc2):
+        if m is not None:
+            m._check_frozen_intervals()
+    dev = lin._packed.device
+    x2 = _flat2d(x.to(dev))
+    b1, b2 = (None if m is None or m.bias is None else m.bias.detach().contiguous().float() for m in (lin, fc2))
+    d1 = lin._desc(x2.shape[0], 1)
+    args = [ctypes.byref(d1), _lib.ptr(x2)]
+    if norm is not None:
+        args += [_lib.ptr(norm.weight), _lib.ptr(norm.bias), float(norm.eps)]
+    args += [_lib.ptr(b1), _lib.ptr(lin._packed)]
+    ws = None
+    if fc2 is not None:                  # fc1's epilogue writes fc2's image, kept in fc2
+        d2 = fc2._desc(x2.shape[0], 1)
+        args += [lin._packed.numel(), ctypes.byref(d2), _lib.ptr(b2), _lib.ptr(fc2._packed), fc2._packed.numel()]
+        ws = _streamed_image(fc2, dev, "p4v_mlp_frozen_workspace_bytes", d1, d2)
+    elif norm is None and not lin._frozen_fused:
+        ws = _streamed_image(lin, dev, "p4v_linear_frozen_workspace_bytes", d1)
+    if fc2 is not None or norm is None:
+        args += [_lib.ptr(ws), 0 if ws is None else ws.numel()]
+    last = lin if fc2 is None else fc2
+    out = torch.empty(x2.shape[0], last.out_features, dtype=torch.float32, device=dev)
+    fn = ("p4v_linear_frozen_forward" if fc2 is None else "p4v_mlp_frozen_forward") + ("" if norm is None else "_norm")
+    _lib.check(getattr(_lib.lib(), fn)(*args, _lib.ptr(out), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), fn)
+    return out.reshape(*x.shape[:-1], last.out_features)
+
+
 def frozen_mlp_applies(fc1, fc2, act, x):
     """Whether one call of an MLP block fc2(act(fc1(x))) can run as the fused frozen MLP (frozen_mlp): fc1 and fc2 frozen
     Linear layers in quant_forward mode, act exactly torch's exact GELU (nn.GELU(approximate='none')), under grad mode
@@ -258,10 +287,7 @@ def frozen_mlp_applies(fc1, fc2, act, x):
         return False
     if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in (fc1, fc2) for p in m.parameters())):
         return False
-    ok = ctypes.c_int()
-    _lib.check(_lib.lib().p4v_mlp_fused_ok(ctypes.byref(fc1._desc(1, 1)), ctypes.byref(fc2._desc(1, 1)), ctypes.byref(ok)),
-               "p4v_mlp_fused_ok")
-    return bool(ok.value)
+    return _rule("p4v_mlp_fused_ok", fc1, fc2)
 
 
 def frozen_mlp(fc1, fc2, x, norm=None):
@@ -270,35 +296,7 @@ def frozen_mlp(fc1, fc2, x, norm=None):
     bits are those of the unfused sequence.  fc2's image is kept between calls in fc2's frozen workspace.
     With `norm` (an nn.LayerNorm for which frozen_norm_applies(norm, fc1, x) and frozen_mlp_norm_ok(fc1, fc2) hold):
     fc2(gelu(fc1(norm(x)))), the LayerNorm folded into fc1's activation quantiser, still two launches."""
-    fc1._check_frozen_intervals()
-    fc2._check_frozen_intervals()
-    dev = fc1._packed.device
-    x2 = _flat2d(x.to(dev))
-    d1, d2 = fc1._desc(x2.shape[0], 1), fc2._desc(x2.shape[0], 1)
-    lib = _lib.lib()
-    nbytes = ctypes.c_size_t()
-    _lib.check(lib.p4v_mlp_frozen_workspace_bytes(ctypes.byref(d1), ctypes.byref(d2), ctypes.byref(nbytes)),
-               "p4v_mlp_frozen_workspace_bytes")
-    if fc2._frozen_ws is None or fc2._frozen_ws.numel() < nbytes.value or fc2._frozen_ws.device != dev:
-        fc2._frozen_ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
-    ws = fc2._frozen_ws
-    out = torch.empty(x2.shape[0], fc2.out_features, dtype=torch.float32, device=dev)
-    b1 = None if fc1.bias is None else fc1.bias.detach().contiguous().float()
-    b2 = None if fc2.bias is None else fc2.bias.detach().contiguous().float()
-    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    if norm is not None:
-        _lib.check(lib.p4v_mlp_frozen_forward_norm(ctypes.byref(d1), _lib.ptr(x2), _lib.ptr(norm.weight), _lib.ptr(norm.bias),
-                                                   float(norm.eps), _lib.ptr(b1), _lib.ptr(fc1._packed), fc1._packed.numel(),
-                                                   ctypes.byref(d2), _lib.ptr(b2), _lib.ptr(fc2._packed), fc2._packed.numel(),
-                                                   _lib.ptr(ws), ws.numel(), _lib.ptr(out), stream),
-                   "p4v_mlp_frozen_forward_norm")
-        return out.reshape(*x.shape[:-1], fc2.out_features)
-    _lib.check(lib.p4v_mlp_frozen_forward(ctypes.byref(d1), _lib.ptr(x2), _lib.ptr(b1), _lib.ptr(fc1._packed), fc1._packed.numel(),
-                                          ctypes.byref(d2), _lib.ptr(b2), _lib.ptr(fc2._packed), fc2._packed.numel(),
-                                          _lib.ptr(ws), ws.numel(), _lib.ptr(out),
-                                          ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-               "p4v_mlp_frozen_forward")
-    return out.reshape(*x.shape[:-1], fc2.out_features)
+    return _frozen_call(fc1, x, norm=norm, fc2=fc2)
 
 
 def frozen_norm_applies(norm, lin, x):
@@ -323,35 +321,20 @@ def frozen_norm_applies(norm, lin, x):
         return False
     if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in (norm, lin) for p in m.parameters())):
         return False
-    ok = ctypes.c_int()
-    _lib.check(_lib.lib().p4v_linear_norm_ok(ctypes.byref(lin._desc(1, 1)), ctypes.byref(ok)), "p4v_linear_norm_ok")
-    return bool(ok.value)
+    return _rule("p4v_linear_norm_ok", lin)
 
 
 def frozen_mlp_norm_ok(fc1, fc2):
     """The shape rule of frozen_mlp(..., norm=): fc1 and fc2 fuse (p4v_mlp_fused_ok) and the plan with the LayerNorm's
     row statistics still fits (p4v_mlp_norm_ok)."""
-    ok = ctypes.c_int()
-    _lib.check(_lib.lib().p4v_mlp_norm_ok(ctypes.byref(fc1._desc(1, 1)), ctypes.byref(fc2._desc(1, 1)), ctypes.byref(ok)),
-               "p4v_mlp_norm_ok")
-    return bool(ok.value)
+    return _rule("p4v_mlp_norm_ok", fc1, fc2)
 
 
 def frozen_norm_linear(norm, lin, x):
     """lin(norm(x)) in one launch, for a call where frozen_norm_applies(norm, lin, x) holds: torch's exact LayerNorm
     computed in the activation quantiser of lin's fused kernel (csrc/forward_tc.cu), bit-identical to the unfolded call;
     the normalised activations never reach HBM.  Only the output is allocated."""
-    lin._check_frozen_intervals()
-    dev = lin._packed.device
-    x2 = _flat2d(x.to(dev))
-    d = lin._desc(x2.shape[0], 1)
-    out = torch.empty(x2.shape[0], lin.out_features, dtype=torch.float32, device=dev)
-    b = None if lin.bias is None else lin.bias.detach().contiguous().float()
-    _lib.check(_lib.lib().p4v_linear_frozen_forward_norm(ctypes.byref(d), _lib.ptr(x2), _lib.ptr(norm.weight), _lib.ptr(norm.bias),
-                                                         float(norm.eps), _lib.ptr(b), _lib.ptr(lin._packed), _lib.ptr(out),
-                                                         ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-               "p4v_linear_frozen_forward_norm")
-    return out.reshape(*x.shape[:-1], lin.out_features)
+    return _frozen_call(lin, x, norm=norm)
 
 
 class PTQSLQuantLinear(MinMaxQuantLinear):
