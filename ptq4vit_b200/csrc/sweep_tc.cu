@@ -196,12 +196,19 @@ __device__ __forceinline__ float reduce8_over_warp(float (&p)[8], int lane) {
 //   kModePair:   two candidate groups over the same candidate column slabs with different resident row parts (twin
 //                activations of post-GELU weight steps, hi/lo parts of split-of-softmax B steps): one ring stage per
 //                job pair, both parts multiplied per 64-column half, r stays in registers, g is parked.
-enum { kModeMulti = 0, kModeSingle = 1, kModePair = 2 };
+//   kModeX8:     the int8 activation step of a bf16 layer (linear_api.cu build_plan, x8): a multi-segment step whose job
+//                list is fixed, so the consumer runs it without reading the jobs.  Every candidate group is one K32 slab,
+//                four per ring stage in group order, the column operand is the resident weight tile and there are no
+//                fixed groups.  Same arithmetic as kModeMulti, group by group; launches report it as kModeMulti.
+enum { kModeMulti = 0, kModeSingle = 1, kModePair = 2, kModeX8 = 3 };
 
 template <bool kInt8, int kMode>
 __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_constant__ SweepParams P) {
   using AccT = typename std::conditional<kInt8, uint32_t, float>::type;
-  constexpr bool kPair = kMode == kModePair, kMulti = kMode == kModeMulti;
+  constexpr bool kX8 = kMode == kModeX8;                       // parks the residual and reads g like kModeMulti
+  constexpr bool kPair = kMode == kModePair, kMulti = kMode == kModeMulti || kX8;
+  static_assert(kInt8 || !kX8, "the x8 loop runs int8 operands only");
+  constexpr int kPhaseKind = (kInt8 ? 3 : 0) + (kX8 ? kModeMulti : kMode);   // phase-clock row: x8 counts as int8 multi
   extern __shared__ uint8_t smem_raw[];
   // 128-byte aligned base, formed by pointer arithmetic on the __shared__ array (not an integer round trip) so that
   // the compiler keeps the shared state space: LDS / STS instead of generic loads and stores with 64-bit addresses.
@@ -287,7 +294,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
         r_cand += P.R_cand_stride; c_cand += P.C_cand_stride;
       }
     }
-    pc.flush((kInt8 ? 3 : 0) + kMode, kPhProducer, lane == 0);
+    pc.flush(kPhaseKind, kPhProducer, lane == 0);
     return;
   }
 
@@ -307,6 +314,8 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
   const uint32_t sR16 = sR >> 4, sC16 = sC >> 4;
   const uint32_t ringR16 = ((ringR & 0x3FFFF) >> 4) + wg * 64, ringC16 = (ringC & 0x3FFFF) >> 4;   // +64 rows x 16 B
   const uint32_t resC16 = (resC & 0x3FFFF) >> 4;
+  // x8: candidate group 0's slab in the resident weight tile, in 16-byte units (the groups' slabs follow it 32 bytes of K apart)
+  const uint32_t x8_b16 = kX8 ? resC16 + (S.jobs[0].c_off >> 4) : 0;
   const uint32_t full0 = smem_u32(&S.full[0]);
   float2* const park = reinterpret_cast<float2*>(red + kRedBytes / 4) + et;  // values (v, v+1) at park[(v / 2) * 256]
   uint32_t stage = 0, phase = 0, rbuf = 0, rphase = 0, cphase = 0;
@@ -439,6 +448,17 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
         return make_float2(ok0 ? x0 * gs : 0.f, ok1 ? x1 * gs : 0.f);
       }
     };
+    // The same loads in the x8 loop, with the predicates folded into one column limit per fragment row (0 when the row
+    // is outside the problem): value (v, v + 1) loads when its column offset dc (+ 1), a compile-time constant, is below it.
+    // gs is a power of two in [2^-100, 2^100] (p4v_make_gscale), so a value that is not loaded gives 0 * gs = +0, the
+    // 0.f that gpair selects.
+    const int glim0 = g0ok ? P.N - gc : 0, glim8 = g8ok ? P.N - gc : 0;
+    auto gpair_x8 = [&](const int v) -> float2 {
+      const int h = (v >> 1) & 1, dc = 8 * (v >> 2);
+      const int lim = h ? glim8 : glim0;
+      const float* const gp = (h ? g8p : g0p) + dc;
+      return make_float2(ldg_if(gp, dc < lim) * gs, ldg_if(gp + 1, dc + 1 < lim) * gs);
+    };
 
     // -- candidates --
     uint32_t res16 = 0;
@@ -456,7 +476,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
     }
     for (int c = f.c0; c < f.c1; ++c) {
       if constexpr (kMulti) {
-        if (c > f.c0) {
+        if (kX8 || c > f.c0) {   // x8: on the first candidate too, so that r is dead after each final epilogue
 #pragma unroll
           for (int v = 0; v < 64; v += 2) { const float2 x = park[(v >> 1) * kConsumers]; r[v] = x.x; r[v + 1] = x.y; }
         }
@@ -507,6 +527,91 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
           warp_arrive(&S.empty[stage], lane);
           if (++stage == nst) { stage = 0; phase ^= 1; }
         }
+      } else if constexpr (kX8) {
+        // Group gi is the K32 slab gi of the candidate's activation rows (ring stage gi / 4, 32 * (gi % 4) bytes in) against
+        // the same slab of the resident weight tile, accumulated from zero.  Per group: one wgmma, its wait, the
+        // epilogue; nothing is read from the job list and no count is dispatched at run time.  The operations per value
+        // are those of the run() path: r = fmaf(-s, acc, r) per candidate group in group order, then
+        // (g * fmaf(-s, acc, r))^2 for the last group.
+        // A group's 8 scales candA[c][k] * candB[gi][k] come from four 16-byte shared loads.  (With the candidate's candA
+        // row held in registers across its groups instead, ptxas -v reports 28 bytes of spill stores.)
+        const int G = P.n_cand_groups;
+        auto scales = [&](const int gi, float (&s)[P4V_TILE_CG]) {
+          const float4* const a4 = reinterpret_cast<const float4*>(S.candA[c]);
+          const float4* const b4 = reinterpret_cast<const float4*>(S.candB[gi]);
+          const float4 a0 = a4[0], a1 = a4[1], b0 = b4[0], b1 = b4[1];
+          const float a[P4V_TILE_CG] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+          const float b[P4V_TILE_CG] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+          const bool noA = (P.cand_noA_mask >> gi) & 1ull;
+#pragma unroll
+          for (int k = 0; k < P4V_TILE_CG; ++k) s[k] = noA ? b[k] : a[k] * b[k];
+        };
+        auto mma = [&](const uint32_t a16, const uint32_t b16) {
+          wg_fence();
+          wgmma_k32(acc, dconst | (uint64_t)a16, dconst | (uint64_t)b16, 0u);
+          wg_commit();
+          pc.skip();
+          wg_wait0();
+          pc.lap(kPhWgWait);
+        };
+        auto cand_epilogue = [&](const int gi) {
+          pc.skip();
+          float s[P4V_TILE_CG];
+          scales(gi, s);
+#pragma unroll
+          for (int k = 0; k < P4V_TILE_CG; ++k)
+#pragma unroll
+            for (int e = 0; e < 8; ++e) r[8 * k + e] = fmaf(-s[k], acc_to_float(acc[8 * k + e]), r[8 * k + e]);
+          pc.lap(kPhCand);
+        };
+        auto wait_stage = [&]() -> uint32_t {                // the stage's row slab, in 16-byte units
+          pc.skip();
+          mbar_wait_addr(full0 + stage * 8, phase);
+          pc.lap(kPhFull);
+          return ringR16 + stage * sR16;
+        };
+        int gi = 0;
+        for (; gi + 4 < G; gi += 4) {                          // stages of four candidate groups
+          const uint32_t a16 = wait_stage(), b16 = x8_b16 + 256 * gi;   // +32 bytes of K = 256 16-byte units
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            mma(a16 + 256 * q, b16 + 256 * q);
+            if (q == 3) warp_arrive(&S.empty[stage], lane);
+            cand_epilogue(gi + q);
+          }
+          if (++stage == nst) { stage = 0; phase ^= 1; }
+        }
+        {                                                     // the last stage: groups gi .. G - 1, the last one final
+          const uint32_t a16 = wait_stage(), b16 = x8_b16 + 256 * gi;
+          const int nq = G - gi;
+          for (int q = 0; q + 1 < nq; ++q) {
+            mma(a16 + 256 * q, b16 + 256 * q);
+            cand_epilogue(gi + q);
+          }
+          mma(a16 + 256 * (nq - 1), b16 + 256 * (nq - 1));
+          warp_arrive(&S.empty[stage], lane);
+          if (++stage == nst) { stage = 0; phase ^= 1; }
+          // the scales one column group at a time, from shared memory: the 64 g loads in flight leave no room for 8 more
+          // live registers
+          pc.skip();
+          const bool noA = (P.cand_noA_mask >> (G - 1)) & 1ull;
+#pragma unroll
+          for (int k = 0; k < P4V_TILE_CG; ++k) {
+            const float s = noA ? S.candB[G - 1][k] : S.candA[c][k] * S.candB[G - 1][k];
+            float q[2] = {0.f, 0.f};
+#pragma unroll
+            for (int e = 0; e < 8; e += 2) {
+              const int v = 8 * k + e;
+              const float2 gv = gpair_x8(v);
+              const float w0 = gv.x * fmaf(-s, acc_to_float(acc[v]), r[v]);
+              const float w1 = gv.y * fmaf(-s, acc_to_float(acc[v + 1]), r[v + 1]);
+              q[(e >> 1) & 1] = fmaf(w0, w0, q[(e >> 1) & 1]);
+              q[(e >> 1) & 1] = fmaf(w1, w1, q[(e >> 1) & 1]);
+            }
+            ph[k][0] = q[0]; ph[k][1] = q[1];
+          }
+          pc.lap(kPhFinal);
+        }
       } else {
         int gi = 0;
         for (int jj = 0; jj < P.n_cand_jobs; ++jj) {
@@ -547,7 +652,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
           });
         }
       }
-      if (!kPair && P.row_keys) {
+      if (!kPair && !kX8 && P.row_keys) {
         // one score per ROW (channel-wise conv search): [tile][candidate][column half][128 rows].  The quad of lanes
         // holding rows (frow, frow + 8) reduces its four (row, column half) totals and scatters them over its lanes.
         float k4[4] = {0.f, 0.f, 0.f, 0.f};
@@ -585,7 +690,7 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
     }
     if (cresB) warp_arrive(&S.cres_empty, lane);
   }
-  pc.flush((kInt8 ? 3 : 0) + kMode, kPhConsumer, lane == 0 && (cw & 3) == 0);
+  pc.flush(kPhaseKind, kPhConsumer, lane == 0 && (cw & 3) == 0);
 }
 
 }  // namespace
@@ -665,6 +770,21 @@ int p4v_launch_sweep_tc(const SweepParams& p_in, const P4VJob* host_jobs, int nu
     }
   }
   const int mode = single ? kModeSingle : pair ? kModePair : kModeMulti;
+  // The int8 activation step of a bf16 layer (build_plan's x8 jobs) runs the multi-segment arithmetic on its own loop
+  // (kModeX8): no fixed groups, and candidate job j is groups 4j .. 4j + 3 (fewer in the last job), K32 slabs that
+  // follow each other in both operand images, the activation slab from the candidate plane, the weight slab from the
+  // tile's resident image, each slab its own accumulator.  Its launches are reported as multi-segment.
+  bool x8 = false;
+  if (mode == kModeMulti && p.is_int8 && !p.row_keys && p.n_fixed_jobs == 0 && p.n_cand_groups >= 2 &&
+      p.n_cand_jobs == (p.n_cand_groups + 3) / 4) {
+    const P4VJob* cj = host_jobs;
+    const uint32_t flags = P4V_JOB_FIRST | P4V_JOB_LAST | P4V_JOB_RCAND | P4V_JOB_CRES;
+    x8 = true;
+    for (int j = 0; j < p.n_cand_jobs; ++j)
+      x8 = x8 && cj[j].flags == flags && cj[j].kb == 32 &&
+           p4v_job_nsub(cj[j]) == (unsigned)std::min(4, p.n_cand_groups - 4 * j) && cj[j].group == 4 * j &&
+           cj[j].r_off == cj[0].r_off + j * 4 * 32 * P4V_TILE && cj[j].c_off == cj[0].c_off + j * 4 * 32 * P4V_TILE;
+  }
   if (decision) *decision = P4VLaunchDecision{mode, nst, (int)p.resident_bufs, p.resident_bytes, p.cres_bytes, grid};
 #define P4V_LAUNCH(I8, MODE)                                                                           \
   do {                                                                                                 \
@@ -677,8 +797,9 @@ int p4v_launch_sweep_tc(const SweepParams& p_in, const P4VJob* host_jobs, int nu
     else if (mode == kModePair) P4V_LAUNCH(I8, kModePair);                                             \
     else P4V_LAUNCH(I8, kModeMulti);                                                                   \
   } while (0)
-  if (p.is_int8) P4V_LAUNCH_MODE(true);
-  else           P4V_LAUNCH_MODE(false);
+  if (x8)             P4V_LAUNCH(true, kModeX8);
+  else if (p.is_int8) P4V_LAUNCH_MODE(true);
+  else                P4V_LAUNCH_MODE(false);
 #undef P4V_LAUNCH_MODE
 #undef P4V_LAUNCH
   P4V_CUDA_OK(cudaGetLastError());
