@@ -269,6 +269,37 @@ P4V_API int p4v_mlp_frozen_forward_norm(const p4v_linear_desc* fc1, const float*
 P4V_API int p4v_layer_norm_probe(const float* x, const float* gamma, const float* beta, float eps, long long M, int N, float* y,
                                  void* stream);
 
+/* A block's residual add folded into the store of the frozen Linear that produces it: out[dst(r)] = fl(y[r] + residual[dst(r)])
+ * for every output row r of the layer, y the output p4v_linear_frozen_forward computes.  Bit-identical to that call
+ * followed by torch's elementwise FP32 add, signed zeros included; the Linear's FP32 output never reaches HBM.
+ * dst is the identity, or for Swin's attention projection the window layout below: window row
+ *   r = ((b * nH + wh) * nW + ww) * window^2 + i * window + j      (nH = height / window, nW = width / window)
+ * is image row b * height * width + ((wh * window + i + shift) mod height) * width + (ww * window + j + shift) mod width,
+ * which replaces  x + roll(window_reverse(proj(...)), (shift, shift))  of a (shifted) Swin block.  A layout needs
+ * window > 0, height % window == 0, width % window == 0, 0 <= shift < window and images * height * width == rows, and the
+ * layer on its fused path (p4v_linear_frozen_path 1): the streamed path takes the identity only.
+ * p4v_linear_frozen_forward_res replaces  residual + p4v_linear_frozen_forward(...)  (either path); layout null = identity.
+ * p4v_mlp_frozen_forward_res / p4v_mlp_frozen_forward_norm_res replace  residual + p4v_mlp_frozen_forward(...)  /
+ * residual + p4v_mlp_frozen_forward_norm(...): the add is fc2's, always on its streamed sweep, in identity rows.
+ * residual is [rows][out_features] FP32, contiguous, 8-byte aligned and must not overlap out.  Every argument of the
+ * underlying call and the residual and layout are validated before anything is launched; the launches are those of the
+ * underlying call, nothing is allocated or copied, so each can be captured in a CUDA graph. */
+typedef struct p4v_window_layout {
+  int32_t images, height, width, window, shift;
+} p4v_window_layout;
+P4V_API int p4v_linear_frozen_forward_res(const p4v_linear_desc* d, const float* x, const float* bias, const void* packed,
+                                          void* workspace, size_t workspace_bytes, const float* residual,
+                                          const p4v_window_layout* layout, float* out, void* stream);
+P4V_API int p4v_mlp_frozen_forward_res(const p4v_linear_desc* fc1, const float* x, const float* bias1, const void* pack1,
+                                       size_t pack1_bytes, const p4v_linear_desc* fc2, const float* bias2, const void* pack2,
+                                       size_t pack2_bytes, void* workspace, size_t workspace_bytes, const float* residual,
+                                       float* out, void* stream);
+P4V_API int p4v_mlp_frozen_forward_norm_res(const p4v_linear_desc* fc1, const float* x, const float* gamma, const float* beta,
+                                            float eps, const float* bias1, const void* pack1, size_t pack1_bytes,
+                                            const p4v_linear_desc* fc2, const float* bias2, const void* pack2,
+                                            size_t pack2_bytes, void* workspace, size_t workspace_bytes,
+                                            const float* residual, float* out, void* stream);
+
 /* The patch-embedding convolution: ChannelwiseBatchingQuantConv2d with a_bit >= 32 (quant_layers/conv.py:444-614, wired
  * by configs/PTQ4ViT.py:52-54): one weight step size per output channel, activations left in FP32.  The caller passes
  * the im2col matrix of the FP32 input (torch.nn.functional.unfold, [images, positions, K], K = in_channels*kh*kw in the

@@ -45,6 +45,10 @@ class ConvFrozenDesc(C.Structure):
                 ("layerwise", C.c_int32), ("has_bias", C.c_int32)]
 
 
+class WindowLayout(C.Structure):
+    _fields_ = [("images", C.c_int32), ("height", C.c_int32), ("width", C.c_int32), ("window", C.c_int32), ("shift", C.c_int32)]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     "p4v_linear_workspace_bytes": [C.POINTER(LinearDesc), C.POINTER(C.c_size_t)],
@@ -86,6 +90,11 @@ _SIGNATURES = {
     "p4v_mlp_frozen_forward_norm": [C.POINTER(LinearDesc), _P, _P, _P, C.c_float, _P, _P, C.c_size_t, C.POINTER(LinearDesc), _P,
                                     _P, C.c_size_t, _P, C.c_size_t, _P, _P],
     "p4v_layer_norm_probe": [_P, _P, _P, C.c_float, C.c_longlong, C.c_int, _P, _P],
+    "p4v_linear_frozen_forward_res": [C.POINTER(LinearDesc), _P, _P, _P, _P, C.c_size_t, _P, C.POINTER(WindowLayout), _P, _P],
+    "p4v_mlp_frozen_forward_res": [C.POINTER(LinearDesc), _P, _P, _P, C.c_size_t, C.POINTER(LinearDesc), _P, _P, C.c_size_t, _P,
+                                   C.c_size_t, _P, _P, _P],
+    "p4v_mlp_frozen_forward_norm_res": [C.POINTER(LinearDesc), _P, _P, _P, C.c_float, _P, _P, C.c_size_t, C.POINTER(LinearDesc),
+                                        _P, _P, C.c_size_t, _P, C.c_size_t, _P, _P, _P],
     "p4v_conv_workspace_bytes": [C.POINTER(ConvDesc), C.POINTER(C.c_size_t)],
     "p4v_conv_calibrate": [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P],
     "p4v_conv_frozen_ok": [C.POINTER(ConvFrozenDesc), C.POINTER(C.c_int)],

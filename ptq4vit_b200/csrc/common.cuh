@@ -77,6 +77,7 @@ struct SweepParams {
   int row_keys;             // single-segment steps: one score per ROW, partial = [tile][candidate][column half][128 rows]
   // shared-memory plan, filled by the launcher
   unsigned int stage_r_bytes, stage_c_bytes, n_stages, resident_bytes, resident_bufs, cres_bytes;
+  const float* res = nullptr;   // with out (not out_residual): out = fl(forward + res), res [M][N] like out (kModeFwdRes)
 };
 
 static inline __host__ __device__ int p4v_cdiv(int a, int b) { return (a + b - 1) / b; }

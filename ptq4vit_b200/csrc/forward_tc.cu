@@ -21,6 +21,8 @@
 // With FwdNormParams / FwdMlpNormParams a LayerNorm is folded into step 1: the CTA first computes each row's mean and
 // rstd with torch's exact reduction (forward.cuh, p4v_ln_row_stats) and the quantise loop normalises every value before
 // quantising it (DESIGN §4.10).
+// With FwdResParams a block's residual add is folded into the FP32 store: each value goes to its destination row (the
+// identity, or Swin's window reverse and reverse shift, p4v_window_row) as fl(value + shortcut) (DESIGN §4.11).
 // 288 threads leave 224 registers per thread without setmaxnreg; the bounded mbarrier wait is inline, and the k32 steps of
 // a stage are one straight-line batch selected by a warp-uniform count (ptxas C7520, see sm90.cuh).
 #include "../../include/ptq4vit_b200.h"
@@ -160,7 +162,8 @@ __device__ __forceinline__ float* ln_stats(const Par& P, uint8_t* smem) {
 }
 
 // Par = FwdParams: the frozen Linear forward, FP32 output.  Par = FwdMlpParams: fc1 of a frozen MLP, GELU-and-quantise
-// epilogue into fc2's image.  FwdNormParams / FwdMlpNormParams: the same with a LayerNorm prologue.
+// epilogue into fc2's image.  FwdNormParams / FwdMlpNormParams: the same with a LayerNorm prologue.  FwdResParams: the
+// plain forward whose store adds the shortcut.
 template <class Par>
 __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_constant__ Par P) {
   constexpr bool kMlp = kIsMlp<Par>;
@@ -342,6 +345,29 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
       asm volatile("bar.sync 1, %0;" ::"n"(kConsumers));   // staged tile complete
       // the next column tile's first barrier orders these reads of the staging before it is written again
       mlp_store_tile(P, mlp_epi(P, smem), tm, tn, et);
+    } else if constexpr (kIsRes<Par>) {
+      // the residual add: out[dst] = fl(-r + res[dst]) (torch's FP32 add of the stored value and the shortcut), the
+      // shortcut read at the destination rows as the pairs the plain store writes
+      const bool pairs = (P.N & 1) == 0;
+      const int d0 = gm < P.M ? p4v_window_row(P.rs.win, gm) : 0, d8 = gm + 8 < P.M ? p4v_window_row(P.rs.win, gm + 8) : 0;
+#pragma unroll
+      for (int v = 0; v < 64; v += 2) {
+        const int row = gm + 8 * ((v >> 1) & 1), col = gc + 8 * (v >> 2);
+        if (row < P.M) {
+          const size_t off = (size_t)((v >> 1) & 1 ? d8 : d0) * P.N + col;
+          float* o = P.out + off;
+          const float* s = P.rs.res + off;
+          if (pairs) {
+            if (col < P.N) {
+              const float2 sv = __ldg(reinterpret_cast<const float2*>(s));
+              *reinterpret_cast<float2*>(o) = make_float2(__fadd_rn(-r[v], sv.x), __fadd_rn(-r[v + 1], sv.y));
+            }
+          } else {
+            if (col < P.N) o[0] = __fadd_rn(-r[v], __ldg(s));
+            if (col + 1 < P.N) o[1] = __fadd_rn(-r[v + 1], __ldg(s + 1));
+          }
+        }
+      }
     } else {
       const bool pairs = (P.N & 1) == 0;       // even row stride: the fragment's column pairs are 8-byte aligned
 #pragma unroll
@@ -369,6 +395,12 @@ template <class Par> int p4v_launch_forward_tc(const Par& p, int num_sms, cudaSt
     P4V_REQUIRE(!p.twin && (p.planes2 == 1 || p.planes2 == 2) && p.epi_bytes == p4v_mlp_epi_bytes(p.planes2, p.n_chunks2) &&
                 (reinterpret_cast<uintptr_t>(p.X2) & 15) == 0, "mlp forward: bad epilogue plan");
   if constexpr (kIsNorm<Par>) P4V_REQUIRE(!p.twin && p.ld % 4 == 0 && p.ln.gamma && p.ln.beta, "forward: bad LayerNorm plan");
+  if constexpr (kIsRes<Par>) {
+    const p4v_window_layout& w = p.rs.win;
+    P4V_REQUIRE(p.rs.res && (reinterpret_cast<uintptr_t>(p.rs.res) & 7) == 0, "forward: residual must be 8-byte aligned");
+    P4V_REQUIRE(w.window == 0 || ((long long)w.images * w.height * w.width == p.M && w.height % w.window == 0 &&
+                                  w.width % w.window == 0 && w.shift >= 0 && w.shift < w.window), "forward: bad window layout");
+  }
   const unsigned extra = p4v_fwd_extra_bytes(p);
   P4V_REQUIRE(p.n_jobs >= 1 && p.n_jobs <= P4V_MAX_JOBS && p.n_groups <= P4V_MAX_GROUPS, "forward: too many K segments");
   P4V_REQUIRE(p.n_stages >= 2 && p.n_stages <= P4V_FWD_MAX_STAGES && p.n_chunks <= P4V_FWD_MAX_CHUNKS &&
@@ -391,6 +423,7 @@ template int p4v_launch_forward_tc(const FwdParams&, int, cudaStream_t);
 template int p4v_launch_forward_tc(const FwdMlpParams&, int, cudaStream_t);
 template int p4v_launch_forward_tc(const FwdNormParams&, int, cudaStream_t);
 template int p4v_launch_forward_tc(const FwdMlpNormParams&, int, cudaStream_t);
+template int p4v_launch_forward_tc(const FwdResParams&, int, cudaStream_t);
 
 // Diagnostic: y = p4v_gelu(x) elementwise (the GELU of mlp_fc1_kernel's epilogue)
 extern "C" int p4v_gelu_probe(const float* x, float* y, long long n, void* stream) {

@@ -824,13 +824,15 @@ void fill_mlp(const FrozenPlan& f2, void* pack2, void* workspace, FwdMlpParams& 
   q.epi_bytes = p4v_mlp_epi_bytes(q.planes2, q.n_chunks2);
 }
 
-// The second half of the streamed path: the sweep forward of the layer's int8 activation image in the workspace
-int streamed_sweep(const FrozenPlan& f, void* packed, void* workspace, const float* bias, float* out, cudaStream_t st) {
+// The second half of the streamed path: the sweep forward of the layer's int8 activation image in the workspace; with
+// res, the store adds the residual (sweep_tc.cu, kModeFwdRes)
+int streamed_sweep(const FrozenPlan& f, void* packed, void* workspace, const float* bias, const float* res, float* out,
+                   cudaStream_t st) {
   const LinPlan& p = f.p;
   SweepParams sp; fill_sweep(p, packed, p.fwd, sp, all_rows(p));
   sp.R_cur = f.X.ptr(workspace);
   sp.bias = p.d.has_bias ? bias : nullptr;
-  sp.out = out; sp.n_cand = 1; sp.order = 0;
+  sp.out = out; sp.res = res; sp.n_cand = 1; sp.order = 0;
   sp.R_cand = nullptr; sp.C_cand = nullptr;
   return run_sweep(p, p.fwd, sp, st);
 }
@@ -844,15 +846,41 @@ int check_norm(const char* what, const float* x, const float* gamma, const float
   return 0;
 }
 
+// The arguments of a folded residual add (res non-null) of a call whose output out is [rows][cols]: res 8-byte aligned
+// and apart from out, and the window layout's rule (win.window == 0: identity rows).  Nothing to check without res.
+int check_residual(const char* fn, const float* res, const float* out, int rows, int cols, const p4v_window_layout& win) {
+  if (!res) return 0;
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(res) & 7) == 0, "%s: residual must be 8-byte aligned", fn);
+  const uintptr_t bytes = (uintptr_t)rows * (uintptr_t)cols * 4, a = reinterpret_cast<uintptr_t>(res),
+                  b = reinterpret_cast<uintptr_t>(out);
+  P4V_REQUIRE(a + bytes <= b || b + bytes <= a, "%s: residual overlaps out", fn);
+  if (win.window != 0 || win.images != 0 || win.height != 0 || win.width != 0 || win.shift != 0) {
+    P4V_REQUIRE(win.window > 0 && win.height > 0 && win.width > 0 && win.images > 0,
+                "%s: window layout needs positive images, height, width and window (got %d, %d, %d, %d)", fn, win.images,
+                win.height, win.width, win.window);
+    P4V_REQUIRE(win.height % win.window == 0 && win.width % win.window == 0,
+                "%s: window layout: height %d and width %d must be multiples of the window %d", fn, win.height, win.width,
+                win.window);
+    P4V_REQUIRE(win.shift >= 0 && win.shift < win.window, "%s: window layout: shift %d must lie in [0, window %d)", fn,
+                win.shift, win.window);
+    P4V_REQUIRE((long long)win.images * win.height * win.width == rows,
+                "%s: window layout: images * height * width = %lld, the layer has %d rows", fn,
+                (long long)win.images * win.height * win.width, rows);
+  }
+  return 0;
+}
+
 // A call of the fused kernel on the frozen layer f1: validates every argument of the entry point fn (in its order, with
 // its name in the messages), fills the kernel's parameters and launches it.  Par selects the variant: with a LayerNorm
 // (ln) folded into the activation quantiser, and as fc1 of a fused MLP whose epilogue writes the image of its fc2 (f2)
 // into the workspace, which fc2's sweep forward then reads.  The arguments of fc2, the packed sizes and the workspace
-// are read by the MLP only.
+// are read by the MLP only.  A residual (rs.res non-null) is added by the last launch's store: the plain kernel's
+// (FwdResParams, with rs.win) or fc2's sweep (identity rows).
 template <class Par>
-int fused_forward(const char* fn, const FrozenPlan& f1, const float* x, const FwdNorm& ln, const float* bias1,
-                  const void* pack1, size_t pack1_bytes, const FrozenPlan* f2, const float* bias2, const void* pack2,
-                  size_t pack2_bytes, void* workspace, size_t workspace_bytes, float* out, cudaStream_t st) {
+int fused_forward(const char* fn, const FrozenPlan& f1, const float* x, const FwdNorm& ln, const FwdResidual& rs,
+                  const float* bias1, const void* pack1, size_t pack1_bytes, const FrozenPlan* f2, const float* bias2,
+                  const void* pack2, size_t pack2_bytes, void* workspace, size_t workspace_bytes, float* out,
+                  cudaStream_t st) {
   constexpr bool mlp = kIsMlp<Par>, norm = kIsNorm<Par>;
   if constexpr (norm) {
     if (int rc = check_norm(fn, x, ln.gamma, ln.beta, ln.eps)) return rc;
@@ -874,6 +902,8 @@ int fused_forward(const char* fn, const FrozenPlan& f1, const float* x, const Fw
                 "%s: %sworkspace must be 16-byte and out 8-byte aligned", fn, norm ? "" : "x and ");   // check_norm took x
     P4V_REQUIRE(workspace_bytes >= f2->X.bytes(), "%s: workspace too small (%zu < %zu)", fn, workspace_bytes, f2->X.bytes());
   }
+  P4V_REQUIRE(!mlp || rs.win.window == 0, "%s: fc2 of a fused MLP takes no window layout", fn);
+  if (int rc = check_residual(fn, rs.res, out, f1.p.M, mlp ? f2->p.O : f1.p.O, rs.win)) return rc;
   // the plan's accessors take the buffers they index; nothing writes them
   void* p1 = const_cast<void*>(pack1);
   void* p2 = const_cast<void*>(pack2);
@@ -882,33 +912,46 @@ int fused_forward(const char* fn, const FrozenPlan& f1, const float* x, const Fw
   q.n_stages = (unsigned)stages;
   if constexpr (norm) q.ln = ln;
   if constexpr (mlp) fill_mlp(*f2, p2, workspace, q);
+  if constexpr (kIsRes<Par>) q.rs = rs;
   const int rc = p4v_launch_forward_tc(q, p4v_num_sms(), st);
   if (rc || !mlp) return rc;
-  return streamed_sweep(*f2, p2, workspace, bias2, out, st);
+  return streamed_sweep(*f2, p2, workspace, bias2, rs.res, out, st);
+}
+
+// p4v_linear_frozen_forward (rs.res null) and p4v_linear_frozen_forward_res, on the layer's path
+int frozen_forward(const char* fn, const p4v_linear_desc* d, const float* x, const float* bias, const void* packed_in,
+                   void* workspace, size_t workspace_bytes, const FwdResidual& rs, float* out, cudaStream_t st) {
+  FrozenPlan f; int rc = build_frozen(d, f, false);
+  if (rc) return rc;
+  const LinPlan& p = f.p;
+  void* packed = const_cast<void*>(packed_in);      // the plan's accessors take the buffer they index; nothing writes it
+  P4V_REQUIRE(x && packed && out, "%s: null pointer", fn);
+  P4V_REQUIRE(!d->has_bias || bias, "%s: has_bias set but bias is null", fn);
+  if (fused_stages(f, nullptr, false)) {
+    if (rs.res)
+      return fused_forward<FwdResParams>(fn, f, x, FwdNorm{}, rs, bias, packed, 0, nullptr, nullptr, nullptr, 0, nullptr, 0,
+                                         out, st);
+    return fused_forward<FwdParams>(fn, f, x, FwdNorm{}, rs, bias, packed, 0, nullptr, nullptr, nullptr, 0, nullptr, 0, out,
+                                    st);
+  }
+  P4V_REQUIRE(workspace && workspace_bytes >= f.X.bytes(), "%s: workspace too small (%zu < %zu)", fn,
+              workspace ? workspace_bytes : (size_t)0, f.X.bytes());
+  P4V_REQUIRE(rs.win.window == 0, "%s: a window layout needs the fused path (p4v_linear_frozen_path 1)", fn);
+  if ((rc = check_residual(fn, rs.res, out, p.M, p.O, rs.win))) return rc;
+  QuantImageArgs qa{};
+  f.X.fill(qa, workspace);
+  qa.src = x; qa.ld = p.K; qa.rows = p.M; qa.delta = at<float>(packed, f.o_dX); qa.d_mod = 1;
+  qa.rows_per_block = p.M + P4V_TILE; qa.segs = p.segsX.dev(packed); qa.nseg = (int)p.segsX.host.size();
+  if ((rc = p4v_quant_image(qa, st))) return rc;
+  return streamed_sweep(f, packed, workspace, bias, rs.res, out, st);
 }
 
 }  // namespace
 
 extern "C" int p4v_linear_frozen_forward(const p4v_linear_desc* d, const float* x, const float* bias, const void* packed_in,
                                          void* workspace, size_t workspace_bytes, float* out, void* stream) {
-  FrozenPlan f; int rc = build_frozen(d, f, false);
-  if (rc) return rc;
-  const LinPlan& p = f.p;
-  void* packed = const_cast<void*>(packed_in);      // the plan's accessors take the buffer they index; nothing writes it
-  P4V_REQUIRE(x && packed && out, "linear_frozen_forward: null pointer");
-  P4V_REQUIRE(!d->has_bias || bias, "linear_frozen_forward: has_bias set but bias is null");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (fused_stages(f, nullptr, false))
-    return fused_forward<FwdParams>("linear_frozen_forward", f, x, FwdNorm{}, bias, packed, 0, nullptr, nullptr, nullptr, 0,
-                                    nullptr, 0, out, st);
-  P4V_REQUIRE(workspace && workspace_bytes >= f.X.bytes(), "linear_frozen_forward: workspace too small (%zu < %zu)",
-              workspace ? workspace_bytes : (size_t)0, f.X.bytes());
-  QuantImageArgs qa{};
-  f.X.fill(qa, workspace);
-  qa.src = x; qa.ld = p.K; qa.rows = p.M; qa.delta = at<float>(packed, f.o_dX); qa.d_mod = 1;
-  qa.rows_per_block = p.M + P4V_TILE; qa.segs = p.segsX.dev(packed); qa.nseg = (int)p.segsX.host.size();
-  if ((rc = p4v_quant_image(qa, st))) return rc;
-  return streamed_sweep(f, packed, workspace, bias, out, st);
+  return frozen_forward("linear_frozen_forward", d, x, bias, packed_in, workspace, workspace_bytes, FwdResidual{}, out,
+                        (cudaStream_t)stream);
 }
 
 // ---- fused frozen MLP: fc1 + GELU + fc2's activation quantiser in one kernel, then fc2's sweep forward -----------
@@ -945,8 +988,8 @@ extern "C" int p4v_mlp_frozen_forward(const p4v_linear_desc* fc1, const float* x
                                       size_t pack2_bytes, void* workspace, size_t workspace_bytes, float* out, void* stream) {
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
-  return fused_forward<FwdMlpParams>("mlp_frozen_forward", f1, x, FwdNorm{}, bias1, pack1, pack1_bytes, &f2, bias2, pack2,
-                                     pack2_bytes, workspace, workspace_bytes, out, (cudaStream_t)stream);
+  return fused_forward<FwdMlpParams>("mlp_frozen_forward", f1, x, FwdNorm{}, FwdResidual{}, bias1, pack1, pack1_bytes, &f2,
+                                     bias2, pack2, pack2_bytes, workspace, workspace_bytes, out, (cudaStream_t)stream);
 }
 
 // ---- LayerNorm folded into the activation quantiser of the fused kernel (forward_tc.cu, DESIGN §4.10) -------------
@@ -970,8 +1013,8 @@ extern "C" int p4v_linear_frozen_forward_norm(const p4v_linear_desc* d, const fl
                                               float eps, const float* bias, const void* packed_in, float* out, void* stream) {
   FrozenPlan f; int rc = build_frozen(d, f, false);
   if (rc) return rc;
-  return fused_forward<FwdNormParams>("linear_frozen_forward_norm", f, x, FwdNorm{gamma, beta, eps}, bias, packed_in, 0,
-                                      nullptr, nullptr, nullptr, 0, nullptr, 0, out, (cudaStream_t)stream);
+  return fused_forward<FwdNormParams>("linear_frozen_forward_norm", f, x, FwdNorm{gamma, beta, eps}, FwdResidual{}, bias,
+                                      packed_in, 0, nullptr, nullptr, nullptr, 0, nullptr, 0, out, (cudaStream_t)stream);
 }
 
 extern "C" int p4v_mlp_frozen_forward_norm(const p4v_linear_desc* fc1, const float* x, const float* gamma, const float* beta,
@@ -980,7 +1023,43 @@ extern "C" int p4v_mlp_frozen_forward_norm(const p4v_linear_desc* fc1, const flo
                                            void* workspace, size_t workspace_bytes, float* out, void* stream) {
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
-  return fused_forward<FwdMlpNormParams>("mlp_frozen_forward_norm", f1, x, FwdNorm{gamma, beta, eps}, bias1, pack1,
-                                         pack1_bytes, &f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out,
+  return fused_forward<FwdMlpNormParams>("mlp_frozen_forward_norm", f1, x, FwdNorm{gamma, beta, eps}, FwdResidual{}, bias1,
+                                         pack1, pack1_bytes, &f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out,
                                          (cudaStream_t)stream);
+}
+
+// ---- a block's residual add folded into the store of the frozen Linear that produces it (DESIGN §4.11) -------------
+// Each entry point replaces  residual + <the call without _res>  (torch's FP32 add; Swin's proj also the window reverse
+// and the reverse roll before it, through the layout).  A null residual is an error here, not the call without it.
+extern "C" int p4v_linear_frozen_forward_res(const p4v_linear_desc* d, const float* x, const float* bias, const void* packed,
+                                             void* workspace, size_t workspace_bytes, const float* residual,
+                                             const p4v_window_layout* layout, float* out, void* stream) {
+  P4V_REQUIRE(residual, "linear_frozen_forward_res: null pointer");
+  return frozen_forward("linear_frozen_forward_res", d, x, bias, packed, workspace, workspace_bytes,
+                        FwdResidual{residual, layout ? *layout : p4v_window_layout{}}, out, (cudaStream_t)stream);
+}
+
+extern "C" int p4v_mlp_frozen_forward_res(const p4v_linear_desc* fc1, const float* x, const float* bias1, const void* pack1,
+                                          size_t pack1_bytes, const p4v_linear_desc* fc2, const float* bias2, const void* pack2,
+                                          size_t pack2_bytes, void* workspace, size_t workspace_bytes, const float* residual,
+                                          float* out, void* stream) {
+  FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
+  if (rc) return rc;
+  P4V_REQUIRE(residual, "mlp_frozen_forward_res: null pointer");
+  return fused_forward<FwdMlpParams>("mlp_frozen_forward_res", f1, x, FwdNorm{}, FwdResidual{residual, {}}, bias1, pack1,
+                                     pack1_bytes, &f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out,
+                                     (cudaStream_t)stream);
+}
+
+extern "C" int p4v_mlp_frozen_forward_norm_res(const p4v_linear_desc* fc1, const float* x, const float* gamma, const float* beta,
+                                               float eps, const float* bias1, const void* pack1, size_t pack1_bytes,
+                                               const p4v_linear_desc* fc2, const float* bias2, const void* pack2,
+                                               size_t pack2_bytes, void* workspace, size_t workspace_bytes,
+                                               const float* residual, float* out, void* stream) {
+  FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
+  if (rc) return rc;
+  P4V_REQUIRE(residual, "mlp_frozen_forward_norm_res: null pointer");
+  return fused_forward<FwdMlpNormParams>("mlp_frozen_forward_norm_res", f1, x, FwdNorm{gamma, beta, eps},
+                                         FwdResidual{residual, {}}, bias1, pack1, pack1_bytes, &f2, bias2, pack2, pack2_bytes,
+                                         workspace, workspace_bytes, out, (cudaStream_t)stream);
 }

@@ -200,15 +200,20 @@ __device__ __forceinline__ float reduce8_over_warp(float (&p)[8], int lane) {
 //                list is fixed, so the consumer runs it without reading the jobs.  Every candidate group is one K32 slab,
 //                four per ring stage in group order, the column operand is the resident weight tile and there are no
 //                fixed groups.  Same arithmetic as kModeMulti, group by group; launches report it as kModeMulti.
-enum { kModeMulti = 0, kModeSingle = 1, kModePair = 2, kModeX8 = 3 };
+//   kModeFwdRes: a forward (out, no candidates) whose store adds the residual res: out = fl(-r + res), a block's
+//                residual add folded into the frozen Linear that produces it (DESIGN §4.11).  The searches and the
+//                plain forward never take it; launches report it as kModeMulti.
+enum { kModeMulti = 0, kModeSingle = 1, kModePair = 2, kModeX8 = 3, kModeFwdRes = 4 };
 
 template <bool kInt8, int kMode>
 __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_constant__ SweepParams P) {
   using AccT = typename std::conditional<kInt8, uint32_t, float>::type;
   constexpr bool kX8 = kMode == kModeX8;                       // parks the residual and reads g like kModeMulti
-  constexpr bool kPair = kMode == kModePair, kMulti = kMode == kModeMulti || kX8;
+  constexpr bool kFwdRes = kMode == kModeFwdRes;              // stops after the forward store: the rest is dead code
+  constexpr bool kPair = kMode == kModePair, kMulti = kMode == kModeMulti || kX8 || kFwdRes;
   static_assert(kInt8 || !kX8, "the x8 loop runs int8 operands only");
-  constexpr int kPhaseKind = (kInt8 ? 3 : 0) + (kX8 ? kModeMulti : kMode);   // phase-clock row: x8 counts as int8 multi
+  // phase-clock row: x8 and the residual forward count as multi
+  constexpr int kPhaseKind = (kInt8 ? 3 : 0) + (kX8 || kFwdRes ? kModeMulti : kMode);
   extern __shared__ uint8_t smem_raw[];
   // 128-byte aligned base, formed by pointer arithmetic on the __shared__ array (not an integer round trip) so that
   // the compiler keeps the shared state space: LDS / STS instead of generic loads and stores with 64-bit addresses.
@@ -416,12 +421,33 @@ __global__ void __launch_bounds__(kThreads, 1) sweep_tc_kernel(const __grid_cons
           pc.lap(kPhFixed);
         });
     }
-    if (P.out != nullptr) {
+    if (kFwdRes || P.out != nullptr) {
       if (cresB) warp_arrive(&S.cres_empty, lane);
+      if constexpr (kFwdRes) {
+        // out = fl(-r + res): torch's FP32 add of the stored value and the shortcut, read as the pairs it writes
+        const bool pairs = ((P.ld | P.N | (long long)pbase) & 1) == 0;
 #pragma unroll
-      for (int v = 0; v < 64; ++v) {
-        const int row = gm + 8 * ((v >> 1) & 1), col = gc + 8 * (v >> 2) + (v & 1);
-        if (row < P.M && col < P.N) P.out[pbase + (size_t)row * P.ld + col] = P.out_residual ? r[v] : -r[v];
+        for (int v = 0; v < 64; v += 2) {
+          const int row = gm + 8 * ((v >> 1) & 1), col = gc + 8 * (v >> 2);
+          if (row < P.M) {
+            const size_t off = pbase + (size_t)row * P.ld + col;
+            if (pairs) {
+              if (col < P.N) {
+                const float2 sv = __ldg(reinterpret_cast<const float2*>(P.res + off));
+                *reinterpret_cast<float2*>(P.out + off) = make_float2(__fadd_rn(-r[v], sv.x), __fadd_rn(-r[v + 1], sv.y));
+              }
+            } else {
+              if (col < P.N) P.out[off] = __fadd_rn(-r[v], __ldg(P.res + off));
+              if (col + 1 < P.N) P.out[off + 1] = __fadd_rn(-r[v + 1], __ldg(P.res + off + 1));
+            }
+          }
+        }
+      } else {
+#pragma unroll
+        for (int v = 0; v < 64; ++v) {
+          const int row = gm + 8 * ((v >> 1) & 1), col = gc + 8 * (v >> 2) + (v & 1);
+          if (row < P.M && col < P.N) P.out[pbase + (size_t)row * P.ld + col] = P.out_residual ? r[v] : -r[v];
+        }
       }
       continue;
     }
@@ -719,6 +745,9 @@ int p4v_launch_sweep_tc(const SweepParams& p_in, const P4VJob* host_jobs, int nu
   P4V_REQUIRE(p.n_cand <= P4V_MAX_CAND && p.n_cand >= 1, "sweep: bad candidate count");
   P4V_REQUIRE(p.out != nullptr ? (p.n_cand == 1 && p.n_cand_jobs == 0) : p.n_cand_groups >= 1, "sweep: bad mode");
   P4V_REQUIRE(!p.row_keys || (p.n_cand_groups == 1 && p.out == nullptr), "sweep: per-row scores need a single-segment step");
+  P4V_REQUIRE(!p.res || (p.out && !p.out_residual && p.is_int8 &&
+                         ((reinterpret_cast<uintptr_t>(p.res) | reinterpret_cast<uintptr_t>(p.out)) & 7) == 0),
+              "sweep: a residual needs an int8 forward with 8-byte aligned out and residual");
   const long long tiles = (long long)p.P * p.tiles_m * p.tiles_n;
   const long long units = tiles * p.n_cand;
   int grid = (int)(units < num_sms ? units : num_sms);
@@ -797,7 +826,8 @@ int p4v_launch_sweep_tc(const SweepParams& p_in, const P4VJob* host_jobs, int nu
     else if (mode == kModePair) P4V_LAUNCH(I8, kModePair);                                             \
     else P4V_LAUNCH(I8, kModeMulti);                                                                   \
   } while (0)
-  if (x8)             P4V_LAUNCH(true, kModeX8);
+  if (p.res)          P4V_LAUNCH(true, kModeFwdRes);
+  else if (x8)        P4V_LAUNCH(true, kModeX8);
   else if (p.is_int8) P4V_LAUNCH_MODE(true);
   else                P4V_LAUNCH_MODE(false);
 #undef P4V_LAUNCH_MODE

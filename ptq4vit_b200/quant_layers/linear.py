@@ -243,11 +243,13 @@ def _streamed_image(lin, dev, fn, *descs):
     return lin._frozen_ws
 
 
-def _frozen_call(lin, x, norm=None, fc2=None):
+def _frozen_call(lin, x, norm=None, fc2=None, residual=None, layout=None):
     """One library call of frozen layers: lin(x), on lin's fused kernel or its streamed path; with `norm`, lin(norm(x))
-    with the LayerNorm folded into lin's fused kernel; with `fc2`, fc2(gelu(lin(...))) as the fused MLP.  The callers'
-    rules say which applies; the library validates the call.  Only the output (and a missing streamed image) is
-    allocated."""
+    with the LayerNorm folded into lin's fused kernel; with `fc2`, fc2(gelu(lin(...))) as the fused MLP; with
+    `residual`, residual + that output, the add folded into the last layer's store (with `layout`, an (images, height,
+    width, window, shift) window layout of lin's output rows: Swin's window reverse and reverse shift before the add).
+    The callers' rules say which applies; the library validates the call.  Only the output (and a missing streamed image)
+    is allocated."""
     for m in (lin, fc2):
         if m is not None:
             m._check_frozen_intervals()
@@ -271,7 +273,14 @@ def _frozen_call(lin, x, norm=None, fc2=None):
     last = lin if fc2 is None else fc2
     out = torch.empty(x2.shape[0], last.out_features, dtype=torch.float32, device=dev)
     fn = ("p4v_linear_frozen_forward" if fc2 is None else "p4v_mlp_frozen_forward") + ("" if norm is None else "_norm")
+    if residual is not None:
+        fn += "_res"
+        args.append(_lib.ptr(residual))
+        if fc2 is None:
+            args.append(None if layout is None else ctypes.byref(_lib.WindowLayout(*[int(v) for v in layout])))
     _lib.check(getattr(_lib.lib(), fn)(*args, _lib.ptr(out), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), fn)
+    if residual is not None:
+        return out.view(residual.shape)
     return out.reshape(*x.shape[:-1], last.out_features)
 
 
@@ -290,13 +299,52 @@ def frozen_mlp_applies(fc1, fc2, act, x):
     return _rule("p4v_mlp_fused_ok", fc1, fc2)
 
 
-def frozen_mlp(fc1, fc2, x, norm=None):
+def frozen_mlp(fc1, fc2, x, norm=None, residual=None):
     """fc2(gelu(fc1(x))) of two frozen layers in two launches (csrc/forward_tc.cu: fc1 with a GELU-and-quantise
     epilogue writing fc2's int8 activation image; fc2's sweep forward), for a call where frozen_mlp_applies holds.  The
     bits are those of the unfused sequence.  fc2's image is kept between calls in fc2's frozen workspace.
     With `norm` (an nn.LayerNorm for which frozen_norm_applies(norm, fc1, x) and frozen_mlp_norm_ok(fc1, fc2) hold):
-    fc2(gelu(fc1(norm(x)))), the LayerNorm folded into fc1's activation quantiser, still two launches."""
-    return _frozen_call(fc1, x, norm=norm, fc2=fc2)
+    fc2(gelu(fc1(norm(x)))), the LayerNorm folded into fc1's activation quantiser, still two launches.
+    With `residual` (frozen_residual_applies(fc2, x, residual) holds): residual + that, added in fc2's store."""
+    return _frozen_call(fc1, x, norm=norm, fc2=fc2, residual=residual)
+
+
+def frozen_residual_applies(lin, x, residual, layout=None):
+    """Whether residual + lin(x) -- with `layout` (images, height, width, window, shift), residual + Swin's window reverse
+    and reverse roll of lin(x) -- can run as one folded call (frozen_residual_linear), or as the same add folded into a
+    fused MLP whose fc2 is `lin` (frozen_mlp(..., residual=)): lin a frozen Linear layer in quant_forward mode, residual an
+    FP32 tensor on lin's device, contiguous, 8-byte aligned, with the output's shape (with a layout: its number of rows
+    and lin's out_features per row), under grad mode nothing that requires grad, and a layout only for a layer on its
+    fused path (the streamed path adds in identity rows only).  x is the input of the call: lin's, or fc1's of the MLP."""
+    if not (isinstance(lin, MinMaxQuantLinear) and lin.frozen and lin.mode == "quant_forward"):
+        return False
+    dev = lin._packed.device
+    if not torch.is_tensor(residual) or residual.dtype != torch.float32 or residual.device != dev:
+        return False
+    if not residual.is_contiguous() or residual.data_ptr() % 8 or x.numel() == 0:
+        return False
+    rows = x.numel() // x.shape[-1]
+    if layout is None:
+        if tuple(residual.shape) != (*x.shape[:-1], lin.out_features):
+            return False
+    else:
+        images, height, width, window, shift = (int(v) for v in layout)
+        if not lin._frozen_fused or residual.shape[-1] != lin.out_features or residual.numel() != rows * lin.out_features:
+            return False
+        if not (window > 0 and height % window == 0 and width % window == 0 and 0 <= shift < window and
+                images * height * width == rows):
+            return False
+    if torch.is_grad_enabled() and (x.requires_grad or residual.requires_grad or any(p.requires_grad for p in lin.parameters())):
+        return False
+    return True
+
+
+def frozen_residual_linear(lin, x, residual, layout=None):
+    """residual + lin(x) in the launches of lin(x), for a call where frozen_residual_applies holds: lin's fused kernel or
+    its streamed sweep adds the shortcut as it stores each output value (csrc/forward_tc.cu, csrc/sweep_tc.cu), with
+    `layout` at the row Swin's window reverse and reverse roll send it to; bit-identical to the unfolded sequence and lin's
+    FP32 output never reaches HBM.  Returns a new tensor of residual's shape; only it is allocated."""
+    return _frozen_call(lin, x, residual=residual, layout=layout)
 
 
 def frozen_norm_applies(norm, lin, x):

@@ -44,7 +44,14 @@ norm2 -> mlp.fc1, Swin's norm2 -> fc1, PatchMerging's norm -> reduction, a ViT's
 rows are normalised): torch's exact LayerNorm runs in the Linear's activation quantiser, one launch instead of two and
 no normalised tensor in HBM, bit-identical.  It composes with fuse_attention and fuse_mlp (norm2, fc1, GELU and fc2's
 quantiser in one kernel).  A folded call skips the LayerNorm's forward hooks, so it is opt-in; `unfuse_norm(net)` undoes
-it.  None of the fusions is recorded by save_quantized: apply them again after load_quantized.
+it.
+
+`fuse_residual(net)` folds each block's residual adds into the frozen Linear whose output they add: `x + attn(...)`
+into attn.proj (in a Swin block also the window reverse and the reverse roll before the add, through a window layout of
+proj's output rows) and `x + mlp(...)` into mlp.fc2, fused MLP included.  The Linear's store adds the shortcut, so its
+FP32 output never reaches HBM and the torch add (reverse, roll) kernels are gone, bit-identical.  It composes with the
+other fusions.  A folded call skips proj's and fc2's forward hooks, so it is opt-in; `unfuse_residual(net)` undoes it.
+None of the fusions is recorded by save_quantized: apply them again after load_quantized.
 """
 import torch
 
@@ -171,6 +178,29 @@ def unfuse_norm(net):
     for m in net.modules():
         for flag, _norm, _lin in _norm_sites(m):
             setattr(m, flag, False)
+
+
+def fuse_residual(net):
+    """Mark every `Block` and `SwinBlock` of `net` whose attn.proj and mlp.fc2 are frozen Linear layers: each residual add
+    that qualifies (quant_layers.linear.frozen_residual_applies: an FP32 contiguous shortcut of the output's shape, no
+    gradient wanted, a window layout only on proj's fused path) is done by the store of the Linear that produces it --
+    Swin's window reverse and reverse roll included -- with the bits of the unfolded sequence; any other call runs the
+    modules and torch's ops as before.  A folded call skips the forward hooks of proj and fc2, which is why the fold is
+    opt-in.  It composes with fuse_attention, fuse_mlp and fuse_norm; save_quantized / load_quantized do not record it.
+    Returns the names of the blocks left unfolded."""
+    left = []
+    for name, m in net.named_modules():
+        if isinstance(m, (Block, SwinBlock)):
+            m.fold_residual = all(isinstance(l, MinMaxQuantLinear) and l.frozen for l in (m.attn.proj, m.mlp.fc2))
+            if not m.fold_residual:
+                left.append(name)
+    return left
+
+
+def unfuse_residual(net):
+    for m in net.modules():
+        if isinstance(m, (Block, SwinBlock)):
+            m.fold_residual = False
 
 
 def _to(v, device):

@@ -6,7 +6,7 @@ import torch
 import torch.nn as nn
 
 from ..quant_layers.linear import (frozen_mlp, frozen_mlp_applies, frozen_mlp_norm_ok, frozen_norm_applies,
-                                   frozen_norm_linear)
+                                   frozen_norm_linear, frozen_residual_applies, frozen_residual_linear)
 from ..quant_layers.matmul import frozen_attention, frozen_attention_applies
 
 
@@ -15,6 +15,16 @@ def _norm_linear(norm, lin, x):
     if frozen_norm_applies(norm, lin, x):
         return frozen_norm_linear(norm, lin, x)
     return lin(norm(x))
+
+
+def _linear_res(lin, x, residual):
+    """residual + lin(x) (lin(x) without a residual): the add folded into lin's store when frozen_residual_applies holds,
+    else the module and torch's add as they are."""
+    if residual is None:
+        return lin(x)
+    if frozen_residual_applies(lin, x, residual):
+        return frozen_residual_linear(lin, x, residual)
+    return residual + lin(x)
 
 
 class MatMul(nn.Module):
@@ -36,21 +46,22 @@ class Attention(nn.Module):
     fused_max_tokens = 256   # set by utils.deploy.fuse_attention: sequences up to this length run fused (the long
                              # kernel above 256 tokens)
 
-    def forward(self, x, norm=None):
-        """norm: a LayerNorm to apply to x first (Block with fold_norm1), folded into qkv when it applies."""
+    def forward(self, x, norm=None, residual=None):
+        """norm: a LayerNorm to apply to x first (Block with fold_norm1), folded into qkv when it applies.  residual: a
+        tensor to add to the output (Block with fold_residual), folded into proj when it applies."""
         B, N, C = x.shape
         y = self.qkv(x) if norm is None else _norm_linear(norm, self.qkv, x)
         if self.fused and frozen_attention_applies(self.matmul1, self.matmul2, N, C // self.num_heads, y,
                                                    max_tokens=self.fused_max_tokens):
             qkv5 = y.reshape(B, N, 3, self.num_heads, C // self.num_heads)
-            return self.proj(frozen_attention(self.matmul1, self.matmul2, qkv5, self.scale, scale_on_q=False,
-                                              max_tokens=self.fused_max_tokens))
+            return _linear_res(self.proj, frozen_attention(self.matmul1, self.matmul2, qkv5, self.scale, scale_on_q=False,
+                                                           max_tokens=self.fused_max_tokens), residual)
         qkv = y.reshape(B, N, 3, self.num_heads, C // self.num_heads).permute(2, 0, 3, 1, 4)
         q, k, v = qkv.unbind(0)
         attn = self.matmul1(q, k.transpose(-2, -1)) * self.scale
         attn = attn.softmax(dim=-1)
         x = self.matmul2(attn, v).transpose(1, 2).reshape(B, N, C)
-        return self.proj(x)
+        return _linear_res(self.proj, x, residual)
 
 
 class Mlp(nn.Module):
@@ -62,18 +73,26 @@ class Mlp(nn.Module):
 
     fused = False      # set by utils.deploy.fuse_mlp: run fc1, GELU and fc2 as the fused frozen MLP when it applies
 
-    def forward(self, x, norm=None):
-        """norm: a LayerNorm to apply to x first (Block / SwinBlock with fold_norm2), folded into fc1 when it applies."""
+    def forward(self, x, norm=None, residual=None):
+        """norm: a LayerNorm to apply to x first (Block / SwinBlock with fold_norm2), folded into fc1 when it applies.
+        residual: a tensor to add to the output (Block / SwinBlock with fold_residual), folded into fc2 when it applies."""
         if norm is not None:
             if frozen_norm_applies(norm, self.fc1, x):
                 if not (self.fused and frozen_mlp_applies(self.fc1, self.fc2, self.act, x)):
-                    return self.fc2(self.act(frozen_norm_linear(norm, self.fc1, x)))
+                    return _linear_res(self.fc2, self.act(frozen_norm_linear(norm, self.fc1, x)), residual)
                 if frozen_mlp_norm_ok(self.fc1, self.fc2):
-                    return frozen_mlp(self.fc1, self.fc2, x, norm=norm)
+                    return self._fused(x, norm, residual)
             x = norm(x)
         if self.fused and frozen_mlp_applies(self.fc1, self.fc2, self.act, x):
-            return frozen_mlp(self.fc1, self.fc2, x)
-        return self.fc2(self.act(self.fc1(x)))
+            return self._fused(x, None, residual)
+        return _linear_res(self.fc2, self.act(self.fc1(x)), residual)
+
+    def _fused(self, x, norm, residual):
+        if residual is None:
+            return frozen_mlp(self.fc1, self.fc2, x, norm=norm)
+        if frozen_residual_applies(self.fc2, x, residual):
+            return frozen_mlp(self.fc1, self.fc2, x, norm=norm, residual=residual)
+        return residual + frozen_mlp(self.fc1, self.fc2, x, norm=norm)
 
 
 class Block(nn.Module):
@@ -86,13 +105,21 @@ class Block(nn.Module):
 
     fold_norm1 = False     # set by utils.deploy.fuse_norm: hand norm1 to attn, which folds it into qkv when it applies
     fold_norm2 = False     # set by utils.deploy.fuse_norm: hand norm2 to mlp, which folds it into fc1 when it applies
+    fold_residual = False  # set by utils.deploy.fuse_residual: hand the shortcut to attn and mlp, which fold the adds
+                           # into proj and fc2 when they apply
 
     def forward(self, x):
+        if self.fold_residual:
+            return self._forward_res(x)
         if not (self.fold_norm1 or self.fold_norm2):
             x = x + self.attn(self.norm1(x))
             return x + self.mlp(self.norm2(x))
         x = x + (self.attn(x, norm=self.norm1) if self.fold_norm1 else self.attn(self.norm1(x)))
         return x + (self.mlp(x, norm=self.norm2) if self.fold_norm2 else self.mlp(self.norm2(x)))
+
+    def _forward_res(self, x):
+        x = self.attn(x, norm=self.norm1, residual=x) if self.fold_norm1 else self.attn(self.norm1(x), residual=x)
+        return self.mlp(x, norm=self.norm2, residual=x) if self.fold_norm2 else self.mlp(self.norm2(x), residual=x)
 
 
 class PatchEmbed(nn.Module):
@@ -179,15 +206,18 @@ class WindowAttention(nn.Module):
 
     fused = False      # set by utils.deploy.fuse_attention, as Attention.fused
 
-    def forward(self, x, mask=None):
+    def forward(self, x, mask=None, residual=None, layout=None):
+        """residual, layout: (SwinBlock with fold_residual) return residual + the image of the output windows under
+        layout = (images, height, width, window, shift) -- window reverse, then roll by (shift, shift) -- with the
+        reverse, roll and add folded into proj's store when it applies."""
         B_, N, C = x.shape
         y = self.qkv(x)
         if self.fused:
             bias = self.relative_position_bias_table[self.relative_position_index.view(-1)].view(N, N, -1).permute(2, 0, 1).contiguous()
             if frozen_attention_applies(self.matmul1, self.matmul2, N, C // self.num_heads, y, bias, mask):
                 qkv5 = y.reshape(B_, N, 3, self.num_heads, C // self.num_heads)
-                return self.proj(frozen_attention(self.matmul1, self.matmul2, qkv5, self.scale, scale_on_q=True, bias=bias,
-                                                  mask=mask))
+                return self._proj(frozen_attention(self.matmul1, self.matmul2, qkv5, self.scale, scale_on_q=True, bias=bias,
+                                                   mask=mask), residual, layout)
         qkv = y.reshape(B_, N, 3, self.num_heads, C // self.num_heads).permute(2, 0, 3, 1, 4)
         q, k, v = qkv.unbind(0)
         q = q * self.scale
@@ -200,7 +230,18 @@ class WindowAttention(nn.Module):
             attn = attn.view(-1, self.num_heads, N, N)
         attn = self.softmax(attn)
         x = self.matmul2(attn, v).transpose(1, 2).reshape(B_, N, C)
-        return self.proj(x)
+        return self._proj(x, residual, layout)
+
+    def _proj(self, x, residual, layout):
+        if residual is None:
+            return self.proj(x)
+        if frozen_residual_applies(self.proj, x, residual, layout):
+            return frozen_residual_linear(self.proj, x, residual, layout)
+        _images, H, W, ws, shift = layout
+        h = _window_reverse(self.proj(x), ws, H, W)
+        if shift > 0:
+            h = torch.roll(h, shifts=(shift, shift), dims=(1, 2))
+        return residual + h.view(residual.shape)
 
 
 class SwinBlock(nn.Module):
@@ -225,8 +266,11 @@ class SwinBlock(nn.Module):
         self.register_buffer("attn_mask", mask)
 
     fold_norm2 = False     # set by utils.deploy.fuse_norm, as Block.fold_norm2
+    fold_residual = False  # set by utils.deploy.fuse_residual, as Block.fold_residual (proj's add with the window layout)
 
     def forward(self, x):
+        if self.fold_residual:
+            return self._forward_res(x)
         B, L, C = x.shape
         H = W = self.res
         h = self.norm1(x).view(B, H, W, C)
@@ -240,6 +284,15 @@ class SwinBlock(nn.Module):
         if self.fold_norm2:
             return x + self.mlp(x, norm=self.norm2)
         return x + self.mlp(self.norm2(x))
+
+    def _forward_res(self, x):
+        B, L, C = x.shape
+        H = W = self.res
+        h = self.norm1(x).view(B, H, W, C)
+        if self.shift > 0:
+            h = torch.roll(h, shifts=(-self.shift, -self.shift), dims=(1, 2))
+        x = self.attn(_window_partition(h, self.ws), mask=self.attn_mask, residual=x, layout=(B, H, W, self.ws, self.shift))
+        return self.mlp(x, norm=self.norm2, residual=x) if self.fold_norm2 else self.mlp(self.norm2(x), residual=x)
 
 
 class PatchMerging(nn.Module):
