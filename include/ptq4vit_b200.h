@@ -300,6 +300,37 @@ P4V_API int p4v_mlp_frozen_forward_norm_res(const p4v_linear_desc* fc1, const fl
                                             size_t pack2_bytes, void* workspace, size_t workspace_bytes,
                                             const float* residual, float* out, void* stream);
 
+/* A row gather in front of a LayerNorm folded into its frozen Linear: out = layer(LayerNorm(gather(x))), where the rows
+ * the layer consumes are read from an image x [images][height][width][C] (contiguous, 16-byte aligned) instead of being
+ * copied there by torch first.  LayerNorm is per row, so the normalised rows are those of the unfolded sequence; the
+ * result is bit-identical to it and neither the normalised nor the gathered activations reach HBM.
+ * P4V_GATHER_WINDOW (Swin's norm1 -> roll(-shift) -> window partition -> qkv): C = in_features, and output row r, in
+ * window order
+ *   r = ((b * nH + wh) * nW + ww) * window^2 + i * window + j      (nH = height / window, nW = width / window)
+ * is computed from image row b * height * width + ((wh * window + i + shift) mod height) * width + (ww * window + j + shift)
+ * mod width -- the window layout of p4v_linear_frozen_forward_res, read in the other direction.  The layout needs
+ * window > 0, height % window == 0, width % window == 0, 0 <= shift < window and images * height * width == rows.
+ * P4V_GATHER_MERGE (Swin's PatchMerging: cat(x[0::2, 0::2], x[1::2, 0::2], x[0::2, 1::2], x[1::2, 1::2]) -> norm ->
+ * reduction): in_features = 4 C, and output row m = (b * (height / 2) + i) * (width / 2) + j takes its columns
+ * [q C, (q + 1) C) from image row b * height * width + (2 i + (q & 1)) * width + 2 j + (q >> 1), q = 0 .. 3.  The layout
+ * has window = shift = 0, height and width even and images * (height / 2) * (width / 2) == rows.
+ * p4v_linear_gather_ok is the shape rule of a mode, a pure function of the descriptor without its rows: p4v_linear_norm_ok,
+ * in_features % 16 == 0 for the merge, and the shared-memory plan with the 512-byte table of source rows fits.  A layer
+ * on the streamed path (p4v_linear_frozen_path 0) never takes a gather.
+ * p4v_linear_frozen_forward_norm_gather mirrors p4v_linear_frozen_forward_norm with the image x and the descriptor g.
+ * Every argument is validated before its one launch (the LayerNorm's as there, g, the rule, the layout, x not
+ * overlapping out); nothing is allocated or copied, so it can be captured in a CUDA graph. */
+#define P4V_GATHER_WINDOW 1
+#define P4V_GATHER_MERGE 2
+typedef struct p4v_input_gather {
+  int32_t mode;                  /* P4V_GATHER_WINDOW or P4V_GATHER_MERGE */
+  p4v_window_layout layout;      /* the image: images, height, width; the window and shift (merge: 0, 0) */
+} p4v_input_gather;
+P4V_API int p4v_linear_gather_ok(const p4v_linear_desc* d, const p4v_input_gather* g, int* ok);
+P4V_API int p4v_linear_frozen_forward_norm_gather(const p4v_linear_desc* d, const float* x, const float* gamma,
+                                                  const float* beta, float eps, const float* bias, const void* packed,
+                                                  const p4v_input_gather* g, float* out, void* stream);
+
 /* The patch-embedding convolution: ChannelwiseBatchingQuantConv2d with a_bit >= 32 (quant_layers/conv.py:444-614, wired
  * by configs/PTQ4ViT.py:52-54): one weight step size per output channel, activations left in FP32.  The caller passes
  * the im2col matrix of the FP32 input (torch.nn.functional.unfold, [images, positions, K], K = in_channels*kh*kw in the

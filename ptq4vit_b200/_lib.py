@@ -49,6 +49,13 @@ class WindowLayout(C.Structure):
     _fields_ = [("images", C.c_int32), ("height", C.c_int32), ("width", C.c_int32), ("window", C.c_int32), ("shift", C.c_int32)]
 
 
+GATHER = {"window": 1, "merge": 2}      # P4V_GATHER_WINDOW, P4V_GATHER_MERGE
+
+
+class InputGather(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("layout", WindowLayout)]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     "p4v_linear_workspace_bytes": [C.POINTER(LinearDesc), C.POINTER(C.c_size_t)],
@@ -95,6 +102,8 @@ _SIGNATURES = {
                                    C.c_size_t, _P, _P, _P],
     "p4v_mlp_frozen_forward_norm_res": [C.POINTER(LinearDesc), _P, _P, _P, C.c_float, _P, _P, C.c_size_t, C.POINTER(LinearDesc),
                                         _P, _P, C.c_size_t, _P, C.c_size_t, _P, _P, _P],
+    "p4v_linear_gather_ok": [C.POINTER(LinearDesc), C.POINTER(InputGather), C.POINTER(C.c_int)],
+    "p4v_linear_frozen_forward_norm_gather": [C.POINTER(LinearDesc), _P, _P, _P, C.c_float, _P, _P, C.POINTER(InputGather), _P, _P],
     "p4v_conv_workspace_bytes": [C.POINTER(ConvDesc), C.POINTER(C.c_size_t)],
     "p4v_conv_calibrate": [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P],
     "p4v_conv_frozen_ok": [C.POINTER(ConvFrozenDesc), C.POINTER(C.c_int)],

@@ -23,6 +23,8 @@
 // quantising it (DESIGN §4.10).
 // With FwdResParams a block's residual add is folded into the FP32 store: each value goes to its destination row (the
 // identity, or Swin's window reverse and reverse shift, p4v_window_row) as fl(value + shortcut) (DESIGN §4.11).
+// With FwdGatherParams the LayerNorm prologue and the quantise loop read each row from elsewhere in an image: Swin's
+// shifted window partition (p4v_window_row) or PatchMerging's 2x2 neighbourhood (p4v_merge_row) (DESIGN §4.12).
 // 288 threads leave 224 registers per thread without setmaxnreg; the bounded mbarrier wait is inline, and the k32 steps of
 // a stage are one straight-line batch selected by a warp-uniform count (ptxas C7520, see sm90.cuh).
 #include "../../include/ptq4vit_b200.h"
@@ -161,9 +163,63 @@ __device__ __forceinline__ float* ln_stats(const Par& P, uint8_t* smem) {
                                   (p4v_fwd_extra_bytes(P) - P4V_NORM_STATS_BYTES));
 }
 
+// ---- the row gather of FwdGatherParams (DESIGN §4.12) ----------------------------------------------------------------
+// The source row of each tile row, right below the row stats: the window map's image row, or the merge's first row
+__device__ __forceinline__ int* gather_rows(const FwdGatherParams& P, uint8_t* smem) {
+  return reinterpret_cast<int*>(ln_stats(P, smem)) - P4V_TILE;
+}
+
+// Mean and rstd of tile row r (global row `row`), read from its source rows; returns the source row
+__device__ __forceinline__ int gather_row_stats(const FwdGatherParams& P, int row, int lane, float& mean, float& rstd) {
+  const int K = (int)P.ld;
+  if (P.ga.mode == P4V_GATHER_WINDOW) {
+    const int s = p4v_window_row(P.ga.win, row);
+    p4v_ln_row_stats(P.x + (size_t)s * K, K, P.ln.eps, lane, mean, rstd);
+    return s;
+  }
+  // merge: float4 i of the 4C row lies in quarter i / (C / 4), since C % 4 == 0
+  const int s = p4v_merge_row(P.ga.win, row), c4 = K >> 4;
+  const float4* x4 = reinterpret_cast<const float4*>(P.x);
+  const p4v_window_layout win = P.ga.win;
+  p4v_ln_row_stats_at([=](int i) {
+    const int q = i / c4;
+    return x4 + (size_t)(s + p4v_merge_quarter(win, q)) * c4 + (i - q * c4);
+  }, K, P.ln.eps, lane, mean, rstd);
+  return s;
+}
+
+// The chunk's FP32 values (ch.n of them, zeros after) of the tile row whose source row is s.  A merge chunk inside one
+// quarter reads like a contiguous row; one that straddles two quarters (C % 16 != 0) reads element by element.
+__device__ __forceinline__ void gather_chunk(const FwdGatherParams& P, int s, int k0, int n, float (&vals)[16]) {
+  const int K = (int)P.ld;
+  const float* src;
+  if (P.ga.mode == P4V_GATHER_WINDOW) {
+    src = P.x + (size_t)s * K + k0;
+  } else {
+    const int C = K >> 2, q = k0 / C, c = k0 - q * C;
+    if (c + n > C) {
+#pragma unroll
+      for (int e = 0; e < 16; ++e) {
+        const int k = k0 + e, qe = k / C;
+        vals[e] = e < n ? __ldg(P.x + (size_t)(s + p4v_merge_quarter(P.ga.win, qe)) * C + (k - qe * C)) : 0.f;
+      }
+      return;
+    }
+    src = P.x + (size_t)(s + p4v_merge_quarter(P.ga.win, q)) * C + c;
+  }
+  if (n == 16 && (reinterpret_cast<uintptr_t>(src) & 15) == 0) {
+    const float4* src4 = reinterpret_cast<const float4*>(src);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) { const float4 t4 = __ldg(src4 + e); vals[4 * e] = t4.x; vals[4 * e + 1] = t4.y; vals[4 * e + 2] = t4.z; vals[4 * e + 3] = t4.w; }
+  } else {
+#pragma unroll
+    for (int e = 0; e < 16; ++e) vals[e] = e < n ? __ldg(src + e) : 0.f;
+  }
+}
+
 // Par = FwdParams: the frozen Linear forward, FP32 output.  Par = FwdMlpParams: fc1 of a frozen MLP, GELU-and-quantise
 // epilogue into fc2's image.  FwdNormParams / FwdMlpNormParams: the same with a LayerNorm prologue.  FwdResParams: the
-// plain forward whose store adds the shortcut.
+// plain forward whose store adds the shortcut.  FwdGatherParams: FwdNormParams with gathered rows.
 template <class Par>
 __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_constant__ Par P) {
   constexpr bool kMlp = kIsMlp<Par>;
@@ -187,7 +243,12 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
       const int row = tm * P4V_TILE + r;
       if (row >= P.M) break;
       float mean, rstd;
-      p4v_ln_row_stats(P.x + (size_t)row * P.ld, (int)P.ld, P.ln.eps, lane, mean, rstd);
+      if constexpr (kIsGather<Par>) {
+        const int s = gather_row_stats(P, row, lane, mean, rstd);
+        if (lane == 0) gather_rows(P, smem)[r] = s;
+      } else {
+        p4v_ln_row_stats(P.x + (size_t)row * P.ld, (int)P.ld, P.ln.eps, lane, mean, rstd);
+      }
       if (lane == 0) { ln_mean[r] = mean; ln_mean[P4V_TILE + r] = rstd; }
     }
   }
@@ -218,14 +279,18 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
       uint32_t wp[4] = {0u, 0u, 0u, 0u}, wn[4] = {0u, 0u, 0u, 0u};
       if (row < P.M && ch.n > 0) {
         float vals[16];
-        const float* src = P.x + (size_t)row * P.ld + ch.k0;
-        if (ch.n == 16 && ((P.ld | ch.k0) & 3) == 0) {
-          const float4* src4 = reinterpret_cast<const float4*>(src);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) { const float4 t4 = __ldg(src4 + e); vals[4 * e] = t4.x; vals[4 * e + 1] = t4.y; vals[4 * e + 2] = t4.z; vals[4 * e + 3] = t4.w; }
+        if constexpr (kIsGather<Par>) {
+          gather_chunk(P, gather_rows(P, smem)[r], ch.k0, ch.n, vals);
         } else {
+          const float* src = P.x + (size_t)row * P.ld + ch.k0;
+          if (ch.n == 16 && ((P.ld | ch.k0) & 3) == 0) {
+            const float4* src4 = reinterpret_cast<const float4*>(src);
 #pragma unroll
-          for (int e = 0; e < 16; ++e) vals[e] = e < ch.n ? src[e] : 0.f;
+            for (int e = 0; e < 4; ++e) { const float4 t4 = __ldg(src4 + e); vals[4 * e] = t4.x; vals[4 * e + 1] = t4.y; vals[4 * e + 2] = t4.z; vals[4 * e + 3] = t4.w; }
+          } else {
+#pragma unroll
+            for (int e = 0; e < 16; ++e) vals[e] = e < ch.n ? src[e] : 0.f;
+          }
         }
         if constexpr (kIsNorm<Par>) {
           const float* ln_mean = ln_stats(P, smem);
@@ -401,6 +466,15 @@ template <class Par> int p4v_launch_forward_tc(const Par& p, int num_sms, cudaSt
     P4V_REQUIRE(w.window == 0 || ((long long)w.images * w.height * w.width == p.M && w.height % w.window == 0 &&
                                   w.width % w.window == 0 && w.shift >= 0 && w.shift < w.window), "forward: bad window layout");
   }
+  if constexpr (kIsGather<Par>) {
+    const p4v_window_layout& w = p.ga.win;
+    const bool window = p.ga.mode == P4V_GATHER_WINDOW && w.window > 0 && w.height % w.window == 0 &&
+                        w.width % w.window == 0 && w.shift >= 0 && w.shift < w.window && p.ld % 4 == 0 &&
+                        (long long)w.images * w.height * w.width == p.M;
+    const bool merge = p.ga.mode == P4V_GATHER_MERGE && w.window == 0 && w.shift == 0 && w.height % 2 == 0 &&
+                       w.width % 2 == 0 && p.ld % 16 == 0 && (long long)w.images * (w.height / 2) * (w.width / 2) == p.M;
+    P4V_REQUIRE(w.images > 0 && w.height > 0 && w.width > 0 && (window || merge), "forward: bad gather layout");
+  }
   const unsigned extra = p4v_fwd_extra_bytes(p);
   P4V_REQUIRE(p.n_jobs >= 1 && p.n_jobs <= P4V_MAX_JOBS && p.n_groups <= P4V_MAX_GROUPS, "forward: too many K segments");
   P4V_REQUIRE(p.n_stages >= 2 && p.n_stages <= P4V_FWD_MAX_STAGES && p.n_chunks <= P4V_FWD_MAX_CHUNKS &&
@@ -424,6 +498,7 @@ template int p4v_launch_forward_tc(const FwdMlpParams&, int, cudaStream_t);
 template int p4v_launch_forward_tc(const FwdNormParams&, int, cudaStream_t);
 template int p4v_launch_forward_tc(const FwdMlpNormParams&, int, cudaStream_t);
 template int p4v_launch_forward_tc(const FwdResParams&, int, cudaStream_t);
+template int p4v_launch_forward_tc(const FwdGatherParams&, int, cudaStream_t);
 
 // Diagnostic: y = p4v_gelu(x) elementwise (the GELU of mlp_fc1_kernel's epilogue)
 extern "C" int p4v_gelu_probe(const float* x, float* y, long long n, void* stream) {

@@ -741,16 +741,24 @@ int build_frozen(const p4v_linear_desc* d, FrozenPlan& f, bool for_pack) {
 }
 
 // The ring stages the fused kernel gets for a call of the layer f1 -- as fc1 of a fused MLP whose fc2 is f2, with a
-// LayerNorm folded into its activation quantiser (norm) -- or 0 when the call does not take the fused kernel.  f1 must
-// be on it itself; an MLP needs fc1's outputs to be fc2's inputs and a plain fc1, a LayerNorm a plain layer with K % 4 == 0.
-// The epilogue and the row stats take their share of shared memory, which can only lower the count.
-int fused_stages(const FrozenPlan& f1, const FrozenPlan* f2, bool norm) {
+// LayerNorm folded into its activation quantiser (norm), with a row gather in front of that LayerNorm (gather) -- or 0
+// when the call does not take the fused kernel.  f1 must be on it itself; an MLP needs fc1's outputs to be fc2's inputs
+// and a plain fc1, a LayerNorm a plain layer with K % 4 == 0.  The epilogue, the gather's source rows and the row stats
+// take their share of shared memory, which can only lower the count.
+int fused_stages(const FrozenPlan& f1, const FrozenPlan* f2, bool norm, bool gather = false) {
   const LinPlan& p1 = f1.p;
   if (f1.stages < 2 || (f2 && (p1.O != f2->p.K || p1.twin)) || (norm && (p1.twin || p1.K % 4 != 0))) return 0;
   // a plane of fc2's activation image has the K layout of its weight image; a post-GELU fc2 has two
   const unsigned epi = f2 ? p4v_mlp_epi_bytes(f2->p.twin ? 2 : 1, f2->p.Wcur.kb / 16) : 0u;
-  return frozen_ring_stages(f1.X.tile_bytes() + p4v_fwd_extra_bytes(epi, norm), (size_t)f1.stage_kb * P4V_TILE,
+  return frozen_ring_stages(f1.X.tile_bytes() + p4v_fwd_extra_bytes(epi, norm, gather), (size_t)f1.stage_kb * P4V_TILE,
                             p1.Wcur.kb / 16);
+}
+
+// The ring stages of a row gather of `mode` in front of the LayerNorm folded into f (p4v_linear_gather_ok), 0 when it
+// does not fold: the merge needs C = K / 4 a multiple of 4, so that no float4 of the LayerNorm's walk straddles a quarter.
+int gather_stages(const FrozenPlan& f, int mode) {
+  if (mode == P4V_GATHER_MERGE && f.p.K % 16 != 0) return 0;
+  return fused_stages(f, nullptr, true, true);
 }
 
 }  // namespace
@@ -846,6 +854,49 @@ int check_norm(const char* what, const float* x, const float* gamma, const float
   return 0;
 }
 
+// The window layout rule of a layer with `rows` output rows (DESIGN §4.11)
+int check_layout(const char* fn, const p4v_window_layout& win, int rows) {
+  P4V_REQUIRE(win.window > 0 && win.height > 0 && win.width > 0 && win.images > 0,
+              "%s: window layout needs positive images, height, width and window (got %d, %d, %d, %d)", fn, win.images,
+              win.height, win.width, win.window);
+  P4V_REQUIRE(win.height % win.window == 0 && win.width % win.window == 0,
+              "%s: window layout: height %d and width %d must be multiples of the window %d", fn, win.height, win.width,
+              win.window);
+  P4V_REQUIRE(win.shift >= 0 && win.shift < win.window, "%s: window layout: shift %d must lie in [0, window %d)", fn,
+              win.shift, win.window);
+  P4V_REQUIRE((long long)win.images * win.height * win.width == rows,
+              "%s: window layout: images * height * width = %lld, the layer has %d rows", fn,
+              (long long)win.images * win.height * win.width, rows);
+  return 0;
+}
+
+// The arguments of a row gather (DESIGN §4.12) of a call with `rows` output rows and K = in_features, the image x
+// apart from out ([rows][out_cols]); x's null pointer and alignment are check_norm's
+int check_gather(const char* fn, const p4v_input_gather* g, const float* x, const float* out, int rows, int K, int out_cols) {
+  P4V_REQUIRE(g, "%s: null pointer", fn);
+  const p4v_window_layout& w = g->layout;
+  if (g->mode == P4V_GATHER_WINDOW) {
+    if (int rc = check_layout(fn, w, rows)) return rc;
+  } else {
+    P4V_REQUIRE(g->mode == P4V_GATHER_MERGE, "%s: gather mode must be P4V_GATHER_WINDOW or P4V_GATHER_MERGE (got %d)", fn,
+                g->mode);
+    P4V_REQUIRE(w.window == 0 && w.shift == 0, "%s: merge layout: window and shift must be 0 (got %d, %d)", fn, w.window,
+                w.shift);
+    P4V_REQUIRE(w.images > 0 && w.height > 0 && w.width > 0 && w.height % 2 == 0 && w.width % 2 == 0,
+                "%s: merge layout needs positive images and even height and width (got %d, %d, %d)", fn, w.images,
+                w.height, w.width);
+    P4V_REQUIRE(K % 4 == 0, "%s: merge: in_features %d must be 4 C", fn, K);
+    P4V_REQUIRE((long long)w.images * (w.height / 2) * (w.width / 2) == rows,
+                "%s: merge layout: images * (height / 2) * (width / 2) = %lld, the layer has %d rows", fn,
+                (long long)w.images * (w.height / 2) * (w.width / 2), rows);
+  }
+  // either way the image holds rows * K floats
+  const uintptr_t xb = (uintptr_t)rows * (uintptr_t)K * 4, ob = (uintptr_t)rows * (uintptr_t)out_cols * 4,
+                  a = reinterpret_cast<uintptr_t>(x), b = reinterpret_cast<uintptr_t>(out);
+  P4V_REQUIRE(a + xb <= b || b + ob <= a, "%s: x overlaps out", fn);
+  return 0;
+}
+
 // The arguments of a folded residual add (res non-null) of a call whose output out is [rows][cols]: res 8-byte aligned
 // and apart from out, and the window layout's rule (win.window == 0: identity rows).  Nothing to check without res.
 int check_residual(const char* fn, const float* res, const float* out, int rows, int cols, const p4v_window_layout& win) {
@@ -854,19 +905,8 @@ int check_residual(const char* fn, const float* res, const float* out, int rows,
   const uintptr_t bytes = (uintptr_t)rows * (uintptr_t)cols * 4, a = reinterpret_cast<uintptr_t>(res),
                   b = reinterpret_cast<uintptr_t>(out);
   P4V_REQUIRE(a + bytes <= b || b + bytes <= a, "%s: residual overlaps out", fn);
-  if (win.window != 0 || win.images != 0 || win.height != 0 || win.width != 0 || win.shift != 0) {
-    P4V_REQUIRE(win.window > 0 && win.height > 0 && win.width > 0 && win.images > 0,
-                "%s: window layout needs positive images, height, width and window (got %d, %d, %d, %d)", fn, win.images,
-                win.height, win.width, win.window);
-    P4V_REQUIRE(win.height % win.window == 0 && win.width % win.window == 0,
-                "%s: window layout: height %d and width %d must be multiples of the window %d", fn, win.height, win.width,
-                win.window);
-    P4V_REQUIRE(win.shift >= 0 && win.shift < win.window, "%s: window layout: shift %d must lie in [0, window %d)", fn,
-                win.shift, win.window);
-    P4V_REQUIRE((long long)win.images * win.height * win.width == rows,
-                "%s: window layout: images * height * width = %lld, the layer has %d rows", fn,
-                (long long)win.images * win.height * win.width, rows);
-  }
+  if (win.window != 0 || win.images != 0 || win.height != 0 || win.width != 0 || win.shift != 0)
+    return check_layout(fn, win, rows);
   return 0;
 }
 
@@ -878,9 +918,9 @@ int check_residual(const char* fn, const float* res, const float* out, int rows,
 // (FwdResParams, with rs.win) or fc2's sweep (identity rows).
 template <class Par>
 int fused_forward(const char* fn, const FrozenPlan& f1, const float* x, const FwdNorm& ln, const FwdResidual& rs,
-                  const float* bias1, const void* pack1, size_t pack1_bytes, const FrozenPlan* f2, const float* bias2,
-                  const void* pack2, size_t pack2_bytes, void* workspace, size_t workspace_bytes, float* out,
-                  cudaStream_t st) {
+                  const p4v_input_gather* ga, const float* bias1, const void* pack1, size_t pack1_bytes,
+                  const FrozenPlan* f2, const float* bias2, const void* pack2, size_t pack2_bytes, void* workspace,
+                  size_t workspace_bytes, float* out, cudaStream_t st) {
   constexpr bool mlp = kIsMlp<Par>, norm = kIsNorm<Par>;
   if constexpr (norm) {
     if (int rc = check_norm(fn, x, ln.gamma, ln.beta, ln.eps)) return rc;
@@ -890,10 +930,16 @@ int fused_forward(const char* fn, const FrozenPlan& f1, const float* x, const Fw
                 f2->p.d.rows);
   P4V_REQUIRE(x && pack1 && (!mlp || (pack2 && workspace)) && out, "%s: null pointer", fn);
   P4V_REQUIRE((!f1.p.d.has_bias || bias1) && (!mlp || !f2->p.d.has_bias || bias2), "%s: has_bias set but bias is null", fn);
-  const int stages = fused_stages(f1, f2, norm);
+  constexpr bool gather = kIsGather<Par>;
+  if constexpr (gather) P4V_REQUIRE(ga, "%s: null pointer", fn);
+  const int stages = gather ? gather_stages(f1, ga->mode) : fused_stages(f1, f2, norm);
   P4V_REQUIRE(stages, "%s: %s", fn, mlp ? (norm ? "these layers do not fuse with the LayerNorm (p4v_mlp_norm_ok)"
                                                 : "these layers do not fuse (p4v_mlp_fused_ok)")
-                                        : "the LayerNorm does not fold into this layer (p4v_linear_norm_ok)");
+                                        : gather ? "the gather does not fold into this layer (p4v_linear_gather_ok)"
+                                                 : "the LayerNorm does not fold into this layer (p4v_linear_norm_ok)");
+  if constexpr (gather) {
+    if (int rc = check_gather(fn, ga, x, out, f1.p.M, f1.p.K, f1.p.O)) return rc;
+  }
   if constexpr (mlp) {
     P4V_REQUIRE(pack1_bytes >= f1.bytes && pack2_bytes >= f2->bytes, "%s: packed buffer too small "
                 "(fc1 %zu < %zu or fc2 %zu < %zu)", fn, pack1_bytes, f1.bytes, pack2_bytes, f2->bytes);
@@ -913,6 +959,7 @@ int fused_forward(const char* fn, const FrozenPlan& f1, const float* x, const Fw
   if constexpr (norm) q.ln = ln;
   if constexpr (mlp) fill_mlp(*f2, p2, workspace, q);
   if constexpr (kIsRes<Par>) q.rs = rs;
+  if constexpr (gather) q.ga = FwdGather{ga->mode, ga->layout};
   const int rc = p4v_launch_forward_tc(q, p4v_num_sms(), st);
   if (rc || !mlp) return rc;
   return streamed_sweep(*f2, p2, workspace, bias2, rs.res, out, st);
@@ -929,10 +976,10 @@ int frozen_forward(const char* fn, const p4v_linear_desc* d, const float* x, con
   P4V_REQUIRE(!d->has_bias || bias, "%s: has_bias set but bias is null", fn);
   if (fused_stages(f, nullptr, false)) {
     if (rs.res)
-      return fused_forward<FwdResParams>(fn, f, x, FwdNorm{}, rs, bias, packed, 0, nullptr, nullptr, nullptr, 0, nullptr, 0,
-                                         out, st);
-    return fused_forward<FwdParams>(fn, f, x, FwdNorm{}, rs, bias, packed, 0, nullptr, nullptr, nullptr, 0, nullptr, 0, out,
-                                    st);
+      return fused_forward<FwdResParams>(fn, f, x, FwdNorm{}, rs, nullptr, bias, packed, 0, nullptr, nullptr, nullptr, 0,
+                                         nullptr, 0, out, st);
+    return fused_forward<FwdParams>(fn, f, x, FwdNorm{}, rs, nullptr, bias, packed, 0, nullptr, nullptr, nullptr, 0, nullptr,
+                                    0, out, st);
   }
   P4V_REQUIRE(workspace && workspace_bytes >= f.X.bytes(), "%s: workspace too small (%zu < %zu)", fn,
               workspace ? workspace_bytes : (size_t)0, f.X.bytes());
@@ -988,8 +1035,8 @@ extern "C" int p4v_mlp_frozen_forward(const p4v_linear_desc* fc1, const float* x
                                       size_t pack2_bytes, void* workspace, size_t workspace_bytes, float* out, void* stream) {
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
-  return fused_forward<FwdMlpParams>("mlp_frozen_forward", f1, x, FwdNorm{}, FwdResidual{}, bias1, pack1, pack1_bytes, &f2,
-                                     bias2, pack2, pack2_bytes, workspace, workspace_bytes, out, (cudaStream_t)stream);
+  return fused_forward<FwdMlpParams>("mlp_frozen_forward", f1, x, FwdNorm{}, FwdResidual{}, nullptr, bias1, pack1, pack1_bytes,
+                                     &f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out, (cudaStream_t)stream);
 }
 
 // ---- LayerNorm folded into the activation quantiser of the fused kernel (forward_tc.cu, DESIGN §4.10) -------------
@@ -1013,8 +1060,8 @@ extern "C" int p4v_linear_frozen_forward_norm(const p4v_linear_desc* d, const fl
                                               float eps, const float* bias, const void* packed_in, float* out, void* stream) {
   FrozenPlan f; int rc = build_frozen(d, f, false);
   if (rc) return rc;
-  return fused_forward<FwdNormParams>("linear_frozen_forward_norm", f, x, FwdNorm{gamma, beta, eps}, FwdResidual{}, bias,
-                                      packed_in, 0, nullptr, nullptr, nullptr, 0, nullptr, 0, out, (cudaStream_t)stream);
+  return fused_forward<FwdNormParams>("linear_frozen_forward_norm", f, x, FwdNorm{gamma, beta, eps}, FwdResidual{}, nullptr,
+                                      bias, packed_in, 0, nullptr, nullptr, nullptr, 0, nullptr, 0, out, (cudaStream_t)stream);
 }
 
 extern "C" int p4v_mlp_frozen_forward_norm(const p4v_linear_desc* fc1, const float* x, const float* gamma, const float* beta,
@@ -1023,9 +1070,9 @@ extern "C" int p4v_mlp_frozen_forward_norm(const p4v_linear_desc* fc1, const flo
                                            void* workspace, size_t workspace_bytes, float* out, void* stream) {
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
-  return fused_forward<FwdMlpNormParams>("mlp_frozen_forward_norm", f1, x, FwdNorm{gamma, beta, eps}, FwdResidual{}, bias1,
-                                         pack1, pack1_bytes, &f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out,
-                                         (cudaStream_t)stream);
+  return fused_forward<FwdMlpNormParams>("mlp_frozen_forward_norm", f1, x, FwdNorm{gamma, beta, eps}, FwdResidual{},
+                                         nullptr, bias1, pack1, pack1_bytes, &f2, bias2, pack2, pack2_bytes, workspace,
+                                         workspace_bytes, out, (cudaStream_t)stream);
 }
 
 // ---- a block's residual add folded into the store of the frozen Linear that produces it (DESIGN §4.11) -------------
@@ -1046,8 +1093,8 @@ extern "C" int p4v_mlp_frozen_forward_res(const p4v_linear_desc* fc1, const floa
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
   P4V_REQUIRE(residual, "mlp_frozen_forward_res: null pointer");
-  return fused_forward<FwdMlpParams>("mlp_frozen_forward_res", f1, x, FwdNorm{}, FwdResidual{residual, {}}, bias1, pack1,
-                                     pack1_bytes, &f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out,
+  return fused_forward<FwdMlpParams>("mlp_frozen_forward_res", f1, x, FwdNorm{}, FwdResidual{residual, {}}, nullptr, bias1,
+                                     pack1, pack1_bytes, &f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out,
                                      (cudaStream_t)stream);
 }
 
@@ -1060,6 +1107,28 @@ extern "C" int p4v_mlp_frozen_forward_norm_res(const p4v_linear_desc* fc1, const
   if (rc) return rc;
   P4V_REQUIRE(residual, "mlp_frozen_forward_norm_res: null pointer");
   return fused_forward<FwdMlpNormParams>("mlp_frozen_forward_norm_res", f1, x, FwdNorm{gamma, beta, eps},
-                                         FwdResidual{residual, {}}, bias1, pack1, pack1_bytes, &f2, bias2, pack2, pack2_bytes,
-                                         workspace, workspace_bytes, out, (cudaStream_t)stream);
+                                         FwdResidual{residual, {}}, nullptr, bias1, pack1, pack1_bytes, &f2, bias2, pack2,
+                                         pack2_bytes, workspace, workspace_bytes, out, (cudaStream_t)stream);
+}
+
+// ---- a row gather in front of the LayerNorm folded into its frozen Linear (DESIGN §4.12) ---------------------------
+// Replaces  layer(LayerNorm(gather(x)))  with gather Swin's roll(-shift) + window partition, or PatchMerging's 2x2 cat.
+extern "C" int p4v_linear_gather_ok(const p4v_linear_desc* d, const p4v_input_gather* g, int* ok) {
+  FrozenPlan f; int rc = build_frozen(d, f, true);
+  if (rc) return rc;
+  P4V_REQUIRE(g && ok, "null argument");
+  P4V_REQUIRE(g->mode == P4V_GATHER_WINDOW || g->mode == P4V_GATHER_MERGE,
+              "linear_gather_ok: gather mode must be P4V_GATHER_WINDOW or P4V_GATHER_MERGE (got %d)", g->mode);
+  *ok = gather_stages(f, g->mode) ? 1 : 0;
+  return 0;
+}
+
+extern "C" int p4v_linear_frozen_forward_norm_gather(const p4v_linear_desc* d, const float* x, const float* gamma,
+                                                     const float* beta, float eps, const float* bias, const void* packed,
+                                                     const p4v_input_gather* g, float* out, void* stream) {
+  FrozenPlan f; int rc = build_frozen(d, f, false);
+  if (rc) return rc;
+  return fused_forward<FwdGatherParams>("linear_frozen_forward_norm_gather", f, x, FwdNorm{gamma, beta, eps}, FwdResidual{},
+                                        g, bias, packed, 0, nullptr, nullptr, nullptr, 0, nullptr, 0, out,
+                                        (cudaStream_t)stream);
 }

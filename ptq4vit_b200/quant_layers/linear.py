@@ -243,20 +243,22 @@ def _streamed_image(lin, dev, fn, *descs):
     return lin._frozen_ws
 
 
-def _frozen_call(lin, x, norm=None, fc2=None, residual=None, layout=None):
+def _frozen_call(lin, x, norm=None, fc2=None, residual=None, layout=None, gather=None):
     """One library call of frozen layers: lin(x), on lin's fused kernel or its streamed path; with `norm`, lin(norm(x))
     with the LayerNorm folded into lin's fused kernel; with `fc2`, fc2(gelu(lin(...))) as the fused MLP; with
     `residual`, residual + that output, the add folded into the last layer's store (with `layout`, an (images, height,
-    width, window, shift) window layout of lin's output rows: Swin's window reverse and reverse shift before the add).
-    The callers' rules say which applies; the library validates the call.  Only the output (and a missing streamed image)
-    is allocated."""
+    width, window, shift) window layout of lin's output rows: Swin's window reverse and reverse shift before the add);
+    with `gather` (and `norm`), lin(norm(rows of the image x)), the rows gathered by lin's fused kernel (see
+    frozen_gather_applies).  The callers' rules say which applies; the library validates the call.  Only the output (and a
+    missing streamed image) is allocated."""
     for m in (lin, fc2):
         if m is not None:
             m._check_frozen_intervals()
     dev = lin._packed.device
     x2 = _flat2d(x.to(dev))
     b1, b2 = (None if m is None or m.bias is None else m.bias.detach().contiguous().float() for m in (lin, fc2))
-    d1 = lin._desc(x2.shape[0], 1)
+    rows = x2.shape[0] if gather is None else _gather_rows(gather)
+    d1 = lin._desc(rows, 1)
     args = [ctypes.byref(d1), _lib.ptr(x2)]
     if norm is not None:
         args += [_lib.ptr(norm.weight), _lib.ptr(norm.bias), float(norm.eps)]
@@ -271,8 +273,11 @@ def _frozen_call(lin, x, norm=None, fc2=None, residual=None, layout=None):
     if fc2 is not None or norm is None:
         args += [_lib.ptr(ws), 0 if ws is None else ws.numel()]
     last = lin if fc2 is None else fc2
-    out = torch.empty(x2.shape[0], last.out_features, dtype=torch.float32, device=dev)
+    out = torch.empty(rows, last.out_features, dtype=torch.float32, device=dev)
     fn = ("p4v_linear_frozen_forward" if fc2 is None else "p4v_mlp_frozen_forward") + ("" if norm is None else "_norm")
+    if gather is not None:
+        fn += "_gather"
+        args.append(ctypes.byref(_gather_desc(gather)))
     if residual is not None:
         fn += "_res"
         args.append(_lib.ptr(residual))
@@ -281,7 +286,21 @@ def _frozen_call(lin, x, norm=None, fc2=None, residual=None, layout=None):
     _lib.check(getattr(_lib.lib(), fn)(*args, _lib.ptr(out), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), fn)
     if residual is not None:
         return out.view(residual.shape)
+    if gather is not None:
+        mode, images, _height, _width, window, _shift = gather
+        return out.view(-1, window * window, lin.out_features) if mode == "window" else out.view(images, -1, lin.out_features)
     return out.reshape(*x.shape[:-1], last.out_features)
+
+
+def _gather_desc(gather):
+    mode, *layout = gather
+    return _lib.InputGather(_lib.GATHER[mode], _lib.WindowLayout(*[int(v) for v in layout]))
+
+
+def _gather_rows(gather):
+    """The output rows of a gathered call: the image's rows (window), a quarter of them (merge)"""
+    mode, images, height, width, _window, _shift = gather
+    return images * height * width if mode == "window" else images * (height // 2) * (width // 2)
 
 
 def frozen_mlp_applies(fc1, fc2, act, x):
@@ -354,6 +373,11 @@ def frozen_norm_applies(norm, lin, x):
     lin's device, under grad mode no input and no parameter of norm or lin that requires grad, and the case in which torch
     itself runs its vectorised LayerNorm kernel (FP32 weight and bias, 16-byte aligned data) -- the kernel whose bits the
     fold reproduces (DESIGN.md section 4.10)."""
+    return _norm_call_ok(norm, lin, x) and _rule("p4v_linear_norm_ok", lin)
+
+
+def _norm_call_ok(norm, lin, x):
+    """frozen_norm_applies without the library's shape rule"""
     if type(norm) is not nn.LayerNorm or norm.weight is None or norm.bias is None:
         return False
     if not (isinstance(lin, MinMaxQuantLinear) and lin.frozen and lin.mode == "quant_forward"):
@@ -369,7 +393,7 @@ def frozen_norm_applies(norm, lin, x):
         return False
     if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in (norm, lin) for p in m.parameters())):
         return False
-    return _rule("p4v_linear_norm_ok", lin)
+    return True
 
 
 def frozen_mlp_norm_ok(fc1, fc2):
@@ -383,6 +407,46 @@ def frozen_norm_linear(norm, lin, x):
     computed in the activation quantiser of lin's fused kernel (csrc/forward_tc.cu), bit-identical to the unfolded call;
     the normalised activations never reach HBM.  Only the output is allocated."""
     return _frozen_call(lin, x, norm=norm)
+
+
+def frozen_gather_ok(lin, mode):
+    """The library's shape rule of a row gather (p4v_linear_gather_ok) for lin, mode "window" or "merge":
+    p4v_linear_norm_ok, in_features % 16 == 0 for the merge, the shared-memory plan with the table of source rows fits."""
+    ok = ctypes.c_int()
+    g = _gather_desc((mode, 0, 0, 0, 0, 0))
+    _lib.check(_lib.lib().p4v_linear_gather_ok(ctypes.byref(lin._desc(1, 1)), ctypes.byref(g), ctypes.byref(ok)),
+               "p4v_linear_gather_ok")
+    return bool(ok.value)
+
+
+def frozen_gather_applies(norm, lin, x, gather):
+    """Whether lin(norm(rows gathered from x)) can run as one folded call (frozen_gather_linear).  gather is
+    ("window", images, height, width, window, shift): x is Swin's [images, height * width, C] block input and the rows
+    are those of window_partition(roll(x, (-shift, -shift))), C = lin.in_features; or ("merge", images, height, width, 0,
+    0): x is PatchMerging's [images, height * width, C] input and the rows are its cat of the 2x2 neighbourhoods,
+    C = lin.in_features / 4.  The conditions of frozen_norm_applies, x contiguous with the image's shape, a valid layout
+    and the library's rule (frozen_gather_ok) -- DESIGN.md section 4.12."""
+    mode, images, height, width, window, shift = gather
+    if mode not in _lib.GATHER or not torch.is_tensor(x) or not x.is_contiguous():
+        return False
+    C = lin.in_features if mode == "window" else lin.in_features // 4
+    if x.dim() < 2 or x.shape[-1] != C or x.numel() != images * height * width * C or images <= 0:
+        return False
+    if mode == "window":
+        if not (window > 0 and height % window == 0 and width % window == 0 and 0 <= shift < window):
+            return False
+    elif not (window == 0 and shift == 0 and height % 2 == 0 and width % 2 == 0 and lin.in_features == 4 * C):
+        return False
+    return _norm_call_ok(norm, lin, x) and frozen_gather_ok(lin, mode)
+
+
+def frozen_gather_linear(norm, lin, x, gather):
+    """lin(norm(rows gathered from x)) in one launch, for a call where frozen_gather_applies(norm, lin, x, gather) holds:
+    lin's fused kernel reads each row from the image x, computes torch's exact LayerNorm of it and quantises it
+    (csrc/forward_tc.cu), bit-identical to torch's LayerNorm, roll and window partition (or cat) followed by lin.  Returns
+    the window rows [images * windows, window^2, out_features] or the merged rows [images, height * width / 4,
+    out_features]; only the output is allocated."""
+    return _frozen_call(lin, x, norm=norm, gather=gather)
 
 
 class PTQSLQuantLinear(MinMaxQuantLinear):

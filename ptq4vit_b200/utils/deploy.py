@@ -51,12 +51,19 @@ into attn.proj (in a Swin block also the window reverse and the reverse roll bef
 proj's output rows) and `x + mlp(...)` into mlp.fc2, fused MLP included.  The Linear's store adds the shortcut, so its
 FP32 output never reaches HBM and the torch add (reverse, roll) kernels are gone, bit-identical.  It composes with the
 other fusions.  A folded call skips proj's and fc2's forward hooks, so it is opt-in; `unfuse_residual(net)` undoes it.
+
+`fuse_gather(net)` folds the row gathers in front of Swin's LayerNorm folds: a Swin block's norm1, roll(-shift) and
+window partition into attn.qkv, and PatchMerging's cat of the 2x2 neighbourhoods (and its norm) into reduction.  The
+Linear's fused kernel reads each row from the block's input image, normalises it with torch's exact LayerNorm and
+quantises it, so the normalised, rolled, partitioned or concatenated copies never reach HBM, bit-identical.  It composes
+with the other fusions.  A folded call skips the LayerNorm's forward hooks, so it is opt-in; `unfuse_gather(net)` undoes
+it.
 None of the fusions is recorded by save_quantized: apply them again after load_quantized.
 """
 import torch
 
 from ..quant_layers.conv import MinMaxQuantConv2d
-from ..quant_layers.linear import MinMaxQuantLinear
+from ..quant_layers.linear import MinMaxQuantLinear, frozen_gather_ok
 from ..quant_layers.matmul import LONG_ATTENTION_TOKENS, SHORT_ATTENTION_TOKENS, MinMaxQuantMatMul
 from . import integer
 from .models import Attention, Block, Mlp, PatchMerging, SwinBlock, VisionTransformer, WindowAttention
@@ -201,6 +208,42 @@ def unfuse_residual(net):
     for m in net.modules():
         if isinstance(m, (Block, SwinBlock)):
             m.fold_residual = False
+
+
+def _gather_site(m):
+    """The (consuming Linear, gather mode) of a row-gather fold site, or None"""
+    if isinstance(m, SwinBlock):
+        return m.attn.qkv, "window"
+    if isinstance(m, PatchMerging):
+        return m.reduction, "merge"
+    return None
+
+
+def fuse_gather(net):
+    """Mark every row-gather fold site of `net` whose Linear is frozen and takes the gather (quant_layers.linear.
+    frozen_gather_ok): a SwinBlock's norm1 -> roll(-shift) -> window partition -> attn.qkv, and a PatchMerging's 2x2 cat
+    -> norm -> reduction.  Each call that qualifies (quant_layers.linear.frozen_gather_applies: the conditions of the
+    LayerNorm fold, a contiguous input of the image's shape) reads its rows from the block's input inside the Linear's
+    activation quantiser, with the bits of the unfolded sequence; any other call runs the modules and torch's ops as
+    before (PatchMerging's fold_norm path included).  A folded call skips the LayerNorm's forward hooks, which is why the
+    fold is opt-in.  It composes with fuse_attention, fuse_mlp, fuse_norm and fuse_residual; save_quantized /
+    load_quantized do not record it.  Returns the names of the sites left unfolded (a reduction on the streamed path, such
+    as Swin-T's last one, always is)."""
+    left = []
+    for name, m in net.named_modules():
+        site = _gather_site(m)
+        if site is not None:
+            lin, mode = site
+            m.fold_gather = isinstance(lin, MinMaxQuantLinear) and lin.frozen and frozen_gather_ok(lin, mode)
+            if not m.fold_gather:
+                left.append(name)
+    return left
+
+
+def unfuse_gather(net):
+    for m in net.modules():
+        if _gather_site(m) is not None:
+            m.fold_gather = False
 
 
 def _to(v, device):

@@ -5,8 +5,9 @@ available offline, so weights are synthetic (trunc-normal 0.02) -- this is harne
 import torch
 import torch.nn as nn
 
-from ..quant_layers.linear import (frozen_mlp, frozen_mlp_applies, frozen_mlp_norm_ok, frozen_norm_applies,
-                                   frozen_norm_linear, frozen_residual_applies, frozen_residual_linear)
+from ..quant_layers.linear import (frozen_gather_applies, frozen_gather_linear, frozen_mlp, frozen_mlp_applies,
+                                   frozen_mlp_norm_ok, frozen_norm_applies, frozen_norm_linear, frozen_residual_applies,
+                                   frozen_residual_linear)
 from ..quant_layers.matmul import frozen_attention, frozen_attention_applies
 
 
@@ -182,6 +183,20 @@ def _window_reverse(win, ws, H, W):
     return x.permute(0, 1, 3, 2, 4, 5).contiguous().view(B, H, W, -1)
 
 
+def _window_qkv(norm, qkv, x, layout):
+    """qkv(window_partition(roll(norm(x), (-shift, -shift)))) of a Swin block input x [images, height * width, C] with
+    layout = (images, height, width, window, shift): one folded call when frozen_gather_applies holds (the LayerNorm, the
+    roll and the partition in qkv's activation quantiser), else the modules and torch's ops as they are."""
+    images, H, W, ws, shift = layout
+    gather = ("window", images, H, W, ws, shift)
+    if frozen_gather_applies(norm, qkv, x, gather):
+        return frozen_gather_linear(norm, qkv, x, gather)
+    h = norm(x).view(images, H, W, -1)
+    if shift > 0:
+        h = torch.roll(h, shifts=(-shift, -shift), dims=(1, 2))
+    return qkv(_window_partition(h, ws))
+
+
 class WindowAttention(nn.Module):
     """reference: utils/models.py:28-56 (window_attention_forward) -- q is scaled BEFORE matmul1; relative position
     bias and the shifted-window mask are added outside the MatMul modules."""
@@ -206,12 +221,19 @@ class WindowAttention(nn.Module):
 
     fused = False      # set by utils.deploy.fuse_attention, as Attention.fused
 
-    def forward(self, x, mask=None, residual=None, layout=None):
+    def forward(self, x, mask=None, residual=None, layout=None, norm=None, gather=None):
         """residual, layout: (SwinBlock with fold_residual) return residual + the image of the output windows under
         layout = (images, height, width, window, shift) -- window reverse, then roll by (shift, shift) -- with the
-        reverse, roll and add folded into proj's store when it applies."""
-        B_, N, C = x.shape
-        y = self.qkv(x)
+        reverse, roll and add folded into proj's store when it applies.  norm, gather: (SwinBlock with fold_gather) x is
+        the block's input [images, height * width, C] and the windows are those of roll(norm(x), (-shift, -shift)) under
+        gather = (images, height, width, window, shift), with the LayerNorm, roll and partition folded into qkv when it
+        applies."""
+        if gather is None:
+            B_, N, C = x.shape
+            y = self.qkv(x)
+        else:
+            y = _window_qkv(norm, self.qkv, x, gather)
+            B_, N, C = y.shape[0], y.shape[1], x.shape[-1]
         if self.fused:
             bias = self.relative_position_bias_table[self.relative_position_index.view(-1)].view(N, N, -1).permute(2, 0, 1).contiguous()
             if frozen_attention_applies(self.matmul1, self.matmul2, N, C // self.num_heads, y, bias, mask):
@@ -267,16 +289,21 @@ class SwinBlock(nn.Module):
 
     fold_norm2 = False     # set by utils.deploy.fuse_norm, as Block.fold_norm2
     fold_residual = False  # set by utils.deploy.fuse_residual, as Block.fold_residual (proj's add with the window layout)
+    fold_gather = False    # set by utils.deploy.fuse_gather: hand x and norm1 to attn, which folds norm1, the roll and the
+                           # window partition into qkv when it applies
 
     def forward(self, x):
         if self.fold_residual:
             return self._forward_res(x)
         B, L, C = x.shape
         H = W = self.res
-        h = self.norm1(x).view(B, H, W, C)
-        if self.shift > 0:
-            h = torch.roll(h, shifts=(-self.shift, -self.shift), dims=(1, 2))
-        win = self.attn(_window_partition(h, self.ws), mask=self.attn_mask)
+        if self.fold_gather:
+            win = self.attn(x, mask=self.attn_mask, norm=self.norm1, gather=(B, H, W, self.ws, self.shift))
+        else:
+            h = self.norm1(x).view(B, H, W, C)
+            if self.shift > 0:
+                h = torch.roll(h, shifts=(-self.shift, -self.shift), dims=(1, 2))
+            win = self.attn(_window_partition(h, self.ws), mask=self.attn_mask)
         h = _window_reverse(win, self.ws, H, W)
         if self.shift > 0:
             h = torch.roll(h, shifts=(self.shift, self.shift), dims=(1, 2))
@@ -288,10 +315,14 @@ class SwinBlock(nn.Module):
     def _forward_res(self, x):
         B, L, C = x.shape
         H = W = self.res
-        h = self.norm1(x).view(B, H, W, C)
-        if self.shift > 0:
-            h = torch.roll(h, shifts=(-self.shift, -self.shift), dims=(1, 2))
-        x = self.attn(_window_partition(h, self.ws), mask=self.attn_mask, residual=x, layout=(B, H, W, self.ws, self.shift))
+        layout = (B, H, W, self.ws, self.shift)
+        if self.fold_gather:
+            x = self.attn(x, mask=self.attn_mask, residual=x, layout=layout, norm=self.norm1, gather=layout)
+        else:
+            h = self.norm1(x).view(B, H, W, C)
+            if self.shift > 0:
+                h = torch.roll(h, shifts=(-self.shift, -self.shift), dims=(1, 2))
+            x = self.attn(_window_partition(h, self.ws), mask=self.attn_mask, residual=x, layout=layout)
         return self.mlp(x, norm=self.norm2, residual=x) if self.fold_norm2 else self.mlp(self.norm2(x), residual=x)
 
 
@@ -303,9 +334,14 @@ class PatchMerging(nn.Module):
         self.reduction = nn.Linear(4 * dim, 2 * dim, bias=False)
 
     fold_norm = False      # set by utils.deploy.fuse_norm: fold norm into reduction when it applies
+    fold_gather = False    # set by utils.deploy.fuse_gather: fold the 2x2 cat and norm into reduction when it applies
 
     def forward(self, x):
         B, L, C = x.shape
+        if self.fold_gather:
+            gather = ("merge", B, self.res, self.res, 0, 0)
+            if frozen_gather_applies(self.norm, self.reduction, x, gather):
+                return frozen_gather_linear(self.norm, self.reduction, x, gather)
         x = x.view(B, self.res, self.res, C)
         x = torch.cat([x[:, 0::2, 0::2], x[:, 1::2, 0::2], x[:, 0::2, 1::2], x[:, 1::2, 1::2]], -1).view(B, -1, 4 * C)
         if self.fold_norm:
