@@ -393,6 +393,31 @@ P4V_API int p4v_conv_pack(const p4v_conv_frozen_desc* d, const float* weight, co
  * No allocation, no copy, no synchronisation: it can be captured in a CUDA graph. */
 P4V_API int p4v_conv_frozen_forward(const p4v_conv_frozen_desc* d, const float* x, const float* bias, const void* packed,
                                     size_t packed_bytes, float* out, void* stream);
+/* The patch embedding's token epilogue folded into the frozen convolution: the kernel stores the token rows the model's
+ * stem makes of the conv output, instead of the NCHW output torch then flattens, transposes and copies.  Each value is
+ * the one p4v_conv_frozen_forward computes, v = conv[b, o, p] (p = py * (width / kernel_w) + px), and the result is
+ * bit-identical to that call followed by torch's ops.  P = (height / kernel_h) * (width / kernel_w).
+ * p4v_conv_frozen_forward_pos (ViT / DeiT): out [images][1 + P][out_channels],
+ *   out[b][0][o] = fl(cls[o] + pos[0][o]),   out[b][1 + p][o] = fl(v + pos[1 + p][o])
+ * which replaces  torch.cat((cls_token.expand(B, -1, -1), conv.flatten(2).transpose(1, 2)), 1) + pos_embed;
+ * cls [out_channels] and pos [1 + P][out_channels] (cls_numel and pos_numel must be exactly that).
+ * p4v_conv_frozen_forward_norm (Swin): out [images][P][out_channels], each token row normalised with torch's exact
+ * LayerNorm (its vectorised kernel, the one the LayerNorm fold of p4v_linear_frozen_forward_norm reproduces), gamma and
+ * beta [out_channels] (norm_numel must be exactly that), eps finite and >= 0; replaces
+ * patch_norm(conv.flatten(2).transpose(1, 2)).
+ * p4v_conv_pos_ok / p4v_conv_norm_ok are their shape rules, pure functions of the module geometry: p4v_conv_frozen_ok
+ * and out_channels % 4 == 0; the LayerNorm also out_channels <= 128 (the whole token row in one CTA of the kernel).
+ * Every argument is validated before the one launch: null pointers, the rule, geometry, packed_bytes, alignment (out,
+ * cls, pos, gamma and beta 16 bytes; the rest as p4v_conv_frozen_forward), the element counts above and out not
+ * overlapping any input.  No workspace, no allocation, no copy: each can be captured in a CUDA graph. */
+P4V_API int p4v_conv_pos_ok(const p4v_conv_frozen_desc* d, int* ok);
+P4V_API int p4v_conv_norm_ok(const p4v_conv_frozen_desc* d, int* ok);
+P4V_API int p4v_conv_frozen_forward_pos(const p4v_conv_frozen_desc* d, const float* x, const float* bias, const void* packed,
+                                        size_t packed_bytes, const float* cls, size_t cls_numel, const float* pos,
+                                        size_t pos_numel, float* out, void* stream);
+P4V_API int p4v_conv_frozen_forward_norm(const p4v_conv_frozen_desc* d, const float* x, const float* bias, const void* packed,
+                                         size_t packed_bytes, const float* gamma, const float* beta, size_t norm_numel,
+                                         float eps, float* out, void* stream);
 
 /* Integer export of a calibrated module (utils/integer.py:8-129): src [rows, cols] fp32 -> dst one byte per element.
  * mode 0: int8 = clamp(rne(x / delta), -q, q-1) (quantize_int_weight :8-18, quantize_matmul_input :27-42, plain

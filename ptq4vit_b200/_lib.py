@@ -110,6 +110,10 @@ _SIGNATURES = {
     "p4v_conv_pack_bytes": [C.POINTER(ConvFrozenDesc), C.POINTER(C.c_size_t)],
     "p4v_conv_pack": [C.POINTER(ConvFrozenDesc), _P, _P, _P, C.c_size_t, _P],
     "p4v_conv_frozen_forward": [C.POINTER(ConvFrozenDesc), _P, _P, _P, C.c_size_t, _P, _P],
+    "p4v_conv_pos_ok": [C.POINTER(ConvFrozenDesc), C.POINTER(C.c_int)],
+    "p4v_conv_norm_ok": [C.POINTER(ConvFrozenDesc), C.POINTER(C.c_int)],
+    "p4v_conv_frozen_forward_pos": [C.POINTER(ConvFrozenDesc), _P, _P, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, _P, _P],
+    "p4v_conv_frozen_forward_norm": [C.POINTER(ConvFrozenDesc), _P, _P, _P, C.c_size_t, _P, _P, C.c_size_t, C.c_float, _P, _P],
     "p4v_export_quantized": [_P, C.c_longlong, C.c_longlong, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                              _P, _P, _P],
 }

@@ -242,30 +242,126 @@ extern "C" int p4v_conv_pack(const p4v_conv_frozen_desc* d, const float* weight,
                               reinterpret_cast<float*>(base), base + f.delta_bytes, (cudaStream_t)stream);
 }
 
-extern "C" int p4v_conv_frozen_forward(const p4v_conv_frozen_desc* d, const float* x, const float* bias, const void* packed,
-                                       size_t packed_bytes, float* out, void* stream) {
-  ConvFrozen f; int rc = build_conv_frozen(d, f, "conv_frozen_forward");
+namespace {
+
+// Validates the arguments every frozen forward shares (in p4v_conv_frozen_forward's order, with fn's name in the
+// messages) and fills the kernel's parameters
+int conv_forward_params(const char* fn, const p4v_conv_frozen_desc* d, const float* x, const float* bias, const void* packed,
+                        size_t packed_bytes, float* out, FwdConvParams& p) {
+  ConvFrozen f; int rc = build_conv_frozen(d, f, fn);
   if (rc) return rc;
-  P4V_REQUIRE(x && packed && out, "conv_frozen_forward: null pointer");
-  P4V_REQUIRE(!d->has_bias || bias, "conv_frozen_forward: has_bias set but bias is null");
+  P4V_REQUIRE(x && packed && out, "%s: null pointer", fn);
+  P4V_REQUIRE(!d->has_bias || bias, "%s: has_bias set but bias is null", fn);
   P4V_REQUIRE(d->images >= 1 && d->height >= d->kernel_h && d->width >= d->kernel_w,
-              "conv_frozen_forward: bad geometry (images %d, input %dx%d, kernel %dx%d): need at least one image and one "
-              "output position", d->images, d->height, d->width, d->kernel_h, d->kernel_w);
+              "%s: bad geometry (images %d, input %dx%d, kernel %dx%d): need at least one image and one "
+              "output position", fn, d->images, d->height, d->width, d->kernel_h, d->kernel_w);
   const long long chw = (long long)d->in_channels * d->height * d->width;
   const int Ph = d->height / d->kernel_h, Pw = d->width / d->kernel_w;
   const long long M = (long long)d->images * Ph * Pw;
   P4V_REQUIRE(chw <= INT_MAX && M <= INT_MAX - P4V_TILE && (long long)p4v_cdiv((int)M, P4V_TILE) * f.tiles_n <= INT_MAX,
-              "conv_frozen_forward: input too large (in_channels*height*width %lld, positions %lld)", chw, M);
-  P4V_REQUIRE(packed_bytes >= f.total, "conv_frozen_forward: packed buffer too small (%zu < %zu)", packed_bytes, f.total);
+              "%s: input too large (in_channels*height*width %lld, positions %lld)", fn, chw, M);
+  P4V_REQUIRE(packed_bytes >= f.total, "%s: packed buffer too small (%zu < %zu)", fn, packed_bytes, f.total);
   P4V_REQUIRE((reinterpret_cast<uintptr_t>(packed) & 15) == 0 && (reinterpret_cast<uintptr_t>(x) & 3) == 0 &&
               (reinterpret_cast<uintptr_t>(out) & 3) == 0 && (reinterpret_cast<uintptr_t>(bias) & 3) == 0,
-              "conv_frozen_forward: packed must be 16-byte, x, bias and out 4-byte aligned");
-  FwdConvParams p{};
+              "%s: packed must be 16-byte, x, bias and out 4-byte aligned", fn);
+  p = FwdConvParams{};
   p.x = x; p.bias = d->has_bias ? bias : nullptr; p.out = out;
   p.delta = static_cast<const float*>(packed);
   p.Wq = static_cast<const uint8_t*>(packed) + f.delta_bytes;
   p.B = d->images; p.C = d->in_channels; p.H = d->height; p.W = d->width; p.O = f.O; p.kh = d->kernel_h; p.kw = d->kernel_w;
   p.Ph = Ph; p.Pw = Pw; p.K = f.K; p.M = (int)M;
   p.tiles_m = p4v_cdiv(p.M, P4V_TILE); p.tiles_n = f.tiles_n; p.n_slabs = f.n_slabs;
+  return 0;
+}
+
+// The token epilogues' rule beyond the shape rule: nullptr when d qualifies, else the reason (norm: the LayerNorm's)
+const char* conv_stem_reason(const p4v_conv_frozen_desc* d, bool norm) {
+  if (const char* why = conv_frozen_reason(d)) return why;
+  if (d->out_channels % 4 != 0) return "out_channels must be a multiple of 4 (a lane stores 4 channels of a token row)";
+  if (norm && d->out_channels > P4V_TILE) return "out_channels above " P4V_STR(P4V_TILE) " (the LayerNorm needs the whole token row in one CTA)";
+  return nullptr;
+}
+
+bool apart(const void* a, size_t abytes, const void* b, size_t bbytes) {
+  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return !a || !b || x + abytes <= y || y + bbytes <= x;
+}
+
+// The arguments of a token-major call (fn, rule `norm`) beyond conv_forward_params: the rule, out 16-byte aligned and
+// apart from x, bias and packed; `tokens` token rows of out_channels per image
+int check_tokens(const char* fn, const p4v_conv_frozen_desc* d, bool norm, const FwdConvParams& p, const void* packed,
+                 size_t packed_bytes, const float* out, long long tokens) {
+  const char* why = conv_stem_reason(d, norm);
+  P4V_REQUIRE(why == nullptr, "%s: %s (%s)", fn, why, norm ? "p4v_conv_norm_ok" : "p4v_conv_pos_ok");
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "%s: out must be 16-byte aligned", fn);
+  const size_t ob = (size_t)p.B * tokens * p.O * 4;
+  P4V_REQUIRE(apart(out, ob, p.x, (size_t)p.B * p.C * p.H * p.W * 4) && apart(out, ob, p.bias, (size_t)p.O * 4) &&
+              apart(out, ob, packed, packed_bytes), "%s: out overlaps x, bias or packed", fn);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int p4v_conv_frozen_forward(const p4v_conv_frozen_desc* d, const float* x, const float* bias, const void* packed,
+                                       size_t packed_bytes, float* out, void* stream) {
+  FwdConvParams p;
+  if (int rc = conv_forward_params("conv_frozen_forward", d, x, bias, packed, packed_bytes, out, p)) return rc;
+  return p4v_launch_forward_conv_tc(p, (cudaStream_t)stream);
+}
+
+extern "C" int p4v_conv_pos_ok(const p4v_conv_frozen_desc* d, int* ok) {
+  P4V_REQUIRE(d && ok, "conv_pos_ok: null pointer");
+  *ok = conv_stem_reason(d, false) == nullptr;
+  return 0;
+}
+
+extern "C" int p4v_conv_norm_ok(const p4v_conv_frozen_desc* d, int* ok) {
+  P4V_REQUIRE(d && ok, "conv_norm_ok: null pointer");
+  *ok = conv_stem_reason(d, true) == nullptr;
+  return 0;
+}
+
+// Replaces, with the conv frozen, VisionTransformer.forward's stem (reference: timm's VisionTransformer.forward_features,
+// as utils/models.py:164 restates it):
+//   x = patch_embed(x)                                  (proj(x).flatten(2).transpose(1, 2))
+//   x = torch.cat((cls_token.expand(B, -1, -1), x), dim=1) + pos_embed
+extern "C" int p4v_conv_frozen_forward_pos(const p4v_conv_frozen_desc* d, const float* x, const float* bias, const void* packed,
+                                           size_t packed_bytes, const float* cls, size_t cls_numel, const float* pos,
+                                           size_t pos_numel, float* out, void* stream) {
+  const char* fn = "conv_frozen_forward_pos";
+  FwdConvPosParams p;
+  if (int rc = conv_forward_params(fn, d, x, bias, packed, packed_bytes, out, p)) return rc;
+  P4V_REQUIRE(cls && pos, "%s: null pointer", fn);
+  const long long tokens = 1 + (long long)p.Ph * p.Pw;
+  P4V_REQUIRE(cls_numel == (size_t)p.O, "%s: cls has %zu elements, out_channels is %d", fn, cls_numel, p.O);
+  P4V_REQUIRE(pos_numel == (size_t)(tokens * p.O), "%s: pos_embed has %zu elements, (1 + positions) * out_channels is %lld", fn,
+              pos_numel, tokens * p.O);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(cls) & 15) == 0 && (reinterpret_cast<uintptr_t>(pos) & 15) == 0,
+              "%s: cls and pos_embed must be 16-byte aligned", fn);
+  if (int rc = check_tokens(fn, d, false, p, packed, packed_bytes, out, tokens)) return rc;
+  const size_t ob = (size_t)p.B * tokens * p.O * 4;
+  P4V_REQUIRE(apart(out, ob, cls, cls_numel * 4) && apart(out, ob, pos, pos_numel * 4), "%s: out overlaps cls or pos_embed", fn);
+  p.cls = cls; p.pos = pos;
+  return p4v_launch_forward_conv_tc(p, (cudaStream_t)stream);
+}
+
+// Replaces, with the conv frozen, SwinTransformer.forward's stem (reference: timm's SwinTransformer.forward_features, as
+// utils/models.py:390 restates it):  x = patch_norm(patch_embed(x))
+extern "C" int p4v_conv_frozen_forward_norm(const p4v_conv_frozen_desc* d, const float* x, const float* bias, const void* packed,
+                                            size_t packed_bytes, const float* gamma, const float* beta, size_t norm_numel,
+                                            float eps, float* out, void* stream) {
+  const char* fn = "conv_frozen_forward_norm";
+  FwdConvNormParams p;
+  if (int rc = conv_forward_params(fn, d, x, bias, packed, packed_bytes, out, p)) return rc;
+  P4V_REQUIRE(gamma && beta, "%s: null pointer", fn);
+  P4V_REQUIRE(norm_numel == (size_t)p.O, "%s: the LayerNorm has %zu features, out_channels is %d", fn, norm_numel, p.O);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(gamma) & 15) == 0 && (reinterpret_cast<uintptr_t>(beta) & 15) == 0,
+              "%s: gamma and beta must be 16-byte aligned", fn);
+  P4V_REQUIRE(eps >= 0.f && eps <= 3.4028234663852886e38f, "%s: eps must be finite and non-negative (got %g)", fn, (double)eps);
+  const long long tokens = (long long)p.Ph * p.Pw;
+  if (int rc = check_tokens(fn, d, true, p, packed, packed_bytes, out, tokens)) return rc;
+  const size_t ob = (size_t)p.B * tokens * p.O * 4;
+  P4V_REQUIRE(apart(out, ob, gamma, norm_numel * 4) && apart(out, ob, beta, norm_numel * 4), "%s: out overlaps gamma or beta", fn);
+  p.ln = FwdNorm{gamma, beta, eps};
   return p4v_launch_forward_conv_tc(p, (cudaStream_t)stream);
 }

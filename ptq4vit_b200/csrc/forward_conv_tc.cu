@@ -14,7 +14,10 @@
 //      term, terms high, middle, low) runs on the other one; the slab's 8 KB of the packed weight image is copied beside
 //      it with 16-byte loads; fence.proxy.async, then one block barrier hands the stage to the async proxy;
 //   2. epilogue: the fp32 accumulators go through shared memory as [channel][position], so that each warp stores runs of
-//      consecutive positions of one channel (the NCHW output is contiguous along the positions).
+//      consecutive positions of one channel (the NCHW output is contiguous along the positions).  The token-major
+//      epilogues (FwdConvPosParams, FwdConvNormParams; DESIGN §4.13) stage them as [position][channel] instead: a warp
+//      takes one position at a time and its lanes store a float4 of 4 consecutive channels each, a run of the token row,
+//      with pos_embed added (ViT) or the row normalised with torch's LayerNorm (Swin, the whole row in this CTA).
 // Gather: a thread owns one position (lanes along consecutive positions) and one 8-element K chunk per unit.  A position's
 // pixels of element k sit at pos_base + koff[k] (koff: c*H*W + i*W + j, a per-CTA table in shared memory), so the
 // thread's 8 values are two float4 loads when kw and W are multiples of 4 and x is 16-byte aligned (one kernel row holds
@@ -37,18 +40,88 @@ constexpr int kMainBytes = (2 * kStage > kOutBytes ? 2 * kStage : kOutBytes);
 constexpr int kUnits = P4V_TILE * kChunks / kThreads;   // (position, chunk) units per thread and slab
 static_assert(kUnits * kThreads == P4V_TILE * kChunks, "units must cover the slab");
 static_assert(kPlane % (16 * kThreads) == 0, "the weight slab is copied in whole 16-byte rounds");
+// token-major staging: row = position, 8 mod 32 words, so that a half-warp's float2 stores (4 rows x 8 columns) and a
+// warp's float4 reads of one row hit distinct banks
+constexpr int kLdTok = P4V_TILE + 8;
+constexpr int kTokBytes = P4V_TILE * kLdTok * 4;
 
-__host__ __device__ constexpr int smem_bytes(int K) { return kMainBytes + ((K * 4 + 127) & ~127) + 128; }
+template <class Par> constexpr bool kIsNchw = std::is_same<Par, FwdConvParams>::value;
+template <class Par> __host__ __device__ constexpr int main_bytes() {
+  return kIsNchw<Par> ? kMainBytes : (2 * kStage > kTokBytes ? 2 * kStage : kTokBytes);
+}
+template <class Par> __host__ __device__ constexpr int smem_bytes(int K) { return main_bytes<Par>() + ((K * 4 + 127) & ~127) + 128; }
 
 __device__ __forceinline__ uint32_t bf16_pair(float a, float b) {
   return (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(a)) | ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(b)) << 16);
 }
 
+// The token-major epilogue (DESIGN §4.13): stage the tile as [position][channel] (the stages are free), then each warp
+// takes positions warp, warp + 8, ... and its lane l the channels o0 + 4l .. + 3 of the position's token row.  The value
+// is the NCHW epilogue's, fmaf(delta[o], S, bias[o]) (delta[o] * S without a bias); ViT adds pos_embed's row and writes
+// the image's cls row along with its position 0, Swin normalises the row with torch's exact LayerNorm (the §4.10 fold's
+// p4v_ln_row_stats_at over the staged row and p4v_ln_apply).  O % 4 == 0: a lane's four channels are all in or all out.
+template <class Par>
+__device__ __forceinline__ void token_epilogue(const Par& P, float* stg, const float (&acc)[64], int r0, int tm, int tn,
+                                               int warp, int lane) {
+#pragma unroll
+  for (int v = 0; v < 64; v += 2) {
+    const int row = r0 + 8 * ((v >> 1) & 1), col = 8 * (v >> 2) + 2 * (lane & 3);
+    *reinterpret_cast<float2*>(stg + row * kLdTok + col) = make_float2(acc[v], acc[v + 1]);
+  }
+  __syncthreads();
+  const int L = P.Ph * P.Pw;
+  const int o = tn * P4V_TILE + 4 * lane;
+  const bool col_in = o < P.O;
+  float4 d = make_float4(0.f, 0.f, 0.f, 0.f), bo = d, ga = d, be = d, head = d;
+  if (col_in) {
+    d = __ldg(reinterpret_cast<const float4*>(P.delta + o));
+    if (P.bias) bo = make_float4(__ldg(P.bias + o), __ldg(P.bias + o + 1), __ldg(P.bias + o + 2), __ldg(P.bias + o + 3));
+    if constexpr (kIsConvNorm<Par>) {
+      ga = __ldg(reinterpret_cast<const float4*>(P.ln.gamma + o));
+      be = __ldg(reinterpret_cast<const float4*>(P.ln.beta + o));
+    } else {   // the cls row: fl(cls + pos_embed[0])
+      const float4 c = __ldg(reinterpret_cast<const float4*>(P.cls + o)), p0 = __ldg(reinterpret_cast<const float4*>(P.pos + o));
+      head = make_float4(__fadd_rn(c.x, p0.x), __fadd_rn(c.y, p0.y), __fadd_rn(c.z, p0.z), __fadd_rn(c.w, p0.w));
+    }
+  }
+  auto conv_out = [&](float dd, float a, float b) { return P.bias ? fmaf(dd, a, b) : __fmul_rn(dd, a); };
+#pragma unroll 1
+  for (int r = warp; r < P4V_TILE; r += kThreads / 32) {
+    const int g = tm * P4V_TILE + r;
+    if (g >= P.M) break;                       // warp-uniform: the LayerNorm's shuffles see the whole warp
+    const int b = g / L, l = g - b * L;
+    float* row = stg + r * kLdTok;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (col_in) {
+      const float4 a = *reinterpret_cast<const float4*>(row + 4 * lane);
+      v = make_float4(conv_out(d.x, a.x, bo.x), conv_out(d.y, a.y, bo.y), conv_out(d.z, a.z, bo.z), conv_out(d.w, a.w, bo.w));
+    }
+    if constexpr (kIsConvNorm<Par>) {
+      if (col_in) *reinterpret_cast<float4*>(row + 4 * lane) = v;
+      __syncwarp();
+      const float4* row4 = reinterpret_cast<const float4*>(row);
+      float mean, rstd;
+      p4v_ln_row_stats_at([row4](int i) { return row4[i]; }, P.O, P.ln.eps, lane, mean, rstd);
+      if (col_in)
+        *reinterpret_cast<float4*>(P.out + (long long)g * P.O + o) =
+            make_float4(p4v_ln_apply(v.x, mean, rstd, ga.x, be.x), p4v_ln_apply(v.y, mean, rstd, ga.y, be.y),
+                        p4v_ln_apply(v.z, mean, rstd, ga.z, be.z), p4v_ln_apply(v.w, mean, rstd, ga.w, be.w));
+    } else if (col_in) {
+      const long long t = (long long)g + b + 1;   // token row: the image's cls row, then its positions
+      const float4 pe = __ldg(reinterpret_cast<const float4*>(P.pos + (long long)(l + 1) * P.O + o));
+      *reinterpret_cast<float4*>(P.out + t * P.O + o) =
+          make_float4(__fadd_rn(v.x, pe.x), __fadd_rn(v.y, pe.y), __fadd_rn(v.z, pe.z), __fadd_rn(v.w, pe.w));
+      if (l == 0) *reinterpret_cast<float4*>(P.out + (t - 1) * P.O + o) = head;
+    }
+  }
+}
+
 // Two CTAs per SM: 128 registers, 2 x ~70-84 KB of shared memory.
-__global__ void __launch_bounds__(kThreads, 2) forward_conv_kernel(const __grid_constant__ FwdConvParams P) {
+template <class Par>
+__global__ void __launch_bounds__(kThreads, 2) forward_conv_kernel(const __grid_constant__ Par P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
-  int* koff = reinterpret_cast<int*>(smem + kMainBytes);
+  int* koff = reinterpret_cast<int*>(smem + main_bytes<Par>());
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const int tn = blockIdx.x % P.tiles_n, tm = blockIdx.x / P.tiles_n;
   const int L = P.Ph * P.Pw;
@@ -147,34 +220,38 @@ __global__ void __launch_bounds__(kThreads, 2) forward_conv_kernel(const __grid_
     __syncthreads();                           // slab s + 1 visible; every warpgroup is done with stage s & 1
   }
 
-  // ---- epilogue: stage [channel][position] (the stages are free), then runs of positions per channel ----
   float* stg = reinterpret_cast<float*>(smem);
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  if constexpr (!kIsNchw<Par>) {
+    token_epilogue(P, stg, acc, r0, tm, tn, warp, lane);
+  } else {
+    // ---- epilogue: stage [channel][position] (the stages are free), then runs of positions per channel ----
 #pragma unroll
-  for (int v = 0; v < 64; ++v) {
-    const int row = r0 + 8 * ((v >> 1) & 1), col = 8 * (v >> 2) + 2 * (lane & 3) + (v & 1);
-    stg[col * kLdOut + row] = acc[v];
-  }
-  __syncthreads();
-  long long obase[P4V_TILE / 32];              // out offset of position lane + 32 i without the channel term, -1 outside
-#pragma unroll
-  for (int i = 0; i < P4V_TILE / 32; ++i) {
-    const int g = tm * P4V_TILE + lane + 32 * i;
-    obase[i] = -1;
-    if (g < P.M) { const int b = g / L; obase[i] = (long long)b * P.O * L + (g - b * L); }
-  }
-  const int o0 = tn * P4V_TILE;
-#pragma unroll 1
-  for (int c = warp; c < P4V_TILE; c += kThreads / 32) {
-    const int o = o0 + c;
-    if (o >= P.O) break;
-    const float d = __ldg(P.delta + o);
-    const float bo = P.bias ? __ldg(P.bias + o) : 0.f;
+    for (int v = 0; v < 64; ++v) {
+      const int row = r0 + 8 * ((v >> 1) & 1), col = 8 * (v >> 2) + 2 * (lane & 3) + (v & 1);
+      stg[col * kLdOut + row] = acc[v];
+    }
+    __syncthreads();
+    long long obase[P4V_TILE / 32];              // out offset of position lane + 32 i without the channel term, -1 outside
 #pragma unroll
     for (int i = 0; i < P4V_TILE / 32; ++i) {
-      if (obase[i] < 0) continue;
-      const float a = stg[c * kLdOut + lane + 32 * i];
-      P.out[obase[i] + (long long)o * L] = P.bias ? fmaf(d, a, bo) : __fmul_rn(d, a);
+      const int g = tm * P4V_TILE + lane + 32 * i;
+      obase[i] = -1;
+      if (g < P.M) { const int b = g / L; obase[i] = (long long)b * P.O * L + (g - b * L); }
+    }
+    const int o0 = tn * P4V_TILE;
+#pragma unroll 1
+    for (int c = warp; c < P4V_TILE; c += kThreads / 32) {
+      const int o = o0 + c;
+      if (o >= P.O) break;
+      const float d = __ldg(P.delta + o);
+      const float bo = P.bias ? __ldg(P.bias + o) : 0.f;
+#pragma unroll
+      for (int i = 0; i < P4V_TILE / 32; ++i) {
+        if (obase[i] < 0) continue;
+        const float a = stg[c * kLdOut + lane + 32 * i];
+        P.out[obase[i] + (long long)o * L] = P.bias ? fmaf(d, a, bo) : __fmul_rn(d, a);
+      }
     }
   }
 }
@@ -211,14 +288,17 @@ __global__ void conv_pack_kernel(const float* __restrict__ w, const float* __res
 
 }  // namespace
 
-int p4v_launch_forward_conv_tc(const FwdConvParams& p, cudaStream_t st) {
-  const int smem = smem_bytes(p.K);
-  P4V_CUDA_OK(cudaFuncSetAttribute(forward_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  forward_conv_kernel<<<(unsigned)(p.tiles_m * p.tiles_n), kThreads, smem, st>>>(p);
+template <class Par> int p4v_launch_forward_conv_tc(const Par& p, cudaStream_t st) {
+  const int smem = smem_bytes<Par>(p.K);
+  P4V_CUDA_OK(cudaFuncSetAttribute(forward_conv_kernel<Par>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  forward_conv_kernel<Par><<<(unsigned)(p.tiles_m * p.tiles_n), kThreads, smem, st>>>(p);
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   return 0;
 }
+template int p4v_launch_forward_conv_tc<FwdConvParams>(const FwdConvParams&, cudaStream_t);
+template int p4v_launch_forward_conv_tc<FwdConvPosParams>(const FwdConvPosParams&, cudaStream_t);
+template int p4v_launch_forward_conv_tc<FwdConvNormParams>(const FwdConvNormParams&, cudaStream_t);
 
 int p4v_launch_conv_pack(const float* weight, const float* w_interval, int layerwise, int O, int K, int w_bit, int tiles_n,
                          int n_slabs, float* delta, uint8_t* Wq, cudaStream_t st) {

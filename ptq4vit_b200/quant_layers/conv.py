@@ -15,6 +15,9 @@ quant_forward call that wants no gradient runs one kernel that gathers the patch
 pixels exactly into three bf16 terms and multiplies them with the integers on the tensor cores
 (csrc/forward_conv_tc.cu).  It reads no FP32 weight and does not depend on torch's TF32 setting.  Not bit-identical to
 cuDNN's F.conv2d: the contract is a bound against fp64 (DESIGN.md section 4.9).
+
+frozen_stem folds the model's stem after the patch embedding into that kernel's store (DESIGN.md section 4.13): ViT's cls
+token and pos_embed, Swin's patch_norm.  It returns the bits of the frozen conv followed by torch's ops.
 """
 import ctypes
 
@@ -24,6 +27,7 @@ import torch.nn.functional as F
 
 from .. import _lib
 from ._metric import check_metric, metric_weight
+from .linear import _layer_norm_ok
 
 
 class MinMaxQuantConv2d(nn.Conv2d):
@@ -157,11 +161,14 @@ class MinMaxQuantConv2d(nn.Conv2d):
     def frozen(self):
         return self._packed is not None
 
-    def _frozen_forward(self, x):
+    def _check_frozen_interval(self):
         w0, v0 = self._frozen_interval
         if self.w_interval is not w0 or getattr(self.w_interval, "_version", None) != v0:
             raise RuntimeError(f"{self}: the step sizes changed after freeze(); call unfreeze() (and freeze() again) "
                                "before running the layer")
+
+    def _frozen_forward(self, x):
+        self._check_frozen_interval()
         dev = self._packed.device
         x4 = x.to(dev).contiguous().float()
         if x4.dim() != 4 or x4.shape[1] != self.in_channels:
@@ -189,6 +196,77 @@ class MinMaxQuantConv2d(nn.Conv2d):
         self.a_interval = (x.abs().max() / (self.a_qmax - 0.5)).detach()
         self.calibrated = True
         return self.quant_forward(x)
+
+
+def frozen_stem_ok(conv, norm):
+    """The library's shape rule of the stem fold for a conv module: p4v_conv_pos_ok (norm False: ViT's cls token and
+    pos_embed) or p4v_conv_norm_ok (norm True: Swin's patch_norm, out_channels <= 128).  Both need out_channels % 4 == 0."""
+    ok = ctypes.c_int()
+    fn = "p4v_conv_norm_ok" if norm else "p4v_conv_pos_ok"
+    _lib.check(getattr(_lib.lib(), fn)(ctypes.byref(conv._frozen_desc()), ctypes.byref(ok)), fn)
+    return bool(ok.value)
+
+
+def frozen_stem_applies(conv, x, cls_token=None, pos_embed=None, norm=None):
+    """Whether a model's stem can run as one folded call (frozen_stem): with cls_token and pos_embed (ViT / DeiT)
+    torch.cat((cls_token.expand(B, -1, -1), conv(x).flatten(2).transpose(1, 2)), 1) + pos_embed, with norm (Swin)
+    norm(conv(x).flatten(2).transpose(1, 2)).  conv a frozen conv module in quant_forward mode; x an FP32, contiguous
+    [images, in_channels, height, width] image on its device; cls_token [1, 1, C] and pos_embed [1, 1 + positions, C] FP32,
+    contiguous and 16-byte aligned there (C = out_channels); norm with the conditions of the LayerNorm folds (an affine
+    nn.LayerNorm over C, torch's vectorised case); under grad mode nothing that requires grad; and the library's rule
+    (frozen_stem_ok)."""
+    if (norm is None) == (cls_token is None) or (cls_token is None) != (pos_embed is None):
+        return False
+    if not (isinstance(conv, MinMaxQuantConv2d) and conv.frozen and conv.mode == "quant_forward"):
+        return False
+    dev = conv._packed.device
+    if not torch.is_tensor(x) or x.dtype != torch.float32 or x.device != dev or not x.is_contiguous() or x.dim() != 4:
+        return False
+    (kh, kw), C = conv.kernel_size, conv.out_channels
+    if x.shape[0] < 1 or x.shape[1] != conv.in_channels or x.shape[2] < kh or x.shape[3] < kw:
+        return False
+    params = list(conv.parameters())
+    if norm is None:
+        shapes = ((1, 1, C), (1, 1 + (x.shape[2] // kh) * (x.shape[3] // kw), C))
+        for t, shape in zip((cls_token, pos_embed), shapes):
+            if not torch.is_tensor(t) or t.dtype != torch.float32 or t.device != dev or not t.is_contiguous() or \
+                    t.data_ptr() % 16 or tuple(t.shape) != shape:
+                return False
+        params += [cls_token, pos_embed]
+    else:
+        if not _layer_norm_ok(norm, C, dev):
+            return False
+        params += list(norm.parameters())
+    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params)):
+        return False
+    return frozen_stem_ok(conv, norm is not None)
+
+
+def frozen_stem(conv, x, cls_token=None, pos_embed=None, norm=None):
+    """The model's stem in one launch, for a call where frozen_stem_applies holds: the frozen conv's kernel stores the
+    token rows instead of its NCHW output (csrc/forward_conv_tc.cu) -- with cls_token and pos_embed the [images,
+    1 + positions, C] rows of ViT's cat and pos_embed add, with norm the [images, positions, C] rows normalised with
+    torch's exact LayerNorm -- bit-identical to the frozen conv followed by torch's ops.  Only the output is allocated."""
+    conv._check_frozen_interval()
+    dev = conv._packed.device
+    d = conv._frozen_desc(x)
+    P, C = (d.height // d.kernel_h) * (d.width // d.kernel_w), conv.out_channels
+    b = None if conv.bias is None else conv.bias.detach().contiguous().float()
+    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    lib = _lib.lib()
+    if norm is None:
+        out = torch.empty(d.images, 1 + P, C, dtype=torch.float32, device=dev)
+        _lib.check(lib.p4v_conv_frozen_forward_pos(ctypes.byref(d), _lib.ptr(x), _lib.ptr(b), _lib.ptr(conv._packed),
+                                                   conv._packed.numel(), _lib.ptr(cls_token), cls_token.numel(),
+                                                   _lib.ptr(pos_embed), pos_embed.numel(), _lib.ptr(out), stream),
+                   "p4v_conv_frozen_forward_pos")
+    else:
+        out = torch.empty(d.images, P, C, dtype=torch.float32, device=dev)
+        _lib.check(lib.p4v_conv_frozen_forward_norm(ctypes.byref(d), _lib.ptr(x), _lib.ptr(b), _lib.ptr(conv._packed),
+                                                    conv._packed.numel(), _lib.ptr(norm.weight), _lib.ptr(norm.bias), C,
+                                                    float(norm.eps), _lib.ptr(out), stream),
+                   "p4v_conv_frozen_forward_norm")
+    return out
 
 
 class PTQSLQuantConv2d(MinMaxQuantConv2d):

@@ -376,18 +376,25 @@ def frozen_norm_applies(norm, lin, x):
     return _norm_call_ok(norm, lin, x) and _rule("p4v_linear_norm_ok", lin)
 
 
-def _norm_call_ok(norm, lin, x):
-    """frozen_norm_applies without the library's shape rule"""
+def _layer_norm_ok(norm, features, dev):
+    """The LayerNorm conditions of every fold that reproduces it: exactly an nn.LayerNorm with weight and bias over
+    `features` (a multiple of 4), both FP32, contiguous and 16-byte aligned on dev -- torch's vectorised case"""
     if type(norm) is not nn.LayerNorm or norm.weight is None or norm.bias is None:
         return False
+    if tuple(norm.normalized_shape) != (features,) or features % 4 != 0:
+        return False
+    return not any(p.dtype != torch.float32 or p.device != dev or not p.is_contiguous() or p.data_ptr() % 16
+                   for p in (norm.weight, norm.bias))
+
+
+def _norm_call_ok(norm, lin, x):
+    """frozen_norm_applies without the library's shape rule"""
     if not (isinstance(lin, MinMaxQuantLinear) and lin.frozen and lin.mode == "quant_forward"):
         return False
-    if tuple(norm.normalized_shape) != (lin.in_features,) or lin.in_features % 4 != 0:
-        return False
     dev = lin._packed.device
-    if x.dtype != torch.float32 or x.device != dev or x.numel() == 0:
+    if not _layer_norm_ok(norm, lin.in_features, dev):
         return False
-    if any(p.dtype != torch.float32 or p.device != dev or not p.is_contiguous() or p.data_ptr() % 16 for p in (norm.weight, norm.bias)):
+    if x.dtype != torch.float32 or x.device != dev or x.numel() == 0:
         return False
     if x.is_contiguous() and x.data_ptr() % 16:       # torch normalises a non-contiguous x from an aligned copy
         return False

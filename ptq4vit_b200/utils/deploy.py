@@ -58,15 +58,20 @@ Linear's fused kernel reads each row from the block's input image, normalises it
 quantises it, so the normalised, rolled, partitioned or concatenated copies never reach HBM, bit-identical.  It composes
 with the other fusions.  A folded call skips the LayerNorm's forward hooks, so it is opt-in; `unfuse_gather(net)` undoes
 it.
+`fuse_stem(net)` folds the model's stem after a frozen patch-embedding conv into the conv kernel's store: ViT / DeiT's
+flatten, transpose, cat with the cls token and pos_embed add, Swin's flatten, transpose and patch_norm.  The kernel
+stores the token rows the first block reads, bit-identical to the frozen conv followed by torch's ops, so the NCHW output
+and its copies never reach HBM.  It composes with the other fusions.  A folded call skips the conv's and patch_norm's
+forward hooks, so it is opt-in; `unfuse_stem(net)` undoes it.
 None of the fusions is recorded by save_quantized: apply them again after load_quantized.
 """
 import torch
 
-from ..quant_layers.conv import MinMaxQuantConv2d
+from ..quant_layers.conv import MinMaxQuantConv2d, frozen_stem_ok
 from ..quant_layers.linear import MinMaxQuantLinear, frozen_gather_ok
 from ..quant_layers.matmul import LONG_ATTENTION_TOKENS, SHORT_ATTENTION_TOKENS, MinMaxQuantMatMul
 from . import integer
-from .models import Attention, Block, Mlp, PatchMerging, SwinBlock, VisionTransformer, WindowAttention
+from .models import Attention, Block, Mlp, PatchMerging, SwinBlock, SwinTransformer, VisionTransformer, WindowAttention
 
 INTERVALS = ("w_interval", "a_interval", "A_interval", "B_interval", "split")
 
@@ -244,6 +249,42 @@ def unfuse_gather(net):
     for m in net.modules():
         if _gather_site(m) is not None:
             m.fold_gather = False
+
+
+def _stem_site(m):
+    """The (patch-embedding conv, whether the fold normalises) of a model whose stem folds, or None"""
+    if isinstance(m, VisionTransformer):
+        return m.patch_embed.proj, False
+    if isinstance(m, SwinTransformer):
+        return m.patch_embed.proj, True
+    return None
+
+
+def fuse_stem(net):
+    """Mark every VisionTransformer and SwinTransformer in `net` (net itself included) whose patch_embed.proj is a frozen
+    conv module that takes the fold (quant_layers.conv.frozen_stem_ok: out_channels % 4 == 0, Swin also <= 128).  Each
+    call that qualifies (quant_layers.conv.frozen_stem_applies: an FP32 contiguous image, FP32 aligned cls_token and
+    pos_embed of the expected shapes or patch_norm with the conditions of the LayerNorm folds, no gradient wanted) runs
+    the stem as one launch of the conv kernel that stores the token rows -- ViT's cls rows and pos_embed added, Swin's
+    rows normalised by patch_norm -- with the bits of the frozen conv followed by torch's ops; any other call runs the
+    modules and torch's ops as before.  A folded call skips the forward hooks of the conv, of patch_embed and of
+    patch_norm, which is why the fold is opt-in.  It composes with every other fusion; save_quantized / load_quantized do
+    not record it.  Returns the names of the models left unfolded ("" for net itself)."""
+    left = []
+    for name, m in net.named_modules():
+        site = _stem_site(m)
+        if site is not None:
+            conv, norm = site
+            m.fold_stem = isinstance(conv, MinMaxQuantConv2d) and conv.frozen and frozen_stem_ok(conv, norm)
+            if not m.fold_stem:
+                left.append(name)
+    return left
+
+
+def unfuse_stem(net):
+    for m in net.modules():
+        if _stem_site(m) is not None:
+            m.fold_stem = False
 
 
 def _to(v, device):

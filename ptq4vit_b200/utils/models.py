@@ -5,6 +5,7 @@ available offline, so weights are synthetic (trunc-normal 0.02) -- this is harne
 import torch
 import torch.nn as nn
 
+from ..quant_layers.conv import frozen_stem, frozen_stem_applies
 from ..quant_layers.linear import (frozen_gather_applies, frozen_gather_linear, frozen_mlp, frozen_mlp_applies,
                                    frozen_mlp_norm_ok, frozen_norm_applies, frozen_norm_linear, frozen_residual_applies,
                                    frozen_residual_linear)
@@ -158,10 +159,15 @@ class VisionTransformer(nn.Module):
             self.pos_embed.copy_(torch.nn.init.trunc_normal_(torch.empty_like(self.pos_embed), std=0.02, generator=gen))
 
     fold_norm = False      # set by utils.deploy.fuse_norm: fold norm into head, normalising only the cls rows
+    fold_stem = False      # set by utils.deploy.fuse_stem: the frozen patch-embedding conv stores the token rows, the cls
+                           # rows and pos_embed added, when it applies
 
     def forward(self, x):
-        x = self.patch_embed(x)
-        x = torch.cat([self.cls_token.expand(x.shape[0], -1, -1), x], dim=1) + self.pos_embed
+        if self.fold_stem and frozen_stem_applies(self.patch_embed.proj, x, cls_token=self.cls_token, pos_embed=self.pos_embed):
+            x = frozen_stem(self.patch_embed.proj, x, cls_token=self.cls_token, pos_embed=self.pos_embed)
+        else:
+            x = self.patch_embed(x)
+            x = torch.cat([self.cls_token.expand(x.shape[0], -1, -1), x], dim=1) + self.pos_embed
         x = self.blocks(x)
         # LayerNorm is per row: the cls rows normalised alone have the bits of the whole tensor's cls rows
         if self.fold_norm and frozen_norm_applies(self.norm, self.head, x):
@@ -386,8 +392,14 @@ class SwinTransformer(nn.Module):
                     m.fc1.weight.mul_(4.0)
             self.head.weight.mul_(8.0)
 
+    fold_stem = False      # set by utils.deploy.fuse_stem: the frozen patch-embedding conv stores the token rows
+                           # normalised by patch_norm, when it applies
+
     def forward(self, x):
-        x = self.patch_norm(self.patch_embed(x))
+        if self.fold_stem and frozen_stem_applies(self.patch_embed.proj, x, norm=self.patch_norm):
+            x = frozen_stem(self.patch_embed.proj, x, norm=self.patch_norm)
+        else:
+            x = self.patch_norm(self.patch_embed(x))
         x = self.norm(self.layers(x))
         return self.head(x.mean(dim=1))
 
