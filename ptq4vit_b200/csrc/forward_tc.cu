@@ -16,15 +16,17 @@
 //      segment group, folded into r after its last job exactly as the sweep's forward branch does (sweep_tc.cu):
 //      r = -bias, r = fmaf(-scale[g][col / 16], (float)acc, r) in the step's group order, out = -r.  Same integers, same
 //      fp32 operations in the same order: the output is bit-identical to p4v_linear_quant_forward.
-// With FwdMlpParams the same kernel is fc1 of a fused frozen MLP: step 2's epilogue applies torch's GELU and fc2's
-// activation quantiser and writes fc2's int8 activation image instead of FP32 (see the epilogue below, DESIGN §4.8).
-// With FwdNormParams / FwdMlpNormParams a LayerNorm is folded into step 1: the CTA first computes each row's mean and
-// rstd with torch's exact reduction (forward.cuh, p4v_ln_row_stats) and the quantise loop normalises every value before
-// quantising it (DESIGN §4.10).
-// With FwdResParams a block's residual add is folded into the FP32 store: each value goes to its destination row (the
-// identity, or Swin's window reverse and reverse shift, p4v_window_row) as fl(value + shortcut) (DESIGN §4.11).
-// With FwdGatherParams the LayerNorm prologue and the quantise loop read each row from elsewhere in an image: Swin's
-// shifted window partition (p4v_window_row) or PatchMerging's 2x2 neighbourhood (p4v_merge_row) (DESIGN §4.12).
+// The kernel is a template on the fold mask of forward.cuh; each fold adds to the plain forward above (DESIGN §4.5):
+// P4V_FOLD_MLP: the same kernel is fc1 of a fused frozen MLP: step 2's epilogue applies torch's GELU and fc2's activation
+//   quantiser and writes fc2's int8 activation image instead of FP32 (see the epilogue below, DESIGN §4.8).
+// P4V_FOLD_NORM: a LayerNorm is folded into step 1: the CTA first computes each row's mean and rstd with torch's exact
+//   reduction (forward.cuh, p4v_ln_row_stats) and the quantise loop normalises every value before quantising it
+//   (DESIGN §4.10).
+// P4V_FOLD_RES: a block's residual add is folded into the FP32 store: each value goes to its destination row (the
+//   identity, or Swin's window reverse and reverse shift, p4v_window_row) as fl(value + shortcut) (DESIGN §4.11).
+// P4V_FOLD_GATHER (with NORM): the LayerNorm prologue and the quantise loop read each row from elsewhere in an image:
+//   Swin's shifted window partition (p4v_window_row) or PatchMerging's 2x2 neighbourhood (p4v_merge_row) (DESIGN §4.12).
+// p4v_launch_forward_tc instantiates the six fold sets the host uses: none, MLP, NORM, MLP|NORM, RES and NORM|GATHER.
 // 288 threads leave 224 registers per thread without setmaxnreg; the bounded mbarrier wait is inline, and the k32 steps of
 // a stage are one straight-line batch selected by a warp-uniform count (ptxas C7520, see sm90.cuh).
 #include "../../include/ptq4vit_b200.h"
@@ -60,18 +62,18 @@ __device__ __forceinline__ void pack16(uint32_t (&w)[4], int e, float q) {
 // to the column tile of its source column; a padding byte to that of its segment's last column.  Every byte of the image
 // then has exactly one owner, and a CTA stores whole chunks it owns as one 16-byte store and the owned bytes of a chunk
 // that straddles two column tiles one by one.
-__device__ __forceinline__ uint8_t* mlp_epi(const FwdMlpParams& P, uint8_t* smem) {
+__device__ __forceinline__ uint8_t* mlp_epi(const FwdParams& P, uint8_t* smem) {
   return smem + P.a_bytes + (size_t)P.n_stages * P.stage_bytes;
 }
-__device__ __forceinline__ float* mlp_steps(const FwdMlpParams& P, uint8_t* epi) {
+__device__ __forceinline__ float* mlp_steps(const FwdParams& P, uint8_t* epi) {
   return reinterpret_cast<float*>(epi + P.planes2 * P4V_TILE * P4V_MLP_STAGE_LD);
 }
-__device__ __forceinline__ P4VMlpChunk* mlp_chunks(const FwdMlpParams& P, uint8_t* epi) {
+__device__ __forceinline__ P4VMlpChunk* mlp_chunks(const FwdParams& P, uint8_t* epi) {
   return reinterpret_cast<P4VMlpChunk*>(mlp_steps(P, epi) + 2 * P4V_TILE);
 }
 
 // fc2's chunk table (one plane of a row of its image), by the whole CTA before the setup barrier
-__device__ __forceinline__ void mlp_chunk_table(const FwdMlpParams& P, uint8_t* epi) {
+__device__ __forceinline__ void mlp_chunk_table(const FwdParams& P, uint8_t* epi) {
   P4VMlpChunk* tab = mlp_chunks(P, epi);
   for (int s = threadIdx.x; s < P.nseg2; s += kThreads) {
     const P4VSeg sg = P.segs2[s];
@@ -82,7 +84,7 @@ __device__ __forceinline__ void mlp_chunk_table(const FwdMlpParams& P, uint8_t* 
 
 // fc2's step size of each column of tile tn and its reciprocal (0 where p4v_rint_div_ok fails: the exact division), by
 // the consumers between the barriers that open a column tile
-__device__ __forceinline__ void mlp_column_steps(const FwdMlpParams& P, uint8_t* epi, int tn, int et) {
+__device__ __forceinline__ void mlp_column_steps(const FwdParams& P, uint8_t* epi, int tn, int et) {
   float* d = mlp_steps(P, epi);
   for (int lc = et; lc < P4V_TILE; lc += kConsumers) {
     const int col = tn * P4V_TILE + lc;
@@ -94,7 +96,7 @@ __device__ __forceinline__ void mlp_column_steps(const FwdMlpParams& P, uint8_t*
 
 // The thread's 64 fc1 values (r = -value, fragment layout of forward_tc_body) -> GELU -> fc2's bytes, staged by column
 // (quant_image_kernel's sequence for fc2's segments: p4v_quant_plain, the negative plane with d_neg, NaN -> 0)
-__device__ __forceinline__ void mlp_stage_tile(const FwdMlpParams& P, uint8_t* epi, const float (&r)[64], int frow, int fcol) {
+__device__ __forceinline__ void mlp_stage_tile(const FwdParams& P, uint8_t* epi, const float (&r)[64], int frow, int fcol) {
   const float* d = mlp_steps(P, epi);
   const float rcp_neg = __frcp_rn(P.d_neg2), rcp_neg_scalar = __fdiv_rn(1.f, P.d_neg2);
   const bool fast_neg = p4v_rint_div_ok(P.d_neg2), twin = P.planes2 == 2;
@@ -116,7 +118,7 @@ __device__ __forceinline__ void mlp_stage_tile(const FwdMlpParams& P, uint8_t* e
 }
 
 // The bytes of fc2's image that column tile tn of row tile tm owns, from the staged tile; rows past M are zeros
-__device__ __forceinline__ void mlp_store_tile(const FwdMlpParams& P, uint8_t* epi, int tm, int tn, int et) {
+__device__ __forceinline__ void mlp_store_tile(const FwdParams& P, uint8_t* epi, int tm, int tn, int et) {
   const P4VMlpChunk* tab = mlp_chunks(P, epi);
   const int c0 = tn * P4V_TILE, c1 = min(c0 + P4V_TILE, P.N);
   // the chunks with a byte in [c0, c1): kf and the owner of the last byte grow with the chunk index
@@ -157,20 +159,19 @@ __device__ __forceinline__ void mlp_store_tile(const FwdMlpParams& P, uint8_t* e
 }
 
 // The LayerNorm prologue's row stats, the last P4V_NORM_STATS_BYTES before the control block: mean [128], then rstd [128]
-template <class Par>
-__device__ __forceinline__ float* ln_stats(const Par& P, uint8_t* smem) {
+__device__ __forceinline__ float* ln_stats(const FwdParams& P, unsigned folds, uint8_t* smem) {
   return reinterpret_cast<float*>(smem + P.a_bytes + (size_t)P.n_stages * P.stage_bytes +
-                                  (p4v_fwd_extra_bytes(P) - P4V_NORM_STATS_BYTES));
+                                  (p4v_fwd_extra_bytes(folds, P.epi_bytes) - P4V_NORM_STATS_BYTES));
 }
 
-// ---- the row gather of FwdGatherParams (DESIGN §4.12) ----------------------------------------------------------------
+// ---- the row gather of P4V_FOLD_GATHER (DESIGN §4.12) ----------------------------------------------------------------
 // The source row of each tile row, right below the row stats: the window map's image row, or the merge's first row
-__device__ __forceinline__ int* gather_rows(const FwdGatherParams& P, uint8_t* smem) {
-  return reinterpret_cast<int*>(ln_stats(P, smem)) - P4V_TILE;
+__device__ __forceinline__ int* gather_rows(const FwdParams& P, uint8_t* smem) {
+  return reinterpret_cast<int*>(ln_stats(P, P4V_FOLD_NORM | P4V_FOLD_GATHER, smem)) - P4V_TILE;
 }
 
 // Mean and rstd of tile row r (global row `row`), read from its source rows; returns the source row
-__device__ __forceinline__ int gather_row_stats(const FwdGatherParams& P, int row, int lane, float& mean, float& rstd) {
+__device__ __forceinline__ int gather_row_stats(const FwdParams& P, int row, int lane, float& mean, float& rstd) {
   const int K = (int)P.ld;
   if (P.ga.mode == P4V_GATHER_WINDOW) {
     const int s = p4v_window_row(P.ga.win, row);
@@ -190,7 +191,7 @@ __device__ __forceinline__ int gather_row_stats(const FwdGatherParams& P, int ro
 
 // The chunk's FP32 values (ch.n of them, zeros after) of the tile row whose source row is s.  A merge chunk inside one
 // quarter reads like a contiguous row; one that straddles two quarters (C % 16 != 0) reads element by element.
-__device__ __forceinline__ void gather_chunk(const FwdGatherParams& P, int s, int k0, int n, float (&vals)[16]) {
+__device__ __forceinline__ void gather_chunk(const FwdParams& P, int s, int k0, int n, float (&vals)[16]) {
   const int K = (int)P.ld;
   const float* src;
   if (P.ga.mode == P4V_GATHER_WINDOW) {
@@ -217,18 +218,18 @@ __device__ __forceinline__ void gather_chunk(const FwdGatherParams& P, int s, in
   }
 }
 
-// Par = FwdParams: the frozen Linear forward, FP32 output.  Par = FwdMlpParams: fc1 of a frozen MLP, GELU-and-quantise
-// epilogue into fc2's image.  FwdNormParams / FwdMlpNormParams: the same with a LayerNorm prologue.  FwdResParams: the
-// plain forward whose store adds the shortcut.  FwdGatherParams: FwdNormParams with gathered rows.
-template <class Par>
-__global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_constant__ Par P) {
-  constexpr bool kMlp = kIsMlp<Par>;
+// kFolds = 0: the frozen Linear forward, FP32 output.  P4V_FOLD_MLP: fc1 of a frozen MLP, GELU-and-quantise epilogue
+// into fc2's image.  P4V_FOLD_NORM: a LayerNorm prologue.  P4V_FOLD_RES: the plain forward whose store adds the
+// shortcut.  P4V_FOLD_GATHER (with NORM): the LayerNorm's rows gathered from an image.
+template <unsigned kFolds>
+__global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_constant__ FwdParams P) {
+  constexpr bool kMlp = kFolds & P4V_FOLD_MLP;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
   // carve: [resident activation tile][weight ring][MLP epilogue][LayerNorm row stats][control]
   const uint32_t nst = P.n_stages, sC = P.stage_bytes;
   const uint32_t resA = smem_u32(smem), ring = resA + P.a_bytes;
-  FwdCtl& S = *reinterpret_cast<FwdCtl*>(smem + P.a_bytes + (size_t)nst * sC + p4v_fwd_extra_bytes(P));
+  FwdCtl& S = *reinterpret_cast<FwdCtl*>(smem + P.a_bytes + (size_t)nst * sC + p4v_fwd_extra_bytes(kFolds, P.epi_bytes));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // the CTA's row tile and its share of the column tiles
@@ -237,13 +238,13 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
   const int tn0 = cs * P.tiles_n / csplit, tn1 = (cs + 1) * P.tiles_n / csplit;
 
   // ---- LayerNorm prologue: mean and rstd of every row of the tile, one warp per row (released by the setup barrier) ----
-  if constexpr (kIsNorm<Par>) {
-    float* ln_mean = ln_stats(P, smem);
+  if constexpr ((kFolds & P4V_FOLD_NORM) != 0) {
+    float* ln_mean = ln_stats(P, kFolds, smem);
     for (int r = warp; r < P4V_TILE; r += kThreads / 32) {
       const int row = tm * P4V_TILE + r;
       if (row >= P.M) break;
       float mean, rstd;
-      if constexpr (kIsGather<Par>) {
+      if constexpr ((kFolds & P4V_FOLD_GATHER) != 0) {
         const int s = gather_row_stats(P, row, lane, mean, rstd);
         if (lane == 0) gather_rows(P, smem)[r] = s;
       } else {
@@ -279,7 +280,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
       uint32_t wp[4] = {0u, 0u, 0u, 0u}, wn[4] = {0u, 0u, 0u, 0u};
       if (row < P.M && ch.n > 0) {
         float vals[16];
-        if constexpr (kIsGather<Par>) {
+        if constexpr ((kFolds & P4V_FOLD_GATHER) != 0) {
           gather_chunk(P, gather_rows(P, smem)[r], ch.k0, ch.n, vals);
         } else {
           const float* src = P.x + (size_t)row * P.ld + ch.k0;
@@ -292,8 +293,8 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
             for (int e = 0; e < 16; ++e) vals[e] = e < ch.n ? src[e] : 0.f;
           }
         }
-        if constexpr (kIsNorm<Par>) {
-          const float* ln_mean = ln_stats(P, smem);
+        if constexpr ((kFolds & P4V_FOLD_NORM) != 0) {
+          const float* ln_mean = ln_stats(P, kFolds, smem);
           const float mean = ln_mean[r], rstd = ln_mean[P4V_TILE + r];
           float g[16], b[16];
           if (ch.n == 16 && (ch.k0 & 3) == 0) {          // gamma and beta are 16-byte aligned at a multiple of 4
@@ -410,7 +411,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
       asm volatile("bar.sync 1, %0;" ::"n"(kConsumers));   // staged tile complete
       // the next column tile's first barrier orders these reads of the staging before it is written again
       mlp_store_tile(P, mlp_epi(P, smem), tm, tn, et);
-    } else if constexpr (kIsRes<Par>) {
+    } else if constexpr ((kFolds & P4V_FOLD_RES) != 0) {
       // the residual add: out[dst] = fl(-r + res[dst]) (torch's FP32 add of the stored value and the shortcut), the
       // shortcut read at the destination rows as the pairs the plain store writes
       const bool pairs = (P.N & 1) == 0;
@@ -455,18 +456,28 @@ __global__ void gelu_probe_kernel(const float* __restrict__ x, float* __restrict
 
 }  // namespace
 
-template <class Par> int p4v_launch_forward_tc(const Par& p, int num_sms, cudaStream_t st) {
-  if constexpr (kIsMlp<Par>)
+int p4v_launch_forward_tc(const FwdParams& p, unsigned folds, int num_sms, cudaStream_t st) {
+  void (*kernel)(const FwdParams);
+  switch (folds) {
+    case 0: kernel = forward_tc_kernel<0>; break;
+    case P4V_FOLD_MLP: kernel = forward_tc_kernel<P4V_FOLD_MLP>; break;
+    case P4V_FOLD_NORM: kernel = forward_tc_kernel<P4V_FOLD_NORM>; break;
+    case P4V_FOLD_MLP | P4V_FOLD_NORM: kernel = forward_tc_kernel<P4V_FOLD_MLP | P4V_FOLD_NORM>; break;
+    case P4V_FOLD_RES: kernel = forward_tc_kernel<P4V_FOLD_RES>; break;
+    case P4V_FOLD_NORM | P4V_FOLD_GATHER: kernel = forward_tc_kernel<P4V_FOLD_NORM | P4V_FOLD_GATHER>; break;
+    default: P4V_REQUIRE(false, "forward: no kernel for the fold set 0x%x", folds);
+  }
+  if (folds & P4V_FOLD_MLP)
     P4V_REQUIRE(!p.twin && (p.planes2 == 1 || p.planes2 == 2) && p.epi_bytes == p4v_mlp_epi_bytes(p.planes2, p.n_chunks2) &&
                 (reinterpret_cast<uintptr_t>(p.X2) & 15) == 0, "mlp forward: bad epilogue plan");
-  if constexpr (kIsNorm<Par>) P4V_REQUIRE(!p.twin && p.ld % 4 == 0 && p.ln.gamma && p.ln.beta, "forward: bad LayerNorm plan");
-  if constexpr (kIsRes<Par>) {
+  if (folds & P4V_FOLD_NORM) P4V_REQUIRE(!p.twin && p.ld % 4 == 0 && p.ln.gamma && p.ln.beta, "forward: bad LayerNorm plan");
+  if (folds & P4V_FOLD_RES) {
     const p4v_window_layout& w = p.rs.win;
     P4V_REQUIRE(p.rs.res && (reinterpret_cast<uintptr_t>(p.rs.res) & 7) == 0, "forward: residual must be 8-byte aligned");
     P4V_REQUIRE(w.window == 0 || ((long long)w.images * w.height * w.width == p.M && w.height % w.window == 0 &&
                                   w.width % w.window == 0 && w.shift >= 0 && w.shift < w.window), "forward: bad window layout");
   }
-  if constexpr (kIsGather<Par>) {
+  if (folds & P4V_FOLD_GATHER) {
     const p4v_window_layout& w = p.ga.win;
     const bool window = p.ga.mode == P4V_GATHER_WINDOW && w.window > 0 && w.height % w.window == 0 &&
                         w.width % w.window == 0 && w.shift >= 0 && w.shift < w.window && p.ld % 4 == 0 &&
@@ -475,7 +486,7 @@ template <class Par> int p4v_launch_forward_tc(const Par& p, int num_sms, cudaSt
                        w.width % 2 == 0 && p.ld % 16 == 0 && (long long)w.images * (w.height / 2) * (w.width / 2) == p.M;
     P4V_REQUIRE(w.images > 0 && w.height > 0 && w.width > 0 && (window || merge), "forward: bad gather layout");
   }
-  const unsigned extra = p4v_fwd_extra_bytes(p);
+  const unsigned extra = p4v_fwd_extra_bytes(folds, p.epi_bytes);
   P4V_REQUIRE(p.n_jobs >= 1 && p.n_jobs <= P4V_MAX_JOBS && p.n_groups <= P4V_MAX_GROUPS, "forward: too many K segments");
   P4V_REQUIRE(p.n_stages >= 2 && p.n_stages <= P4V_FWD_MAX_STAGES && p.n_chunks <= P4V_FWD_MAX_CHUNKS &&
               p.stage_bytes % 128 == 0 && p.a_bytes % 128 == 0 && extra % 128 == 0, "forward: bad shared-memory plan");
@@ -487,18 +498,12 @@ template <class Par> int p4v_launch_forward_tc(const Par& p, int num_sms, cudaSt
   // from L2) so that the whole GPU writes output.
   int csplit = num_sms / p.tiles_m;
   csplit = csplit < 1 ? 1 : (csplit > p.tiles_n ? p.tiles_n : csplit);
-  P4V_CUDA_OK(cudaFuncSetAttribute(forward_tc_kernel<Par>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  forward_tc_kernel<Par><<<p.tiles_m * csplit, kThreads, smem, st>>>(p);
+  P4V_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<p.tiles_m * csplit, kThreads, smem, st>>>(p);
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   return 0;
 }
-template int p4v_launch_forward_tc(const FwdParams&, int, cudaStream_t);
-template int p4v_launch_forward_tc(const FwdMlpParams&, int, cudaStream_t);
-template int p4v_launch_forward_tc(const FwdNormParams&, int, cudaStream_t);
-template int p4v_launch_forward_tc(const FwdMlpNormParams&, int, cudaStream_t);
-template int p4v_launch_forward_tc(const FwdResParams&, int, cudaStream_t);
-template int p4v_launch_forward_tc(const FwdGatherParams&, int, cudaStream_t);
 
 // Diagnostic: y = p4v_gelu(x) elementwise (the GELU of mlp_fc1_kernel's epilogue)
 extern "C" int p4v_gelu_probe(const float* x, float* y, long long n, void* stream) {

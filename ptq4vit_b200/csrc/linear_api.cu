@@ -740,25 +740,21 @@ int build_frozen(const p4v_linear_desc* d, FrozenPlan& f, bool for_pack) {
   return 0;
 }
 
-// The ring stages the fused kernel gets for a call of the layer f1 -- as fc1 of a fused MLP whose fc2 is f2, with a
-// LayerNorm folded into its activation quantiser (norm), with a row gather in front of that LayerNorm (gather) -- or 0
-// when the call does not take the fused kernel.  f1 must be on it itself; an MLP needs fc1's outputs to be fc2's inputs
-// and a plain fc1, a LayerNorm a plain layer with K % 4 == 0.  The epilogue, the gather's source rows and the row stats
-// take their share of shared memory, which can only lower the count.
-int fused_stages(const FrozenPlan& f1, const FrozenPlan* f2, bool norm, bool gather = false) {
+// The ring stages the fused kernel gets for a call of the layer f1 with the folds `folds` -- as fc1 of a fused MLP whose
+// fc2 is f2 (P4V_FOLD_MLP), with a LayerNorm folded into its activation quantiser (NORM), with a row gather of
+// gather_mode in front of that LayerNorm (GATHER) -- or 0 when the call does not take the fused kernel.  f1 must be on it
+// itself; an MLP needs fc1's outputs to be fc2's inputs and a plain fc1, a LayerNorm a plain layer with K % 4 == 0, the
+// merge gather C = K / 4 a multiple of 4, so that no float4 of the LayerNorm's walk straddles a quarter.  The epilogue,
+// the gather's source rows and the row stats take their share of shared memory, which can only lower the count.
+int fold_stages(const FrozenPlan& f1, const FrozenPlan* f2, unsigned folds, int gather_mode = 0) {
   const LinPlan& p1 = f1.p;
-  if (f1.stages < 2 || (f2 && (p1.O != f2->p.K || p1.twin)) || (norm && (p1.twin || p1.K % 4 != 0))) return 0;
+  if (f1.stages < 2 || (f2 && (p1.O != f2->p.K || p1.twin)) ||
+      ((folds & P4V_FOLD_NORM) && (p1.twin || p1.K % 4 != 0)) ||
+      ((folds & P4V_FOLD_GATHER) && gather_mode == P4V_GATHER_MERGE && p1.K % 16 != 0)) return 0;
   // a plane of fc2's activation image has the K layout of its weight image; a post-GELU fc2 has two
   const unsigned epi = f2 ? p4v_mlp_epi_bytes(f2->p.twin ? 2 : 1, f2->p.Wcur.kb / 16) : 0u;
-  return frozen_ring_stages(f1.X.tile_bytes() + p4v_fwd_extra_bytes(epi, norm, gather), (size_t)f1.stage_kb * P4V_TILE,
+  return frozen_ring_stages(f1.X.tile_bytes() + p4v_fwd_extra_bytes(folds, epi), (size_t)f1.stage_kb * P4V_TILE,
                             p1.Wcur.kb / 16);
-}
-
-// The ring stages of a row gather of `mode` in front of the LayerNorm folded into f (p4v_linear_gather_ok), 0 when it
-// does not fold: the merge needs C = K / 4 a multiple of 4, so that no float4 of the LayerNorm's walk straddles a quarter.
-int gather_stages(const FrozenPlan& f, int mode) {
-  if (mode == P4V_GATHER_MERGE && f.p.K % 16 != 0) return 0;
-  return fused_stages(f, nullptr, true, true);
 }
 
 }  // namespace
@@ -792,7 +788,7 @@ extern "C" int p4v_linear_frozen_path(const p4v_linear_desc* d, int* path) {
   FrozenPlan f; int rc = build_frozen(d, f, true);
   if (rc) return rc;
   P4V_REQUIRE(path != nullptr, "null output");
-  *path = fused_stages(f, nullptr, false) ? 1 : 0;
+  *path = fold_stages(f, nullptr, 0) ? 1 : 0;
   return 0;
 }
 
@@ -800,7 +796,7 @@ extern "C" int p4v_linear_frozen_workspace_bytes(const p4v_linear_desc* d, size_
   FrozenPlan f; int rc = build_frozen(d, f, false);
   if (rc) return rc;
   P4V_REQUIRE(bytes != nullptr, "null output");
-  *bytes = fused_stages(f, nullptr, false) ? 0 : f.X.bytes();
+  *bytes = fold_stages(f, nullptr, 0) ? 0 : f.X.bytes();
   return 0;
 }
 
@@ -822,7 +818,7 @@ void fill_fwd(const FrozenPlan& f, const float* x, const float* bias, void* pack
 }
 
 // fc2's part of a fused MLP's parameters: the epilogue writes fc2's activation image into the workspace
-void fill_mlp(const FrozenPlan& f2, void* pack2, void* workspace, FwdMlpParams& q) {
+void fill_mlp(const FrozenPlan& f2, void* pack2, void* workspace, FwdParams& q) {
   const LinPlan& p2 = f2.p;
   q.X2 = f2.X.ptr(workspace); q.X2_tile_bytes = f2.X.tile_bytes(); q.X2_plane_bytes = (unsigned)p2.Wcur.tile_bytes();
   q.segs2 = p2.segsX.dev(pack2); q.nseg2 = (int)p2.segs.size();
@@ -870,16 +866,15 @@ int check_layout(const char* fn, const p4v_window_layout& win, int rows) {
   return 0;
 }
 
-// The arguments of a row gather (DESIGN §4.12) of a call with `rows` output rows and K = in_features, the image x
+// The layout of a non-null row gather (DESIGN §4.12) of a call with `rows` output rows and K = in_features, the image x
 // apart from out ([rows][out_cols]); x's null pointer and alignment are check_norm's
-int check_gather(const char* fn, const p4v_input_gather* g, const float* x, const float* out, int rows, int K, int out_cols) {
-  P4V_REQUIRE(g, "%s: null pointer", fn);
-  const p4v_window_layout& w = g->layout;
-  if (g->mode == P4V_GATHER_WINDOW) {
+int check_gather(const char* fn, const p4v_input_gather& g, const float* x, const float* out, int rows, int K, int out_cols) {
+  const p4v_window_layout& w = g.layout;
+  if (g.mode == P4V_GATHER_WINDOW) {
     if (int rc = check_layout(fn, w, rows)) return rc;
   } else {
-    P4V_REQUIRE(g->mode == P4V_GATHER_MERGE, "%s: gather mode must be P4V_GATHER_WINDOW or P4V_GATHER_MERGE (got %d)", fn,
-                g->mode);
+    P4V_REQUIRE(g.mode == P4V_GATHER_MERGE, "%s: gather mode must be P4V_GATHER_WINDOW or P4V_GATHER_MERGE (got %d)", fn,
+                g.mode);
     P4V_REQUIRE(w.window == 0 && w.shift == 0, "%s: merge layout: window and shift must be 0 (got %d, %d)", fn, w.window,
                 w.shift);
     P4V_REQUIRE(w.images > 0 && w.height > 0 && w.width > 0 && w.height % 2 == 0 && w.width % 2 == 0,
@@ -910,95 +905,109 @@ int check_residual(const char* fn, const float* res, const float* out, int rows,
   return 0;
 }
 
-// A call of the fused kernel on the frozen layer f1: validates every argument of the entry point fn (in its order, with
-// its name in the messages), fills the kernel's parameters and launches it.  Par selects the variant: with a LayerNorm
-// (ln) folded into the activation quantiser, and as fc1 of a fused MLP whose epilogue writes the image of its fc2 (f2)
-// into the workspace, which fc2's sweep forward then reads.  The arguments of fc2, the packed sizes and the workspace
-// are read by the MLP only.  A residual (rs.res non-null) is added by the last launch's store: the plain kernel's
-// (FwdResParams, with rs.win) or fc2's sweep (identity rows).
-template <class Par>
-int fused_forward(const char* fn, const FrozenPlan& f1, const float* x, const FwdNorm& ln, const FwdResidual& rs,
-                  const p4v_input_gather* ga, const float* bias1, const void* pack1, size_t pack1_bytes,
-                  const FrozenPlan* f2, const float* bias2, const void* pack2, size_t pack2_bytes, void* workspace,
-                  size_t workspace_bytes, float* out, cudaStream_t st) {
-  constexpr bool mlp = kIsMlp<Par>, norm = kIsNorm<Par>;
-  if constexpr (norm) {
-    if (int rc = check_norm(fn, x, ln.gamma, ln.beta, ln.eps)) return rc;
-  }
-  if constexpr (mlp)
-    P4V_REQUIRE(f1.p.d.rows == f2->p.d.rows, "%s: fc1 and fc2 must have the same rows (%d != %d)", fn, f1.p.d.rows,
-                f2->p.d.rows);
-  P4V_REQUIRE(x && pack1 && (!mlp || (pack2 && workspace)) && out, "%s: null pointer", fn);
-  P4V_REQUIRE((!f1.p.d.has_bias || bias1) && (!mlp || !f2->p.d.has_bias || bias2), "%s: has_bias set but bias is null", fn);
-  constexpr bool gather = kIsGather<Par>;
-  if constexpr (gather) P4V_REQUIRE(ga, "%s: null pointer", fn);
-  const int stages = gather ? gather_stages(f1, ga->mode) : fused_stages(f1, f2, norm);
-  P4V_REQUIRE(stages, "%s: %s", fn, mlp ? (norm ? "these layers do not fuse with the LayerNorm (p4v_mlp_norm_ok)"
-                                                : "these layers do not fuse (p4v_mlp_fused_ok)")
-                                        : gather ? "the gather does not fold into this layer (p4v_linear_gather_ok)"
-                                                 : "the LayerNorm does not fold into this layer (p4v_linear_norm_ok)");
-  if constexpr (gather) {
-    if (int rc = check_gather(fn, ga, x, out, f1.p.M, f1.p.K, f1.p.O)) return rc;
-  }
-  if constexpr (mlp) {
-    P4V_REQUIRE(pack1_bytes >= f1.bytes && pack2_bytes >= f2->bytes, "%s: packed buffer too small "
-                "(fc1 %zu < %zu or fc2 %zu < %zu)", fn, pack1_bytes, f1.bytes, pack2_bytes, f2->bytes);
-    P4V_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0 &&
-                (reinterpret_cast<uintptr_t>(workspace) & 15) == 0,
-                "%s: %sworkspace must be 16-byte and out 8-byte aligned", fn, norm ? "" : "x and ");   // check_norm took x
-    P4V_REQUIRE(workspace_bytes >= f2->X.bytes(), "%s: workspace too small (%zu < %zu)", fn, workspace_bytes, f2->X.bytes());
-  }
-  P4V_REQUIRE(!mlp || rs.win.window == 0, "%s: fc2 of a fused MLP takes no window layout", fn);
-  if (int rc = check_residual(fn, rs.res, out, f1.p.M, mlp ? f2->p.O : f1.p.O, rs.win)) return rc;
-  // the plan's accessors take the buffers they index; nothing writes them
-  void* p1 = const_cast<void*>(pack1);
-  void* p2 = const_cast<void*>(pack2);
-  Par q{};
-  fill_fwd(f1, x, bias1, p1, mlp ? nullptr : out, q);
-  q.n_stages = (unsigned)stages;
-  if constexpr (norm) q.ln = ln;
-  if constexpr (mlp) fill_mlp(*f2, p2, workspace, q);
-  if constexpr (kIsRes<Par>) q.rs = rs;
-  if constexpr (gather) q.ga = FwdGather{ga->mode, ga->layout};
-  const int rc = p4v_launch_forward_tc(q, p4v_num_sms(), st);
-  if (rc || !mlp) return rc;
-  return streamed_sweep(*f2, p2, workspace, bias2, rs.res, out, st);
+// One call of frozen layers: layer f1 on x, optionally with a LayerNorm folded into its activation quantiser (ln), with
+// its rows gathered from an image in front of that LayerNorm (gather, *ga), as fc1 of a fused MLP whose epilogue writes
+// the image of its fc2 (f2) into the workspace, which fc2's sweep forward then reads, and with a residual added by the
+// last store (rs.res non-null; rs.win: Swin's window reverse, on f1's fused kernel only).
+struct FrozenCall {
+  const FrozenPlan* f1; const float* x; const float* bias1; const void* pack1; size_t pack1_bytes;
+  const FwdNorm* ln;                                   // null: no LayerNorm
+  bool gather; const p4v_input_gather* ga;
+  const FrozenPlan* f2; const float* bias2; const void* pack2; size_t pack2_bytes;   // f2 null: no MLP
+  FwdResidual rs;
+  void* workspace; size_t workspace_bytes;
+  float* out;
+};
+
+FrozenCall linear_call(const FrozenPlan& f, const float* x, const float* bias, const void* packed, float* out) {
+  FrozenCall c{};
+  c.f1 = &f; c.x = x; c.bias1 = bias; c.pack1 = packed; c.out = out;
+  return c;
 }
 
-// p4v_linear_frozen_forward (rs.res null) and p4v_linear_frozen_forward_res, on the layer's path
-int frozen_forward(const char* fn, const p4v_linear_desc* d, const float* x, const float* bias, const void* packed_in,
-                   void* workspace, size_t workspace_bytes, const FwdResidual& rs, float* out, cudaStream_t st) {
-  FrozenPlan f; int rc = build_frozen(d, f, false);
-  if (rc) return rc;
-  const LinPlan& p = f.p;
-  void* packed = const_cast<void*>(packed_in);      // the plan's accessors take the buffer they index; nothing writes it
-  P4V_REQUIRE(x && packed && out, "%s: null pointer", fn);
-  P4V_REQUIRE(!d->has_bias || bias, "%s: has_bias set but bias is null", fn);
-  if (fused_stages(f, nullptr, false)) {
-    if (rs.res)
-      return fused_forward<FwdResParams>(fn, f, x, FwdNorm{}, rs, nullptr, bias, packed, 0, nullptr, nullptr, nullptr, 0,
-                                         nullptr, 0, out, st);
-    return fused_forward<FwdParams>(fn, f, x, FwdNorm{}, rs, nullptr, bias, packed, 0, nullptr, nullptr, nullptr, 0, nullptr,
-                                    0, out, st);
+FrozenCall mlp_call(const FrozenPlan& f1, const float* x, const float* bias1, const void* pack1, size_t pack1_bytes,
+                    const FrozenPlan& f2, const float* bias2, const void* pack2, size_t pack2_bytes, void* workspace,
+                    size_t workspace_bytes, float* out) {
+  FrozenCall c = linear_call(f1, x, bias1, pack1, out);
+  c.pack1_bytes = pack1_bytes; c.f2 = &f2; c.bias2 = bias2; c.pack2 = pack2; c.pack2_bytes = pack2_bytes;
+  c.workspace = workspace; c.workspace_bytes = workspace_bytes;
+  return c;
+}
+
+// Validates every argument of the call c of entry point fn (with its name in the messages), then runs it: the fused
+// kernel with the call's folds (then fc2's sweep forward for an MLP), or, for a plain layer that is not on the fused
+// kernel, the streamed path (the int8 activation image in the workspace, then the layer's sweep forward).
+int frozen_call(const char* fn, const FrozenCall& c, cudaStream_t st) {
+  const FrozenPlan& f1 = *c.f1;
+  const bool mlp = c.f2 != nullptr, norm = c.ln != nullptr;
+  const unsigned folds = (mlp ? P4V_FOLD_MLP : 0u) | (norm ? P4V_FOLD_NORM : 0u) | (c.gather ? P4V_FOLD_GATHER : 0u) |
+                         (c.rs.res && !mlp ? P4V_FOLD_RES : 0u);
+  if (norm) {
+    if (int rc = check_norm(fn, c.x, c.ln->gamma, c.ln->beta, c.ln->eps)) return rc;
   }
-  P4V_REQUIRE(workspace && workspace_bytes >= f.X.bytes(), "%s: workspace too small (%zu < %zu)", fn,
-              workspace ? workspace_bytes : (size_t)0, f.X.bytes());
-  P4V_REQUIRE(rs.win.window == 0, "%s: a window layout needs the fused path (p4v_linear_frozen_path 1)", fn);
-  if ((rc = check_residual(fn, rs.res, out, p.M, p.O, rs.win))) return rc;
-  QuantImageArgs qa{};
-  f.X.fill(qa, workspace);
-  qa.src = x; qa.ld = p.K; qa.rows = p.M; qa.delta = at<float>(packed, f.o_dX); qa.d_mod = 1;
-  qa.rows_per_block = p.M + P4V_TILE; qa.segs = p.segsX.dev(packed); qa.nseg = (int)p.segsX.host.size();
-  if ((rc = p4v_quant_image(qa, st))) return rc;
-  return streamed_sweep(f, packed, workspace, bias, rs.res, out, st);
+  if (mlp)
+    P4V_REQUIRE(f1.p.d.rows == c.f2->p.d.rows, "%s: fc1 and fc2 must have the same rows (%d != %d)", fn, f1.p.d.rows,
+                c.f2->p.d.rows);
+  P4V_REQUIRE(c.x && c.pack1 && (!mlp || (c.pack2 && c.workspace)) && c.out, "%s: null pointer", fn);
+  P4V_REQUIRE((!f1.p.d.has_bias || c.bias1) && (!mlp || !c.f2->p.d.has_bias || c.bias2), "%s: has_bias set but bias is null", fn);
+  if (c.gather) P4V_REQUIRE(c.ga, "%s: null pointer", fn);
+  const int stages = fold_stages(f1, c.f2, folds, c.gather ? c.ga->mode : 0);
+  if (folds & ~P4V_FOLD_RES)
+    P4V_REQUIRE(stages, "%s: %s", fn, mlp ? (norm ? "these layers do not fuse with the LayerNorm (p4v_mlp_norm_ok)"
+                                                  : "these layers do not fuse (p4v_mlp_fused_ok)")
+                                          : c.gather ? "the gather does not fold into this layer (p4v_linear_gather_ok)"
+                                                     : "the LayerNorm does not fold into this layer (p4v_linear_norm_ok)");
+  if (c.gather) {
+    if (int rc = check_gather(fn, *c.ga, c.x, c.out, f1.p.M, f1.p.K, f1.p.O)) return rc;
+  }
+  if (mlp) {
+    P4V_REQUIRE(c.pack1_bytes >= f1.bytes && c.pack2_bytes >= c.f2->bytes, "%s: packed buffer too small "
+                "(fc1 %zu < %zu or fc2 %zu < %zu)", fn, c.pack1_bytes, f1.bytes, c.pack2_bytes, c.f2->bytes);
+    P4V_REQUIRE((reinterpret_cast<uintptr_t>(c.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.out) & 7) == 0 &&
+                (reinterpret_cast<uintptr_t>(c.workspace) & 15) == 0,
+                "%s: %sworkspace must be 16-byte and out 8-byte aligned", fn, norm ? "" : "x and ");   // check_norm took x
+    P4V_REQUIRE(c.workspace_bytes >= c.f2->X.bytes(), "%s: workspace too small (%zu < %zu)", fn, c.workspace_bytes,
+                c.f2->X.bytes());
+  }
+  if (!stages) {
+    P4V_REQUIRE(c.workspace && c.workspace_bytes >= f1.X.bytes(), "%s: workspace too small (%zu < %zu)", fn,
+                c.workspace ? c.workspace_bytes : (size_t)0, f1.X.bytes());
+    P4V_REQUIRE(c.rs.win.window == 0, "%s: a window layout needs the fused path (p4v_linear_frozen_path 1)", fn);
+  }
+  if (int rc = check_residual(fn, c.rs.res, c.out, f1.p.M, mlp ? c.f2->p.O : f1.p.O, c.rs.win)) return rc;
+  // the plan's accessors take the buffers they index; nothing writes them
+  void* p1 = const_cast<void*>(c.pack1);
+  void* p2 = const_cast<void*>(c.pack2);
+  if (!stages) {
+    const LinPlan& p = f1.p;
+    QuantImageArgs qa{};
+    f1.X.fill(qa, c.workspace);
+    qa.src = c.x; qa.ld = p.K; qa.rows = p.M; qa.delta = at<float>(p1, f1.o_dX); qa.d_mod = 1;
+    qa.rows_per_block = p.M + P4V_TILE; qa.segs = p.segsX.dev(p1); qa.nseg = (int)p.segsX.host.size();
+    if (int rc = p4v_quant_image(qa, st)) return rc;
+    return streamed_sweep(f1, p1, c.workspace, c.bias1, c.rs.res, c.out, st);
+  }
+  FwdParams q{};
+  fill_fwd(f1, c.x, c.bias1, p1, mlp ? nullptr : c.out, q);
+  q.n_stages = (unsigned)stages;
+  if (mlp) fill_mlp(*c.f2, p2, c.workspace, q);
+  if (norm) q.ln = *c.ln;
+  if (folds & P4V_FOLD_RES) q.rs = c.rs;
+  if (c.gather) q.ga = FwdGather{c.ga->mode, c.ga->layout};
+  const int rc = p4v_launch_forward_tc(q, folds, p4v_num_sms(), st);
+  if (rc || !mlp) return rc;
+  return streamed_sweep(*c.f2, p2, c.workspace, c.bias2, c.rs.res, c.out, st);
 }
 
 }  // namespace
 
-extern "C" int p4v_linear_frozen_forward(const p4v_linear_desc* d, const float* x, const float* bias, const void* packed_in,
+extern "C" int p4v_linear_frozen_forward(const p4v_linear_desc* d, const float* x, const float* bias, const void* packed,
                                          void* workspace, size_t workspace_bytes, float* out, void* stream) {
-  return frozen_forward("linear_frozen_forward", d, x, bias, packed_in, workspace, workspace_bytes, FwdResidual{}, out,
-                        (cudaStream_t)stream);
+  FrozenPlan f; int rc = build_frozen(d, f, false);
+  if (rc) return rc;
+  FrozenCall c = linear_call(f, x, bias, packed, out);
+  c.workspace = workspace; c.workspace_bytes = workspace_bytes;
+  return frozen_call("linear_frozen_forward", c, (cudaStream_t)stream);
 }
 
 // ---- fused frozen MLP: fc1 + GELU + fc2's activation quantiser in one kernel, then fc2's sweep forward -----------
@@ -1017,7 +1026,7 @@ extern "C" int p4v_mlp_fused_ok(const p4v_linear_desc* fc1, const p4v_linear_des
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, true);
   if (rc) return rc;
   P4V_REQUIRE(ok != nullptr, "null output");
-  *ok = fused_stages(f1, &f2, false) ? 1 : 0;
+  *ok = fold_stages(f1, &f2, P4V_FOLD_MLP) ? 1 : 0;
   return 0;
 }
 
@@ -1035,8 +1044,8 @@ extern "C" int p4v_mlp_frozen_forward(const p4v_linear_desc* fc1, const float* x
                                       size_t pack2_bytes, void* workspace, size_t workspace_bytes, float* out, void* stream) {
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
-  return fused_forward<FwdMlpParams>("mlp_frozen_forward", f1, x, FwdNorm{}, FwdResidual{}, nullptr, bias1, pack1, pack1_bytes,
-                                     &f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out, (cudaStream_t)stream);
+  return frozen_call("mlp_frozen_forward", mlp_call(f1, x, bias1, pack1, pack1_bytes, f2, bias2, pack2, pack2_bytes,
+                                                    workspace, workspace_bytes, out), (cudaStream_t)stream);
 }
 
 // ---- LayerNorm folded into the activation quantiser of the fused kernel (forward_tc.cu, DESIGN §4.10) -------------
@@ -1044,7 +1053,7 @@ extern "C" int p4v_linear_norm_ok(const p4v_linear_desc* d, int* ok) {
   FrozenPlan f; int rc = build_frozen(d, f, true);
   if (rc) return rc;
   P4V_REQUIRE(ok != nullptr, "null output");
-  *ok = fused_stages(f, nullptr, true) ? 1 : 0;
+  *ok = fold_stages(f, nullptr, P4V_FOLD_NORM) ? 1 : 0;
   return 0;
 }
 
@@ -1052,16 +1061,18 @@ extern "C" int p4v_mlp_norm_ok(const p4v_linear_desc* fc1, const p4v_linear_desc
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, true);
   if (rc) return rc;
   P4V_REQUIRE(ok != nullptr, "null output");
-  *ok = fused_stages(f1, &f2, true) ? 1 : 0;
+  *ok = fold_stages(f1, &f2, P4V_FOLD_MLP | P4V_FOLD_NORM) ? 1 : 0;
   return 0;
 }
 
 extern "C" int p4v_linear_frozen_forward_norm(const p4v_linear_desc* d, const float* x, const float* gamma, const float* beta,
-                                              float eps, const float* bias, const void* packed_in, float* out, void* stream) {
+                                              float eps, const float* bias, const void* packed, float* out, void* stream) {
   FrozenPlan f; int rc = build_frozen(d, f, false);
   if (rc) return rc;
-  return fused_forward<FwdNormParams>("linear_frozen_forward_norm", f, x, FwdNorm{gamma, beta, eps}, FwdResidual{}, nullptr,
-                                      bias, packed_in, 0, nullptr, nullptr, nullptr, 0, nullptr, 0, out, (cudaStream_t)stream);
+  const FwdNorm ln{gamma, beta, eps};
+  FrozenCall c = linear_call(f, x, bias, packed, out);
+  c.ln = &ln;
+  return frozen_call("linear_frozen_forward_norm", c, (cudaStream_t)stream);
 }
 
 extern "C" int p4v_mlp_frozen_forward_norm(const p4v_linear_desc* fc1, const float* x, const float* gamma, const float* beta,
@@ -1070,9 +1081,10 @@ extern "C" int p4v_mlp_frozen_forward_norm(const p4v_linear_desc* fc1, const flo
                                            void* workspace, size_t workspace_bytes, float* out, void* stream) {
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
-  return fused_forward<FwdMlpNormParams>("mlp_frozen_forward_norm", f1, x, FwdNorm{gamma, beta, eps}, FwdResidual{},
-                                         nullptr, bias1, pack1, pack1_bytes, &f2, bias2, pack2, pack2_bytes, workspace,
-                                         workspace_bytes, out, (cudaStream_t)stream);
+  const FwdNorm ln{gamma, beta, eps};
+  FrozenCall c = mlp_call(f1, x, bias1, pack1, pack1_bytes, f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out);
+  c.ln = &ln;
+  return frozen_call("mlp_frozen_forward_norm", c, (cudaStream_t)stream);
 }
 
 // ---- a block's residual add folded into the store of the frozen Linear that produces it (DESIGN §4.11) -------------
@@ -1082,8 +1094,12 @@ extern "C" int p4v_linear_frozen_forward_res(const p4v_linear_desc* d, const flo
                                              void* workspace, size_t workspace_bytes, const float* residual,
                                              const p4v_window_layout* layout, float* out, void* stream) {
   P4V_REQUIRE(residual, "linear_frozen_forward_res: null pointer");
-  return frozen_forward("linear_frozen_forward_res", d, x, bias, packed, workspace, workspace_bytes,
-                        FwdResidual{residual, layout ? *layout : p4v_window_layout{}}, out, (cudaStream_t)stream);
+  FrozenPlan f; int rc = build_frozen(d, f, false);
+  if (rc) return rc;
+  FrozenCall c = linear_call(f, x, bias, packed, out);
+  c.workspace = workspace; c.workspace_bytes = workspace_bytes;
+  c.rs = FwdResidual{residual, layout ? *layout : p4v_window_layout{}};
+  return frozen_call("linear_frozen_forward_res", c, (cudaStream_t)stream);
 }
 
 extern "C" int p4v_mlp_frozen_forward_res(const p4v_linear_desc* fc1, const float* x, const float* bias1, const void* pack1,
@@ -1093,9 +1109,9 @@ extern "C" int p4v_mlp_frozen_forward_res(const p4v_linear_desc* fc1, const floa
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
   P4V_REQUIRE(residual, "mlp_frozen_forward_res: null pointer");
-  return fused_forward<FwdMlpParams>("mlp_frozen_forward_res", f1, x, FwdNorm{}, FwdResidual{residual, {}}, nullptr, bias1,
-                                     pack1, pack1_bytes, &f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out,
-                                     (cudaStream_t)stream);
+  FrozenCall c = mlp_call(f1, x, bias1, pack1, pack1_bytes, f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out);
+  c.rs.res = residual;
+  return frozen_call("mlp_frozen_forward_res", c, (cudaStream_t)stream);
 }
 
 extern "C" int p4v_mlp_frozen_forward_norm_res(const p4v_linear_desc* fc1, const float* x, const float* gamma, const float* beta,
@@ -1106,9 +1122,10 @@ extern "C" int p4v_mlp_frozen_forward_norm_res(const p4v_linear_desc* fc1, const
   FrozenPlan f1, f2; int rc = build_mlp(fc1, fc2, f1, f2, false);
   if (rc) return rc;
   P4V_REQUIRE(residual, "mlp_frozen_forward_norm_res: null pointer");
-  return fused_forward<FwdMlpNormParams>("mlp_frozen_forward_norm_res", f1, x, FwdNorm{gamma, beta, eps},
-                                         FwdResidual{residual, {}}, nullptr, bias1, pack1, pack1_bytes, &f2, bias2, pack2,
-                                         pack2_bytes, workspace, workspace_bytes, out, (cudaStream_t)stream);
+  const FwdNorm ln{gamma, beta, eps};
+  FrozenCall c = mlp_call(f1, x, bias1, pack1, pack1_bytes, f2, bias2, pack2, pack2_bytes, workspace, workspace_bytes, out);
+  c.ln = &ln; c.rs.res = residual;
+  return frozen_call("mlp_frozen_forward_norm_res", c, (cudaStream_t)stream);
 }
 
 // ---- a row gather in front of the LayerNorm folded into its frozen Linear (DESIGN §4.12) ---------------------------
@@ -1119,7 +1136,7 @@ extern "C" int p4v_linear_gather_ok(const p4v_linear_desc* d, const p4v_input_ga
   P4V_REQUIRE(g && ok, "null argument");
   P4V_REQUIRE(g->mode == P4V_GATHER_WINDOW || g->mode == P4V_GATHER_MERGE,
               "linear_gather_ok: gather mode must be P4V_GATHER_WINDOW or P4V_GATHER_MERGE (got %d)", g->mode);
-  *ok = gather_stages(f, g->mode) ? 1 : 0;
+  *ok = fold_stages(f, nullptr, P4V_FOLD_NORM | P4V_FOLD_GATHER, g->mode) ? 1 : 0;
   return 0;
 }
 
@@ -1128,7 +1145,8 @@ extern "C" int p4v_linear_frozen_forward_norm_gather(const p4v_linear_desc* d, c
                                                      const p4v_input_gather* g, float* out, void* stream) {
   FrozenPlan f; int rc = build_frozen(d, f, false);
   if (rc) return rc;
-  return fused_forward<FwdGatherParams>("linear_frozen_forward_norm_gather", f, x, FwdNorm{gamma, beta, eps}, FwdResidual{},
-                                        g, bias, packed, 0, nullptr, nullptr, nullptr, 0, nullptr, 0, out,
-                                        (cudaStream_t)stream);
+  const FwdNorm ln{gamma, beta, eps};
+  FrozenCall c = linear_call(f, x, bias, packed, out);
+  c.ln = &ln; c.gather = true; c.ga = g;
+  return frozen_call("linear_frozen_forward_norm_gather", c, (cudaStream_t)stream);
 }

@@ -225,12 +225,29 @@ class MinMaxQuantLinear(nn.Linear):
         return out
 
 
-def _rule(fn, *layers):
-    """A shape rule of the library (an int written through its last argument) over the layers' descriptors; the rules
-    ignore the rows."""
+def _rule(fn, *layers, extra=()):
+    """A shape rule of the library (an int written through its last argument) over the layers' descriptors and the
+    ctypes structures `extra`, all by reference; the rules ignore the rows."""
     ok = ctypes.c_int()
-    _lib.check(getattr(_lib.lib(), fn)(*[ctypes.byref(m._desc(1, 1)) for m in layers], ctypes.byref(ok)), fn)
+    args = [ctypes.byref(m._desc(1, 1)) for m in layers] + [ctypes.byref(a) for a in extra]
+    _lib.check(getattr(_lib.lib(), fn)(*args, ctypes.byref(ok)), fn)
     return bool(ok.value)
+
+
+def _frozen_quant_forward(m):
+    """m is a frozen Linear layer in quant_forward mode"""
+    return isinstance(m, MinMaxQuantLinear) and m.frozen and m.mode == "quant_forward"
+
+
+def _wants_no_grad(tensors, modules):
+    """Under grad mode no tensor and no parameter of the modules requires grad (else the unfused call has a grad_fn)"""
+    return not (torch.is_grad_enabled() and (any(t.requires_grad for t in tensors) or
+                                             any(p.requires_grad for m in modules for p in m.parameters())))
+
+
+def _window_layout_ok(height, width, window, shift):
+    """Swin's window rule: windows tile the image and the shift lies inside one"""
+    return window > 0 and height % window == 0 and width % window == 0 and 0 <= shift < window
 
 
 def _streamed_image(lin, dev, fn, *descs):
@@ -309,13 +326,11 @@ def frozen_mlp_applies(fc1, fc2, act, x):
     no input and no parameter of the layers that requires grad (the unfused call then carries a grad_fn), and a shape the
     kernel holds (p4v_mlp_fused_ok: fc1.out_features == fc2.in_features, fc1 not post-GELU and on its fused kernel, the
     shared-memory plan fits)."""
-    if not all(isinstance(m, MinMaxQuantLinear) and m.frozen and m.mode == "quant_forward" for m in (fc1, fc2)):
+    if not (_frozen_quant_forward(fc1) and _frozen_quant_forward(fc2)):
         return False
     if type(act) is not nn.GELU or act.approximate != "none":
         return False
-    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in (fc1, fc2) for p in m.parameters())):
-        return False
-    return _rule("p4v_mlp_fused_ok", fc1, fc2)
+    return _wants_no_grad((x,), (fc1, fc2)) and _rule("p4v_mlp_fused_ok", fc1, fc2)
 
 
 def frozen_mlp(fc1, fc2, x, norm=None, residual=None):
@@ -335,7 +350,7 @@ def frozen_residual_applies(lin, x, residual, layout=None):
     FP32 tensor on lin's device, contiguous, 8-byte aligned, with the output's shape (with a layout: its number of rows
     and lin's out_features per row), under grad mode nothing that requires grad, and a layout only for a layer on its
     fused path (the streamed path adds in identity rows only).  x is the input of the call: lin's, or fc1's of the MLP."""
-    if not (isinstance(lin, MinMaxQuantLinear) and lin.frozen and lin.mode == "quant_forward"):
+    if not _frozen_quant_forward(lin):
         return False
     dev = lin._packed.device
     if not torch.is_tensor(residual) or residual.dtype != torch.float32 or residual.device != dev:
@@ -350,12 +365,9 @@ def frozen_residual_applies(lin, x, residual, layout=None):
         images, height, width, window, shift = (int(v) for v in layout)
         if not lin._frozen_fused or residual.shape[-1] != lin.out_features or residual.numel() != rows * lin.out_features:
             return False
-        if not (window > 0 and height % window == 0 and width % window == 0 and 0 <= shift < window and
-                images * height * width == rows):
+        if not (_window_layout_ok(height, width, window, shift) and images * height * width == rows):
             return False
-    if torch.is_grad_enabled() and (x.requires_grad or residual.requires_grad or any(p.requires_grad for p in lin.parameters())):
-        return False
-    return True
+    return _wants_no_grad((x, residual), (lin,))
 
 
 def frozen_residual_linear(lin, x, residual, layout=None):
@@ -389,7 +401,7 @@ def _layer_norm_ok(norm, features, dev):
 
 def _norm_call_ok(norm, lin, x):
     """frozen_norm_applies without the library's shape rule"""
-    if not (isinstance(lin, MinMaxQuantLinear) and lin.frozen and lin.mode == "quant_forward"):
+    if not _frozen_quant_forward(lin):
         return False
     dev = lin._packed.device
     if not _layer_norm_ok(norm, lin.in_features, dev):
@@ -398,9 +410,7 @@ def _norm_call_ok(norm, lin, x):
         return False
     if x.is_contiguous() and x.data_ptr() % 16:       # torch normalises a non-contiguous x from an aligned copy
         return False
-    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in (norm, lin) for p in m.parameters())):
-        return False
-    return True
+    return _wants_no_grad((x,), (norm, lin))
 
 
 def frozen_mlp_norm_ok(fc1, fc2):
@@ -419,11 +429,7 @@ def frozen_norm_linear(norm, lin, x):
 def frozen_gather_ok(lin, mode):
     """The library's shape rule of a row gather (p4v_linear_gather_ok) for lin, mode "window" or "merge":
     p4v_linear_norm_ok, in_features % 16 == 0 for the merge, the shared-memory plan with the table of source rows fits."""
-    ok = ctypes.c_int()
-    g = _gather_desc((mode, 0, 0, 0, 0, 0))
-    _lib.check(_lib.lib().p4v_linear_gather_ok(ctypes.byref(lin._desc(1, 1)), ctypes.byref(g), ctypes.byref(ok)),
-               "p4v_linear_gather_ok")
-    return bool(ok.value)
+    return _rule("p4v_linear_gather_ok", lin, extra=(_gather_desc((mode, 0, 0, 0, 0, 0)),))
 
 
 def frozen_gather_applies(norm, lin, x, gather):
@@ -440,7 +446,7 @@ def frozen_gather_applies(norm, lin, x, gather):
     if x.dim() < 2 or x.shape[-1] != C or x.numel() != images * height * width * C or images <= 0:
         return False
     if mode == "window":
-        if not (window > 0 and height % window == 0 and width % window == 0 and 0 <= shift < window):
+        if not _window_layout_ok(height, width, window, shift):
             return False
     elif not (window == 0 and shift == 0 and height % 2 == 0 and width % 2 == 0 and lin.in_features == 4 * C):
         return False
