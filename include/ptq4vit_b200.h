@@ -331,6 +331,43 @@ P4V_API int p4v_linear_frozen_forward_norm_gather(const p4v_linear_desc* d, cons
                                                   const float* beta, float eps, const float* bias, const void* packed,
                                                   const p4v_input_gather* g, float* out, void* stream);
 
+/* The attention operands' quantisation folded into the frozen qkv Linear of an attention block whose matmul1 and matmul2
+ * are frozen: the qkv kernel's epilogue quantises its output with the step sizes of the attention's operands and writes
+ * int8 planes instead of the FP32 output, and the short attention kernel reads those planes instead of quantising q, k and
+ * v from FP32.  Output row r = b * N + n and column c of qkv (torch's reshape(batch, N, 3, heads, head_dim)) go to
+ *   planes[part][b][h][n][j]   ([3][batch][heads][N][head_dim] int8, contiguous), part = c / C, h = (c % C) / head_dim,
+ *                              j = c % head_dim, C = heads * head_dim
+ * as clamp(rne(y / delta), lo, hi) with, for q, y = fl(value * (float)scale) when scale_on_q and the value otherwise,
+ * matmul1's A step size of head h; for k matmul1's B step size; for v matmul2's B step size -- the bytes the attention
+ * kernel of p4v_attention_frozen_forward makes of them.  p4v_linear_frozen_forward_qkv8 followed by
+ * p4v_attention_frozen_forward_i8 is bit-identical to p4v_linear_frozen_forward (or its LayerNorm / gather variants)
+ * followed by p4v_attention_frozen_forward, and qkv's FP32 output never reaches HBM.
+ * p4v_linear_qkv8_ok is the shape rule, a pure function of the descriptors without their rows: out_features == 3 heads
+ * head_dim, p4v_attention_fused_ok(tokens, head_dim), the layer on its fused path (p4v_linear_frozen_path 1; a streamed
+ * qkv never folds) and the shared-memory plan with the epilogue's staging fits beside a two-stage weight ring -- with the
+ * LayerNorm's row statistics too when the layer can take a LayerNorm (p4v_linear_norm_ok's conditions), so the rule
+ * holds with and without one.  gather_mode: 0, or P4V_GATHER_WINDOW for a call with a window gather (and the rule of
+ * p4v_linear_gather_ok).
+ * p4v_linear_frozen_forward_qkv8: qkv's descriptor (rows = batch * tokens), x, bias and pack as for
+ * p4v_linear_frozen_forward; the attention descriptor and matmul1's and matmul2's descriptors and packs as for
+ * p4v_attention_frozen_forward; planes (16-byte aligned, 3 * rows * C bytes); an optional LayerNorm (gamma, beta, eps as
+ * p4v_linear_frozen_forward_norm; gamma null = none) and an optional window gather (g null = none; with the LayerNorm, as
+ * p4v_linear_frozen_forward_norm_gather).  p4v_attention_frozen_forward_i8 takes the planes in place of qkv and its
+ * strides, and otherwise the arguments of p4v_attention_frozen_forward (N <= 256).  Both validate every argument before
+ * their one launch: null pointers, alignment, heads and head_dim against the descriptors, pack sizes, a split-of-softmax
+ * matmul1 (refused), the rule, and x or out overlapping the planes.  Neither allocates, copies or synchronises: both can
+ * be captured in a CUDA graph. */
+P4V_API int p4v_linear_qkv8_ok(const p4v_linear_desc* d, const p4v_attention_desc* a, int gather_mode, int* ok);
+P4V_API int p4v_linear_frozen_forward_qkv8(const p4v_linear_desc* d, const float* x, const float* bias, const void* packed,
+                                           const p4v_attention_desc* a, const p4v_matmul_desc* mm1, const void* pack1,
+                                           size_t pack1_bytes, const p4v_matmul_desc* mm2, const void* pack2,
+                                           size_t pack2_bytes, int8_t* planes, const float* gamma, const float* beta,
+                                           float eps, const p4v_input_gather* g, void* stream);
+P4V_API int p4v_attention_frozen_forward_i8(const p4v_attention_desc* a, const int8_t* planes, const p4v_matmul_desc* mm1,
+                                            const void* pack1, size_t pack1_bytes, const p4v_matmul_desc* mm2,
+                                            const void* pack2, size_t pack2_bytes, const float* bias, const float* mask,
+                                            float* out, void* stream);
+
 /* The patch-embedding convolution: ChannelwiseBatchingQuantConv2d with a_bit >= 32 (quant_layers/conv.py:444-614, wired
  * by configs/PTQ4ViT.py:52-54): one weight step size per output channel, activations left in FP32.  The caller passes
  * the im2col matrix of the FP32 input (torch.nn.functional.unfold, [images, positions, K], K = in_channels*kh*kw in the

@@ -104,6 +104,12 @@ _SIGNATURES = {
                                         _P, _P, C.c_size_t, _P, C.c_size_t, _P, _P, _P],
     "p4v_linear_gather_ok": [C.POINTER(LinearDesc), C.POINTER(InputGather), C.POINTER(C.c_int)],
     "p4v_linear_frozen_forward_norm_gather": [C.POINTER(LinearDesc), _P, _P, _P, C.c_float, _P, _P, C.POINTER(InputGather), _P, _P],
+    "p4v_linear_qkv8_ok": [C.POINTER(LinearDesc), C.POINTER(AttentionDesc), C.c_int, C.POINTER(C.c_int)],
+    "p4v_linear_frozen_forward_qkv8": [C.POINTER(LinearDesc), _P, _P, _P, C.POINTER(AttentionDesc), C.POINTER(MatMulDesc), _P,
+                                       C.c_size_t, C.POINTER(MatMulDesc), _P, C.c_size_t, _P, _P, _P, C.c_float,
+                                       C.POINTER(InputGather), _P],
+    "p4v_attention_frozen_forward_i8": [C.POINTER(AttentionDesc), _P, C.POINTER(MatMulDesc), _P, C.c_size_t, C.POINTER(MatMulDesc),
+                                        _P, C.c_size_t, _P, _P, _P, _P],
     "p4v_conv_workspace_bytes": [C.POINTER(ConvDesc), C.POINTER(C.c_size_t)],
     "p4v_conv_calibrate": [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, C.c_size_t, _P, _P, _P],
     "p4v_conv_frozen_ok": [C.POINTER(ConvFrozenDesc), C.POINTER(C.c_int)],

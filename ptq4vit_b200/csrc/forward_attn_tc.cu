@@ -25,6 +25,9 @@
 // The key axis is padded to 64 (zero key rows and zero v rows: padded probabilities meet zero v bytes), the head
 // dimension to 32 for matmul1 and 64 for matmul2 (zero bytes).  Shared memory is a function of the padded key length:
 // 112 KiB at 256 keys with split-of-softmax, so two CTAs share an SM.
+// The int8 variant (I8, DESIGN §4.14) reads q, k and v as the bytes the qkv Linear's epilogue already quantised with the
+// same quantisers (FwdQkv8): step 1 copies the q tile and the keys as 16-byte chunks and transposes v's bytes; steps 2-4
+// are the same code.
 #include "forward.cuh"
 #include "sm90.cuh"
 #include <climits>
@@ -46,7 +49,7 @@ __host__ __device__ inline AttnLayout attn_layout(int sp, int kd, bool sos) {
   return L;
 }
 
-template <bool SOS>
+template <bool SOS, bool I8>
 __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_constant__ FwdAttnParams P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
@@ -72,53 +75,84 @@ __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_
   uint8_t* sV = smem + L.v;
   float* sS = reinterpret_cast<float*>(smem + L.s);
 
-  // ---- 1. operands: lanes along d for q and k (a warp reads whole 128-byte row segments), v transposed in registers
+  if constexpr (I8) {
+    // ---- 1. operands from the planes [3][batch][heads][N][D]: a thread copies one 16-byte chunk of a q or key row, or
+    // gathers one column d of a 16-key chunk of v (64 threads read 64 consecutive bytes of a row)
+    const long long plane = (long long)P.batch * P.heads * P.N * P.D;
+    const uint8_t* q8 = P.planes + ((long long)img * P.heads + h) * P.N * P.D;
+    const uint8_t* k8 = q8 + plane;
+    const uint8_t* v8 = q8 + 2 * plane;
+    const int nc = P.D / 16;
 #pragma unroll 1
-  for (int j = 0; j < P.kd / 32; ++j) {
-    const int d = lane + 32 * j;
-    float x[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int r = warp + 8 * i;
-      x[i] = (r < rows && d < P.D) ? __ldg(q + (long long)(row0 + r) * P.s_n + d) : 0.f;
+    for (int u = threadIdx.x; u < (P.kd / 16) * kRows; u += kThreads) {
+      const int c = u / kRows, r = u % kRows;
+      *reinterpret_cast<uint4*>(sQ + (c * kRows + r) * 16) =
+          (r < rows && c < nc) ? __ldg(reinterpret_cast<const uint4*>(q8 + (long long)(row0 + r) * P.D) + c) : make_uint4(0u, 0u, 0u, 0u);
     }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int r = warp + 8 * i;
-      const float xs = P.scale_on_q ? __fmul_rn(x[i], P.scale) : x[i];
-      sQ[((d >> 4) * kRows + r) * 16 + (d & 15)] =
-          (uint8_t)((r < rows && d < P.D) ? p4v_qbyte(p4v_quant_plain(xs, dA1, fA1, rA1, false, 0.f, P.A1_lo, P.A1_hi)) : 0u);
-    }
-  }
 #pragma unroll 1
-  for (int pass = 0; pass < (P.sp / 64) * (P.kd / 32); ++pass) {
-    const int j = pass % (P.kd / 32), n0 = 64 * (pass / (P.kd / 32));
-    const int d = lane + 32 * j;
-    float x[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int n = n0 + warp + 8 * i;
-      x[i] = (n < P.N && d < P.D) ? __ldg(k + (long long)n * P.s_n + d) : 0.f;
+    for (int u = threadIdx.x; u < (P.kd / 16) * P.sp; u += kThreads) {
+      const int c = u / P.sp, n = u % P.sp;
+      *reinterpret_cast<uint4*>(sK + (c * P.sp + n) * 16) =
+          (n < P.N && c < nc) ? __ldg(reinterpret_cast<const uint4*>(k8 + (long long)n * P.D) + c) : make_uint4(0u, 0u, 0u, 0u);
     }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int n = n0 + warp + 8 * i;
-      sK[((d >> 4) * P.sp + n) * 16 + (d & 15)] =
-          (uint8_t)((n < P.N && d < P.D) ? p4v_qbyte(p4v_quant_plain(x[i], dB1, fB1, rB1, false, 0.f, P.B1_lo, P.B1_hi)) : 0u);
-    }
-  }
 #pragma unroll 1
-  for (int u = threadIdx.x; u < 4 * P.sp; u += kThreads) {     // one thread = one column d x one 16-key chunk
-    const int d = u % 64, kb = 16 * (u / 64);
-    float x[16];
+    for (int u = threadIdx.x; u < 4 * P.sp; u += kThreads) {
+      const int d = u % 64, kb = 16 * (u / 64);
+      uint32_t w[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
-    for (int e = 0; e < 16; ++e)
-      x[e] = (d < P.D && kb + e < P.N) ? __ldg(v + (long long)(kb + e) * P.s_n + d) : 0.f;
-    uint32_t w[4] = {0u, 0u, 0u, 0u};
+      for (int e = 0; e < 16; ++e)
+        if (d < P.D && kb + e < P.N) w[e >> 2] |= (uint32_t)__ldg(v8 + (long long)(kb + e) * P.D + d) << ((e & 3) * 8);
+      *reinterpret_cast<uint4*>(sV + (kb / 16 * 64 + d) * 16) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+  } else {
+    // ---- 1. operands: lanes along d for q and k (a warp reads whole 128-byte row segments), v transposed in registers
+#pragma unroll 1
+    for (int j = 0; j < P.kd / 32; ++j) {
+      const int d = lane + 32 * j;
+      float x[8];
 #pragma unroll
-    for (int e = 0; e < 16; ++e)
-      if (d < P.D && kb + e < P.N) w[e >> 2] |= p4v_qbyte(p4v_quant_plain(x[e], dB2, fB2, rB2, false, 0.f, P.B2_lo, P.B2_hi)) << ((e & 3) * 8);
-    *reinterpret_cast<uint4*>(sV + (kb / 16 * 64 + d) * 16) = make_uint4(w[0], w[1], w[2], w[3]);
+      for (int i = 0; i < 8; ++i) {
+        const int r = warp + 8 * i;
+        x[i] = (r < rows && d < P.D) ? __ldg(q + (long long)(row0 + r) * P.s_n + d) : 0.f;
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int r = warp + 8 * i;
+        const float xs = P.scale_on_q ? __fmul_rn(x[i], P.scale) : x[i];
+        sQ[((d >> 4) * kRows + r) * 16 + (d & 15)] =
+            (uint8_t)((r < rows && d < P.D) ? p4v_qbyte(p4v_quant_plain(xs, dA1, fA1, rA1, false, 0.f, P.A1_lo, P.A1_hi)) : 0u);
+      }
+    }
+#pragma unroll 1
+    for (int pass = 0; pass < (P.sp / 64) * (P.kd / 32); ++pass) {
+      const int j = pass % (P.kd / 32), n0 = 64 * (pass / (P.kd / 32));
+      const int d = lane + 32 * j;
+      float x[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int n = n0 + warp + 8 * i;
+        x[i] = (n < P.N && d < P.D) ? __ldg(k + (long long)n * P.s_n + d) : 0.f;
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int n = n0 + warp + 8 * i;
+        sK[((d >> 4) * P.sp + n) * 16 + (d & 15)] =
+            (uint8_t)((n < P.N && d < P.D) ? p4v_qbyte(p4v_quant_plain(x[i], dB1, fB1, rB1, false, 0.f, P.B1_lo, P.B1_hi)) : 0u);
+      }
+    }
+#pragma unroll 1
+    for (int u = threadIdx.x; u < 4 * P.sp; u += kThreads) {     // one thread = one column d x one 16-key chunk
+      const int d = u % 64, kb = 16 * (u / 64);
+      float x[16];
+#pragma unroll
+      for (int e = 0; e < 16; ++e)
+        x[e] = (d < P.D && kb + e < P.N) ? __ldg(v + (long long)(kb + e) * P.s_n + d) : 0.f;
+      uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+      for (int e = 0; e < 16; ++e)
+        if (d < P.D && kb + e < P.N) w[e >> 2] |= p4v_qbyte(p4v_quant_plain(x[e], dB2, fB2, rB2, false, 0.f, P.B2_lo, P.B2_hi)) << ((e & 3) * 8);
+      *reinterpret_cast<uint4*>(sV + (kb / 16 * 64 + d) * 16) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
   }
   fence_proxy_async();   // generic-proxy stores -> wgmma (async proxy) reads
   __syncthreads();
@@ -230,7 +264,7 @@ __global__ void __launch_bounds__(kThreads, 2) forward_attn_kernel(const __grid_
   }
 }
 
-template <bool SOS>
+template <bool SOS, bool I8>
 int launch(const FwdAttnParams& p_in, cudaStream_t st) {
   FwdAttnParams p = p_in;
   p.sp = (p.N + 63) / 64 * 64;
@@ -238,8 +272,8 @@ int launch(const FwdAttnParams& p_in, cudaStream_t st) {
   const int smem = (int)p4v_attn_smem_bytes(p.sp, p.kd, SOS);
   const long long ctas = (long long)p.batch * p.heads * p4v_cdiv(p.N, kRows);
   P4V_REQUIRE(ctas <= INT_MAX, "attention_frozen_forward: grid too large (%lld tiles)", ctas);
-  P4V_CUDA_OK(cudaFuncSetAttribute(forward_attn_kernel<SOS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  forward_attn_kernel<SOS><<<(unsigned)ctas, kThreads, smem, st>>>(p);
+  P4V_CUDA_OK(cudaFuncSetAttribute(forward_attn_kernel<SOS, I8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  forward_attn_kernel<SOS, I8><<<(unsigned)ctas, kThreads, smem, st>>>(p);
   p4v_count_launch();
   P4V_CUDA_OK(cudaGetLastError());
   return 0;
@@ -249,6 +283,7 @@ int launch(const FwdAttnParams& p_in, cudaStream_t st) {
 
 size_t p4v_attn_smem_bytes(int sp, int kd, bool sos) { return (size_t)attn_layout(sp, kd, sos).total + 128; }
 
-int p4v_launch_forward_attn_tc(const FwdAttnParams& p, bool sos, cudaStream_t st) {
-  return sos ? launch<true>(p, st) : launch<false>(p, st);
+int p4v_launch_forward_attn_tc(const FwdAttnParams& p, bool sos, cudaStream_t st, bool i8) {
+  if (i8) return sos ? launch<true, true>(p, st) : launch<false, true>(p, st);
+  return sos ? launch<true, false>(p, st) : launch<false, false>(p, st);
 }

@@ -26,7 +26,10 @@
 //   identity, or Swin's window reverse and reverse shift, p4v_window_row) as fl(value + shortcut) (DESIGN §4.11).
 // P4V_FOLD_GATHER (with NORM): the LayerNorm prologue and the quantise loop read each row from elsewhere in an image:
 //   Swin's shifted window partition (p4v_window_row) or PatchMerging's 2x2 neighbourhood (p4v_merge_row) (DESIGN §4.12).
-// p4v_launch_forward_tc instantiates the six fold sets the host uses: none, MLP, NORM, MLP|NORM, RES and NORM|GATHER.
+// P4V_FOLD_QKV8: the layer is an attention block's qkv; the epilogue quantises q, k and v with the attention's step sizes
+//   and stores them as the int8 planes the attention kernel reads, instead of the FP32 output (DESIGN §4.14).
+// p4v_launch_forward_tc instantiates the nine fold sets the host uses: none, MLP, NORM, MLP|NORM, RES, NORM|GATHER, QKV8,
+// NORM|QKV8 and NORM|GATHER|QKV8.
 // 288 threads leave 224 registers per thread without setmaxnreg; the bounded mbarrier wait is inline, and the k32 steps of
 // a stage are one straight-line batch selected by a warp-uniform count (ptxas C7520, see sm90.cuh).
 #include "../../include/ptq4vit_b200.h"
@@ -166,8 +169,8 @@ __device__ __forceinline__ float* ln_stats(const FwdParams& P, unsigned folds, u
 
 // ---- the row gather of P4V_FOLD_GATHER (DESIGN §4.12) ----------------------------------------------------------------
 // The source row of each tile row, right below the row stats: the window map's image row, or the merge's first row
-__device__ __forceinline__ int* gather_rows(const FwdParams& P, uint8_t* smem) {
-  return reinterpret_cast<int*>(ln_stats(P, P4V_FOLD_NORM | P4V_FOLD_GATHER, smem)) - P4V_TILE;
+__device__ __forceinline__ int* gather_rows(const FwdParams& P, unsigned folds, uint8_t* smem) {
+  return reinterpret_cast<int*>(ln_stats(P, folds, smem)) - P4V_TILE;
 }
 
 // Mean and rstd of tile row r (global row `row`), read from its source rows; returns the source row
@@ -218,6 +221,68 @@ __device__ __forceinline__ void gather_chunk(const FwdParams& P, int s, int k0, 
   }
 }
 
+// ---- the qkv epilogue of P4V_FOLD_QKV8 (DESIGN §4.14) ---------------------------------------------------------------
+// Shared memory, in the place of the MLP epilogue's: [staged bytes: 128 rows x P4V_MLP_STAGE_LD][a Qkv8Group per 16-column
+// group of the column tile].  A 16-byte chunk of a plane row is one 16-column group of one output row of one column tile,
+// so every byte of the planes has exactly one owner and is stored in a whole 16-byte store.
+struct Qkv8Group { float d, rcp, lo, hi; int scaled, pad; long long off; };   // off: planes + off + (b * heads * N + n) * D
+__device__ __forceinline__ Qkv8Group* qkv8_groups(uint8_t* epi) {
+  return reinterpret_cast<Qkv8Group*>(epi + P4V_TILE * P4V_MLP_STAGE_LD);
+}
+
+// The step size, reciprocal, clamp range, q-scaling and (part, head, j) offset of each 16-column group of tile tn, by the
+// consumers between the barriers that open a column tile
+__device__ __forceinline__ void qkv8_column_groups(const FwdParams& P, uint8_t* epi, int tn, int et) {
+  if (et >= P4V_TILE / 16) return;
+  const FwdQkv8& Q = P.q8;
+  const int c = tn * P4V_TILE + 16 * et;
+  Qkv8Group g{1.f, 1.f, 0.f, 0.f, 0, 0, 0};
+  if (c < P.N) {
+    const int part = c / Q.C, h = (c - part * Q.C) / Q.D, j = c - part * Q.C - h * Q.D;
+    g.d = __ldg((part == 0 ? Q.dq : part == 1 ? Q.dk : Q.dv) + h);
+    g.rcp = p4v_rint_div_ok(g.d) ? __frcp_rn(g.d) : 0.f;
+    g.lo = part == 0 ? Q.q_lo : part == 1 ? Q.k_lo : Q.v_lo;
+    g.hi = part == 0 ? Q.q_hi : part == 1 ? Q.k_hi : Q.v_hi;
+    g.scaled = part == 0 && Q.scale_on_q;
+    g.off = ((long long)part * Q.batch * Q.heads + h) * Q.N * Q.D + j;     // [part][b = 0][h][n = 0][j]
+  }
+  qkv8_groups(epi)[et] = g;
+}
+
+// The thread's 64 qkv values (r = -value, fragment layout of forward_tc_body) -> the attention kernel's bytes, staged by
+// column: p4v_qbyte(p4v_quant_plain(...)) with the arguments of forward_attn_tc.cu's loaders
+__device__ __forceinline__ void qkv8_stage_tile(const FwdParams& P, uint8_t* epi, const float (&r)[64], int frow, int fcol) {
+  const Qkv8Group* grp = qkv8_groups(epi);
+#pragma unroll
+  for (int v = 0; v < 64; v += 2) {
+    const int row = frow + 8 * ((v >> 1) & 1), lc = fcol + 8 * (v >> 2);
+    const Qkv8Group g = grp[lc >> 4];
+    uint32_t b = 0u;
+#pragma unroll
+    for (int t = 0; t < 2; ++t) {
+      const float y = -r[v + t];
+      const float xs = g.scaled ? __fmul_rn(y, P.q8.scale) : y;
+      b |= p4v_qbyte(p4v_quant_plain(xs, g.d, p4v_rint_div_ok(g.d), g.rcp, false, 0.f, g.lo, g.hi)) << (8 * t);
+    }
+    *reinterpret_cast<uint16_t*>(epi + row * P4V_MLP_STAGE_LD + lc) = (uint16_t)b;
+  }
+}
+
+// The planes' 16-byte chunks of row tile tm and column tile tn from the staged tile: one (row, 16-column group) per
+// item, groups fastest, so that a warp stores whole runs of a head's rows
+__device__ __forceinline__ void qkv8_store_tile(const FwdParams& P, uint8_t* epi, int tm, int tn, int et) {
+  const FwdQkv8& Q = P.q8;
+  const Qkv8Group* grp = qkv8_groups(epi);
+  const int ng = min(P4V_TILE, P.N - tn * P4V_TILE) / 16;
+  for (int u = et; u < P4V_TILE * (P4V_TILE / 16); u += kConsumers) {
+    const int g = u & 7, r = u >> 3, row = tm * P4V_TILE + r;
+    if (g >= ng || row >= P.M) continue;
+    const int b = row / Q.N, n = row - b * Q.N;
+    uint8_t* dst = Q.planes + grp[g].off + ((long long)b * Q.heads * Q.N + n) * Q.D;
+    *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(epi + r * P4V_MLP_STAGE_LD + 16 * g);
+  }
+}
+
 // kFolds = 0: the frozen Linear forward, FP32 output.  P4V_FOLD_MLP: fc1 of a frozen MLP, GELU-and-quantise epilogue
 // into fc2's image.  P4V_FOLD_NORM: a LayerNorm prologue.  P4V_FOLD_RES: the plain forward whose store adds the
 // shortcut.  P4V_FOLD_GATHER (with NORM): the LayerNorm's rows gathered from an image.
@@ -246,7 +311,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
       float mean, rstd;
       if constexpr ((kFolds & P4V_FOLD_GATHER) != 0) {
         const int s = gather_row_stats(P, row, lane, mean, rstd);
-        if (lane == 0) gather_rows(P, smem)[r] = s;
+        if (lane == 0) gather_rows(P, kFolds, smem)[r] = s;
       } else {
         p4v_ln_row_stats(P.x + (size_t)row * P.ld, (int)P.ld, P.ln.eps, lane, mean, rstd);
       }
@@ -281,7 +346,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
       if (row < P.M && ch.n > 0) {
         float vals[16];
         if constexpr ((kFolds & P4V_FOLD_GATHER) != 0) {
-          gather_chunk(P, gather_rows(P, smem)[r], ch.k0, ch.n, vals);
+          gather_chunk(P, gather_rows(P, kFolds, smem)[r], ch.k0, ch.n, vals);
         } else {
           const float* src = P.x + (size_t)row * P.ld + ch.k0;
           if (ch.n == 16 && ((P.ld | ch.k0) & 3) == 0) {
@@ -377,6 +442,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
     for (int i = et; i < P.n_groups * P4V_TILE_CG; i += kConsumers)
       S.scale[i >> 3][i & 7] = P.scale[(size_t)(i >> 3) * P.nsg + tn * P4V_TILE_CG + (i & 7)];
     if constexpr (kMlp) mlp_column_steps(P, mlp_epi(P, smem), tn, et);
+    if constexpr ((kFolds & P4V_FOLD_QKV8) != 0) qkv8_column_groups(P, mlp_epi(P, smem), tn, et);
     const int gc = tn * P4V_TILE + fcol;               // global columns gc + 8 * i + {0, 1}
 #pragma unroll
     for (int v = 0; v < 64; ++v) {
@@ -411,6 +477,11 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(const __grid_co
       asm volatile("bar.sync 1, %0;" ::"n"(kConsumers));   // staged tile complete
       // the next column tile's first barrier orders these reads of the staging before it is written again
       mlp_store_tile(P, mlp_epi(P, smem), tm, tn, et);
+    } else if constexpr ((kFolds & P4V_FOLD_QKV8) != 0) {
+      qkv8_stage_tile(P, mlp_epi(P, smem), r, frow, fcol);
+      asm volatile("bar.sync 1, %0;" ::"n"(kConsumers));   // staged tile complete
+      // the next column tile's first barrier orders these reads of the staging before it is written again
+      qkv8_store_tile(P, mlp_epi(P, smem), tm, tn, et);
     } else if constexpr ((kFolds & P4V_FOLD_RES) != 0) {
       // the residual add: out[dst] = fl(-r + res[dst]) (torch's FP32 add of the stored value and the shortcut), the
       // shortcut read at the destination rows as the pairs the plain store writes
@@ -465,6 +536,10 @@ int p4v_launch_forward_tc(const FwdParams& p, unsigned folds, int num_sms, cudaS
     case P4V_FOLD_MLP | P4V_FOLD_NORM: kernel = forward_tc_kernel<P4V_FOLD_MLP | P4V_FOLD_NORM>; break;
     case P4V_FOLD_RES: kernel = forward_tc_kernel<P4V_FOLD_RES>; break;
     case P4V_FOLD_NORM | P4V_FOLD_GATHER: kernel = forward_tc_kernel<P4V_FOLD_NORM | P4V_FOLD_GATHER>; break;
+    case P4V_FOLD_QKV8: kernel = forward_tc_kernel<P4V_FOLD_QKV8>; break;
+    case P4V_FOLD_NORM | P4V_FOLD_QKV8: kernel = forward_tc_kernel<P4V_FOLD_NORM | P4V_FOLD_QKV8>; break;
+    case P4V_FOLD_NORM | P4V_FOLD_GATHER | P4V_FOLD_QKV8:
+      kernel = forward_tc_kernel<P4V_FOLD_NORM | P4V_FOLD_GATHER | P4V_FOLD_QKV8>; break;
     default: P4V_REQUIRE(false, "forward: no kernel for the fold set 0x%x", folds);
   }
   if (folds & P4V_FOLD_MLP)
@@ -485,6 +560,13 @@ int p4v_launch_forward_tc(const FwdParams& p, unsigned folds, int num_sms, cudaS
     const bool merge = p.ga.mode == P4V_GATHER_MERGE && w.window == 0 && w.shift == 0 && w.height % 2 == 0 &&
                        w.width % 2 == 0 && p.ld % 16 == 0 && (long long)w.images * (w.height / 2) * (w.width / 2) == p.M;
     P4V_REQUIRE(w.images > 0 && w.height > 0 && w.width > 0 && (window || merge), "forward: bad gather layout");
+  }
+  if (folds & P4V_FOLD_QKV8) {
+    const FwdQkv8& q = p.q8;
+    P4V_REQUIRE(q.planes && (reinterpret_cast<uintptr_t>(q.planes) & 15) == 0 && q.dq && q.dk && q.dv,
+                "forward: qkv planes must be 16-byte aligned");
+    P4V_REQUIRE(q.D > 0 && q.D % 16 == 0 && q.heads > 0 && q.C == q.heads * q.D && p.N == 3 * q.C && q.N > 0 &&
+                (long long)q.batch * q.N == p.M, "forward: bad qkv plane layout");
   }
   const unsigned extra = p4v_fwd_extra_bytes(folds, p.epi_bytes);
   P4V_REQUIRE(p.n_jobs >= 1 && p.n_jobs <= P4V_MAX_JOBS && p.n_groups <= P4V_MAX_GROUPS, "forward: too many K segments");

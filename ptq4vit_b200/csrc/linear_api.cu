@@ -742,7 +742,8 @@ int build_frozen(const p4v_linear_desc* d, FrozenPlan& f, bool for_pack) {
 
 // The ring stages the fused kernel gets for a call of the layer f1 with the folds `folds` -- as fc1 of a fused MLP whose
 // fc2 is f2 (P4V_FOLD_MLP), with a LayerNorm folded into its activation quantiser (NORM), with a row gather of
-// gather_mode in front of that LayerNorm (GATHER) -- or 0 when the call does not take the fused kernel.  f1 must be on it
+// gather_mode in front of that LayerNorm (GATHER), as an attention block's qkv writing int8 planes (QKV8) -- or 0 when
+// the call does not take the fused kernel.  f1 must be on it
 // itself; an MLP needs fc1's outputs to be fc2's inputs and a plain fc1, a LayerNorm a plain layer with K % 4 == 0, the
 // merge gather C = K / 4 a multiple of 4, so that no float4 of the LayerNorm's walk straddles a quarter.  The epilogue,
 // the gather's source rows and the row stats take their share of shared memory, which can only lower the count.
@@ -867,8 +868,9 @@ int check_layout(const char* fn, const p4v_window_layout& win, int rows) {
 }
 
 // The layout of a non-null row gather (DESIGN §4.12) of a call with `rows` output rows and K = in_features, the image x
-// apart from out ([rows][out_cols]); x's null pointer and alignment are check_norm's
-int check_gather(const char* fn, const p4v_input_gather& g, const float* x, const float* out, int rows, int K, int out_cols) {
+// apart from out (out_bytes: [rows][out_cols] FP32, or the int8 planes of a qkv fold); x's null pointer and alignment are
+// check_norm's
+int check_gather(const char* fn, const p4v_input_gather& g, const float* x, const void* out, size_t out_bytes, int rows, int K) {
   const p4v_window_layout& w = g.layout;
   if (g.mode == P4V_GATHER_WINDOW) {
     if (int rc = check_layout(fn, w, rows)) return rc;
@@ -886,8 +888,8 @@ int check_gather(const char* fn, const p4v_input_gather& g, const float* x, cons
                 (long long)w.images * (w.height / 2) * (w.width / 2), rows);
   }
   // either way the image holds rows * K floats
-  const uintptr_t xb = (uintptr_t)rows * (uintptr_t)K * 4, ob = (uintptr_t)rows * (uintptr_t)out_cols * 4,
-                  a = reinterpret_cast<uintptr_t>(x), b = reinterpret_cast<uintptr_t>(out);
+  const uintptr_t xb = (uintptr_t)rows * (uintptr_t)K * 4, ob = out_bytes, a = reinterpret_cast<uintptr_t>(x),
+                  b = reinterpret_cast<uintptr_t>(out);
   P4V_REQUIRE(a + xb <= b || b + ob <= a, "%s: x overlaps out", fn);
   return 0;
 }
@@ -908,13 +910,15 @@ int check_residual(const char* fn, const float* res, const float* out, int rows,
 // One call of frozen layers: layer f1 on x, optionally with a LayerNorm folded into its activation quantiser (ln), with
 // its rows gathered from an image in front of that LayerNorm (gather, *ga), as fc1 of a fused MLP whose epilogue writes
 // the image of its fc2 (f2) into the workspace, which fc2's sweep forward then reads, and with a residual added by the
-// last store (rs.res non-null; rs.win: Swin's window reverse, on f1's fused kernel only).
+// last store (rs.res non-null; rs.win: Swin's window reverse, on f1's fused kernel only), or as an attention block's qkv
+// whose epilogue writes the attention's int8 planes (q8 non-null; out null).
 struct FrozenCall {
   const FrozenPlan* f1; const float* x; const float* bias1; const void* pack1; size_t pack1_bytes;
   const FwdNorm* ln;                                   // null: no LayerNorm
   bool gather; const p4v_input_gather* ga;
   const FrozenPlan* f2; const float* bias2; const void* pack2; size_t pack2_bytes;   // f2 null: no MLP
   FwdResidual rs;
+  const FwdQkv8* q8;                                   // null: FP32 output
   void* workspace; size_t workspace_bytes;
   float* out;
 };
@@ -941,24 +945,32 @@ int frozen_call(const char* fn, const FrozenCall& c, cudaStream_t st) {
   const FrozenPlan& f1 = *c.f1;
   const bool mlp = c.f2 != nullptr, norm = c.ln != nullptr;
   const unsigned folds = (mlp ? P4V_FOLD_MLP : 0u) | (norm ? P4V_FOLD_NORM : 0u) | (c.gather ? P4V_FOLD_GATHER : 0u) |
-                         (c.rs.res && !mlp ? P4V_FOLD_RES : 0u);
+                         (c.rs.res && !mlp ? P4V_FOLD_RES : 0u) | (c.q8 ? P4V_FOLD_QKV8 : 0u);
   if (norm) {
     if (int rc = check_norm(fn, c.x, c.ln->gamma, c.ln->beta, c.ln->eps)) return rc;
   }
   if (mlp)
     P4V_REQUIRE(f1.p.d.rows == c.f2->p.d.rows, "%s: fc1 and fc2 must have the same rows (%d != %d)", fn, f1.p.d.rows,
                 c.f2->p.d.rows);
-  P4V_REQUIRE(c.x && c.pack1 && (!mlp || (c.pack2 && c.workspace)) && c.out, "%s: null pointer", fn);
+  P4V_REQUIRE(c.x && c.pack1 && (!mlp || (c.pack2 && c.workspace)) && (c.out || (c.q8 && c.q8->planes)), "%s: null pointer", fn);
   P4V_REQUIRE((!f1.p.d.has_bias || c.bias1) && (!mlp || !c.f2->p.d.has_bias || c.bias2), "%s: has_bias set but bias is null", fn);
   if (c.gather) P4V_REQUIRE(c.ga, "%s: null pointer", fn);
   const int stages = fold_stages(f1, c.f2, folds, c.gather ? c.ga->mode : 0);
   if (folds & ~P4V_FOLD_RES)
-    P4V_REQUIRE(stages, "%s: %s", fn, mlp ? (norm ? "these layers do not fuse with the LayerNorm (p4v_mlp_norm_ok)"
+    P4V_REQUIRE(stages, "%s: %s", fn, c.q8 ? "the attention operands do not fold into this qkv (p4v_linear_qkv8_ok)"
+                                    : mlp ? (norm ? "these layers do not fuse with the LayerNorm (p4v_mlp_norm_ok)"
                                                   : "these layers do not fuse (p4v_mlp_fused_ok)")
                                           : c.gather ? "the gather does not fold into this layer (p4v_linear_gather_ok)"
                                                      : "the LayerNorm does not fold into this layer (p4v_linear_norm_ok)");
+  // the int8 planes of a qkv fold take the place of the FP32 output
+  const void* dst = c.q8 ? static_cast<const void*>(c.q8->planes) : static_cast<const void*>(c.out);
+  const size_t dst_bytes = (size_t)f1.p.M * (size_t)f1.p.O * (c.q8 ? 1 : 4);
   if (c.gather) {
-    if (int rc = check_gather(fn, *c.ga, c.x, c.out, f1.p.M, f1.p.K, f1.p.O)) return rc;
+    if (int rc = check_gather(fn, *c.ga, c.x, dst, dst_bytes, f1.p.M, f1.p.K)) return rc;
+  } else if (c.q8) {
+    const uintptr_t xb = (uintptr_t)f1.p.M * (uintptr_t)f1.p.K * 4, a = reinterpret_cast<uintptr_t>(c.x),
+                    b = reinterpret_cast<uintptr_t>(dst);
+    P4V_REQUIRE(a + xb <= b || b + dst_bytes <= a, "%s: x overlaps the planes", fn);
   }
   if (mlp) {
     P4V_REQUIRE(c.pack1_bytes >= f1.bytes && c.pack2_bytes >= c.f2->bytes, "%s: packed buffer too small "
@@ -994,6 +1006,7 @@ int frozen_call(const char* fn, const FrozenCall& c, cudaStream_t st) {
   if (norm) q.ln = *c.ln;
   if (folds & P4V_FOLD_RES) q.rs = c.rs;
   if (c.gather) q.ga = FwdGather{c.ga->mode, c.ga->layout};
+  if (c.q8) q.q8 = *c.q8;
   const int rc = p4v_launch_forward_tc(q, folds, p4v_num_sms(), st);
   if (rc || !mlp) return rc;
   return streamed_sweep(*c.f2, p2, c.workspace, c.bias2, c.rs.res, c.out, st);
@@ -1149,4 +1162,62 @@ extern "C" int p4v_linear_frozen_forward_norm_gather(const p4v_linear_desc* d, c
   FrozenCall c = linear_call(f, x, bias, packed, out);
   c.ln = &ln; c.gather = true; c.ga = g;
   return frozen_call("linear_frozen_forward_norm_gather", c, (cudaStream_t)stream);
+}
+
+// ---- the attention operands' quantisation folded into the frozen qkv (DESIGN §4.14) --------------------------------
+namespace {
+
+// The fold set of a qkv call for the rule: with a window gather NORM | GATHER; without one, NORM too when the layer can
+// take a LayerNorm, so that the rule holds with and without it
+unsigned qkv8_rule_folds(const FrozenPlan& f, int gather_mode) {
+  if (gather_mode) return P4V_FOLD_QKV8 | P4V_FOLD_NORM | P4V_FOLD_GATHER;
+  return P4V_FOLD_QKV8 | (!f.p.twin && f.p.K % 4 == 0 ? P4V_FOLD_NORM : 0u);
+}
+
+// The rule without the attention's own (p4v_attention_fused_ok): out_features == 3 C and the fused plan fits
+bool qkv8_fits(const FrozenPlan& f, const p4v_attention_desc& a, int gather_mode) {
+  return (long long)f.p.O == 3LL * a.heads * a.head_dim && fold_stages(f, nullptr, qkv8_rule_folds(f, gather_mode), gather_mode) > 0;
+}
+
+}  // namespace
+
+extern "C" int p4v_linear_qkv8_ok(const p4v_linear_desc* d, const p4v_attention_desc* a, int gather_mode, int* ok) {
+  FrozenPlan f; int rc = build_frozen(d, f, true);
+  if (rc) return rc;
+  P4V_REQUIRE(a && ok, "null argument");
+  P4V_REQUIRE(gather_mode == 0 || gather_mode == P4V_GATHER_WINDOW,
+              "linear_qkv8_ok: gather mode must be 0 or P4V_GATHER_WINDOW (got %d)", gather_mode);
+  int attn = 0;
+  p4v_attention_fused_ok(a->tokens, a->head_dim, &attn);
+  *ok = attn && a->heads > 0 && qkv8_fits(f, *a, gather_mode) ? 1 : 0;
+  return 0;
+}
+
+extern "C" int p4v_linear_frozen_forward_qkv8(const p4v_linear_desc* d, const float* x, const float* bias, const void* packed,
+                                              const p4v_attention_desc* a, const p4v_matmul_desc* mm1, const void* pack1,
+                                              size_t pack1_bytes, const p4v_matmul_desc* mm2, const void* pack2,
+                                              size_t pack2_bytes, int8_t* planes, const float* gamma, const float* beta,
+                                              float eps, const p4v_input_gather* g, void* stream) {
+  const char* fn = "linear_frozen_forward_qkv8";
+  FrozenPlan f; int rc = build_frozen(d, f, false);
+  if (rc) return rc;
+  P4V_REQUIRE(planes, "%s: null pointer", fn);
+  P4V_REQUIRE((reinterpret_cast<uintptr_t>(planes) & 15) == 0, "%s: planes must be 16-byte aligned", fn);
+  P4V_REQUIRE(!g || g->mode == P4V_GATHER_WINDOW, "%s: gather mode must be P4V_GATHER_WINDOW (got %d)", fn, g->mode);
+  P4V_REQUIRE(!g || gamma, "%s: a gather needs the LayerNorm (gamma, beta)", fn);
+  FwdQkv8 q8{};
+  if ((rc = p4v_qkv8_steps(fn, a, mm1, pack1, pack1_bytes, mm2, pack2, pack2_bytes, q8))) return rc;
+  P4V_REQUIRE((long long)a->batch * a->tokens == d->rows, "%s: batch * tokens = %lld, the layer has %d rows", fn,
+              (long long)a->batch * a->tokens, d->rows);
+  int attn = 0;
+  p4v_attention_fused_ok(a->tokens, a->head_dim, &attn);
+  P4V_REQUIRE(attn && qkv8_fits(f, *a, g ? g->mode : 0), "%s: the attention operands do not fold into this qkv "
+              "(p4v_linear_qkv8_ok)", fn);
+  q8.planes = reinterpret_cast<uint8_t*>(planes);
+  const FwdNorm ln{gamma, beta, eps};
+  FrozenCall c = linear_call(f, x, bias, packed, nullptr);
+  c.q8 = &q8;
+  if (gamma) c.ln = &ln;
+  if (g) { c.gather = true; c.ga = g; }
+  return frozen_call(fn, c, (cudaStream_t)stream);
 }

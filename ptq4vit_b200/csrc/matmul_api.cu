@@ -519,12 +519,15 @@ extern "C" int p4v_attention_fused_ok(int32_t tokens, int32_t head_dim, int* ok)
 namespace {
 
 // Validates every argument of an attention call and fills the kernel parameters; `long_seq` applies the long kernel's
-// rules (N <= 1024; no q-scaling, bias or mask).
+// rules (N <= 1024; no q-scaling, bias or mask).  planes non-null: the int8 variant reads q, k and v from the planes of
+// the qkv epilogue ([3][batch][heads][N][head_dim], 16-byte aligned, not overlapping out) instead of qkv (null, as are
+// qkv_strides).
 int attention_params(const p4v_attention_desc* a, const float* qkv, const long long* qkv_strides, const p4v_matmul_desc* mm1,
                      const void* pack1, size_t pack1_bytes, const p4v_matmul_desc* mm2, const void* pack2, size_t pack2_bytes,
-                     const float* bias, const float* mask, float* out, bool long_seq, FwdAttnParams& q) {
-  const char* fn = long_seq ? "attention_frozen_forward_long" : "attention_frozen_forward";
-  P4V_REQUIRE(a && qkv && qkv_strides && mm1 && pack1 && mm2 && pack2 && out, "%s: null pointer", fn);
+                     const float* bias, const float* mask, float* out, bool long_seq, FwdAttnParams& q,
+                     const int8_t* planes = nullptr) {
+  const char* fn = planes ? "attention_frozen_forward_i8" : long_seq ? "attention_frozen_forward_long" : "attention_frozen_forward";
+  P4V_REQUIRE(a && (planes || (qkv && qkv_strides)) && mm1 && pack1 && mm2 && pack2 && out, "%s: null pointer", fn);
   P4V_REQUIRE(a->batch > 0 && a->heads > 0 && a->tokens > 0 && a->head_dim > 0, "%s: empty shape", fn);
   const int max_tokens = long_seq ? P4V_ATTN_LONG_MAX_TOKENS : P4V_ATTN_MAX_TOKENS;
   int ok = 0;
@@ -540,7 +543,8 @@ int attention_params(const p4v_attention_desc* a, const float* qkv, const long l
   const Packed k1 = packed_layout(mm1), k2 = packed_layout(mm2);
   P4V_REQUIRE(pack1_bytes == k1.bytes && pack2_bytes == k2.bytes,
               "%s: pack sizes %zu and %zu, expected %zu and %zu", fn, pack1_bytes, pack2_bytes, k1.bytes, k2.bytes);
-  for (int i = 0; i < 4; ++i) P4V_REQUIRE(qkv_strides[i] >= 0, "%s: negative stride", fn);
+  if (!planes)
+    for (int i = 0; i < 4; ++i) P4V_REQUIRE(qkv_strides[i] >= 0, "%s: negative stride", fn);
   P4V_REQUIRE(!a->scale_on_q || a->scale_on_q == 1, "%s: scale_on_q must be 0 or 1", fn);
   if (long_seq) {
     P4V_REQUIRE(!a->scale_on_q, "%s: scale_on_q is not supported (scores * scale after matmul1 only)", fn);
@@ -554,8 +558,18 @@ int attention_params(const p4v_attention_desc* a, const float* qkv, const long l
   P4V_REQUIRE((reinterpret_cast<uintptr_t>(out) & 7) == 0, "%s: out must be 8-byte aligned", fn);
   P4V_REQUIRE(((reinterpret_cast<uintptr_t>(pack1) | reinterpret_cast<uintptr_t>(pack2)) & 15) == 0,
               "%s: packs must be 16-byte aligned", fn);
+  if (planes) {
+    P4V_REQUIRE((reinterpret_cast<uintptr_t>(planes) & 15) == 0, "%s: planes must be 16-byte aligned", fn);
+    const uintptr_t n = (uintptr_t)a->batch * a->tokens * a->heads * a->head_dim, pa = reinterpret_cast<uintptr_t>(planes),
+                    po = reinterpret_cast<uintptr_t>(out);
+    P4V_REQUIRE(pa + 3 * n <= po || po + 4 * n <= pa, "%s: planes overlap out", fn);
+  }
   q = FwdAttnParams{};
-  q.qkv = qkv; q.s_b = qkv_strides[0]; q.s_n = qkv_strides[1]; q.s_p = qkv_strides[2]; q.s_h = qkv_strides[3];
+  if (planes) {
+    q.planes = reinterpret_cast<const uint8_t*>(planes);
+  } else {
+    q.qkv = qkv; q.s_b = qkv_strides[0]; q.s_n = qkv_strides[1]; q.s_p = qkv_strides[2]; q.s_h = qkv_strides[3];
+  }
   q.out = out;
   q.batch = a->batch; q.heads = a->heads; q.N = a->tokens; q.D = a->head_dim;
   q.scale = (float)a->scale; q.scale_on_q = a->scale_on_q;
@@ -582,6 +596,45 @@ extern "C" int p4v_attention_frozen_forward(const p4v_attention_desc* a, const f
   if (int rc = attention_params(a, qkv, qkv_strides, mm1, pack1, pack1_bytes, mm2, pack2, pack2_bytes, bias, mask, out, false, q))
     return rc;
   return p4v_launch_forward_attn_tc(q, mm2->sos != 0, (cudaStream_t)stream);
+}
+
+// ---- q, k and v as int8 planes from the qkv Linear's epilogue (DESIGN §4.14) ----------------------------------------
+extern "C" int p4v_attention_frozen_forward_i8(const p4v_attention_desc* a, const int8_t* planes, const p4v_matmul_desc* mm1,
+                                               const void* pack1, size_t pack1_bytes, const p4v_matmul_desc* mm2,
+                                               const void* pack2, size_t pack2_bytes, const float* bias, const float* mask,
+                                               float* out, void* stream) {
+  P4V_REQUIRE(planes, "attention_frozen_forward_i8: null pointer");
+  FwdAttnParams q;
+  if (int rc = attention_params(a, nullptr, nullptr, mm1, pack1, pack1_bytes, mm2, pack2, pack2_bytes, bias, mask, out, false, q,
+                                planes))
+    return rc;
+  return p4v_launch_forward_attn_tc(q, mm2->sos != 0, (cudaStream_t)stream, true);
+}
+
+int p4v_qkv8_steps(const char* fn, const p4v_attention_desc* a, const p4v_matmul_desc* mm1, const void* pack1,
+                   size_t pack1_bytes, const p4v_matmul_desc* mm2, const void* pack2, size_t pack2_bytes, FwdQkv8& q) {
+  P4V_REQUIRE(a && mm1 && pack1 && mm2 && pack2, "%s: null pointer", fn);
+  P4V_REQUIRE(a->batch > 0 && a->heads > 0 && a->tokens > 0 && a->head_dim > 0, "%s: empty shape", fn);
+  P4V_REQUIRE(!a->scale_on_q || a->scale_on_q == 1, "%s: scale_on_q must be 0 or 1", fn);
+  if (int rc = check_shape(mm1)) return rc;
+  if (int rc = check_shape(mm2)) return rc;
+  P4V_REQUIRE(mm1->heads == a->heads && mm2->heads == a->heads,
+              "%s: packs made for %d and %d heads, the call has %d", fn, mm1->heads, mm2->heads, a->heads);
+  P4V_REQUIRE(!mm1->sos, "%s: matmul1 cannot be split-of-softmax", fn);
+  const Packed k1 = packed_layout(mm1), k2 = packed_layout(mm2);
+  P4V_REQUIRE(pack1_bytes == k1.bytes && pack2_bytes == k2.bytes,
+              "%s: pack sizes %zu and %zu, expected %zu and %zu", fn, pack1_bytes, pack2_bytes, k1.bytes, k2.bytes);
+  P4V_REQUIRE(((reinterpret_cast<uintptr_t>(pack1) | reinterpret_cast<uintptr_t>(pack2)) & 15) == 0,
+              "%s: packs must be 16-byte aligned", fn);
+  void* p1 = const_cast<void*>(pack1);          // read only
+  void* p2 = const_cast<void*>(pack2);
+  const int A1 = 1 << (mm1->A_bit - 1), B1 = 1 << (mm1->B_bit - 1), B2 = 1 << (mm2->B_bit - 1);
+  q.N = a->tokens; q.heads = a->heads; q.D = a->head_dim; q.C = a->heads * a->head_dim; q.batch = a->batch;
+  q.scale_on_q = a->scale_on_q; q.scale = (float)a->scale;
+  q.dq = at<float>(p1, k1.o_dA); q.dk = at<float>(p1, k1.o_dB); q.dv = at<float>(p2, k2.o_dB);
+  q.q_lo = (float)-A1; q.q_hi = (float)(A1 - 1); q.k_lo = (float)-B1; q.k_hi = (float)(B1 - 1);
+  q.v_lo = (float)-B2; q.v_hi = (float)(B2 - 1);
+  return 0;
 }
 
 // ---- the long-sequence variant (forward_attn_long_tc.cu) ---------------------------------------------------------

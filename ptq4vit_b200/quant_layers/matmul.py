@@ -12,6 +12,7 @@ from torch import nn
 from .. import _lib
 from ._chunking import choose_chunks, workspace_budget
 from ._metric import metric_weight
+from .linear import _flat2d, _frozen_quant_forward, _gather_desc, _norm_call_ok, _wants_no_grad, frozen_gather_applies
 
 
 class _QuantMatMulFn(torch.autograd.Function):
@@ -281,6 +282,98 @@ def frozen_attention(matmul1, matmul2, qkv, scale, scale_on_q, bias=None, mask=N
         ctypes.byref(a), _lib.ptr(qkv), (ctypes.c_longlong * 4)(*qkv.stride()[:4]), ctypes.byref(d1), _lib.ptr(p1), p1.numel(),
         ctypes.byref(d2), _lib.ptr(p2), p2.numel(), _lib.ptr(bias), _lib.ptr(mask), _lib.ptr(out),
         ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), name)
+    return out
+
+
+def _attention_desc(batch, tokens, heads, head_dim, scale, scale_on_q, n_windows=0):
+    a = _lib.AttentionDesc()
+    a.batch, a.tokens, a.heads, a.head_dim = int(batch), int(tokens), int(heads), int(head_dim)
+    a.scale_on_q, a.n_windows, a.scale = int(bool(scale_on_q)), int(n_windows), float(scale)
+    return a
+
+
+def frozen_qkv_ok(qkv, tokens, heads, head_dim, gather=False):
+    """The library's shape rule of the qkv fold (p4v_linear_qkv8_ok): out_features == 3 * heads * head_dim, the short
+    attention kernel's shape (at most 256 tokens, head_dim a multiple of 16 up to 64), qkv on its fused path, the plan
+    with the epilogue's staging (and the LayerNorm's statistics, and with `gather` the window gather's table) fits."""
+    ok = ctypes.c_int()
+    a = _attention_desc(1, tokens, heads, head_dim, 1.0, False)
+    _lib.check(_lib.lib().p4v_linear_qkv8_ok(ctypes.byref(qkv._desc(1, 1)), ctypes.byref(a), _lib.GATHER["window"] if gather else 0,
+                                             ctypes.byref(ok)), "p4v_linear_qkv8_ok")
+    return bool(ok.value)
+
+
+def frozen_qkv_applies(qkv, matmul1, matmul2, x, tokens, heads, head_dim, *inputs, norm=None, gather=None):
+    """Whether one attention call -- qkv(x) (qkv(norm(x)) with `norm`; with `gather` = (images, height, width, window,
+    shift) the windows of roll(norm(x), -shift), as frozen_gather_applies) followed by the attention core -- can run with
+    the attention operands' quantisation folded into qkv (frozen_qkv_attention): qkv a frozen Linear layer in
+    quant_forward mode, the conditions of frozen_attention_applies on the short kernel (both MatMul modules frozen,
+    matmul1 not split-of-softmax, at most 256 tokens, no input -- x and `inputs` -- that requires grad under grad mode),
+    those of the LayerNorm or gather fold when one is given, and the library's rule (frozen_qkv_ok).  Decided from the
+    shapes before qkv runs, so a refused call runs the unfolded sequence once (DESIGN.md section 4.14)."""
+    if tokens > SHORT_ATTENTION_TOKENS or not _frozen_quant_forward(qkv):
+        return False
+    if not frozen_attention_applies(matmul1, matmul2, tokens, head_dim, x, *inputs):
+        return False
+    dev = qkv._packed.device
+    if not torch.is_tensor(x) or x.dtype != torch.float32 or x.device != dev or x.numel() == 0 or x.shape[-1] != qkv.in_features:
+        return False
+    if gather is not None:
+        if not frozen_gather_applies(norm, qkv, x, ("window", *gather)):
+            return False
+    elif norm is not None:
+        if not _norm_call_ok(norm, qkv, x):
+            return False
+    elif not _wants_no_grad((x,), (qkv,)):
+        return False
+    if (x.numel() // x.shape[-1]) % tokens:
+        return False
+    return frozen_qkv_ok(qkv, tokens, heads, head_dim, gather is not None)
+
+
+def frozen_qkv_planes(qkv, matmul1, matmul2, x, tokens, heads, head_dim, scale, scale_on_q, norm=None, gather=None):
+    """The first launch of frozen_qkv_attention: qkv(x) (with `norm` / `gather` as frozen_qkv_applies) on qkv's fused
+    kernel, whose epilogue quantises q (times scale first with scale_on_q), k and v with matmul1's A and B and matmul2's B
+    step sizes (csrc/forward_tc.cu).  Returns the int8 planes [3, batch, heads, tokens, head_dim], the bytes the short
+    attention kernel would make of qkv's FP32 output; only they are allocated."""
+    qkv._check_frozen_intervals()
+    p1, p2 = matmul1._frozen_pack(heads), matmul2._frozen_pack(heads)
+    dev = qkv._packed.device
+    x2 = _flat2d(x.to(dev))
+    rows = x2.shape[0]
+    planes = torch.empty(3, rows // tokens, heads, tokens, head_dim, dtype=torch.int8, device=dev)
+    a = _attention_desc(rows // tokens, tokens, heads, head_dim, scale, scale_on_q)
+    d, d1, d2 = qkv._desc(rows, 1), matmul1._desc_dims(1, heads, 1, 1, 1), matmul2._desc_dims(1, heads, 1, 1, 1)
+    b = None if qkv.bias is None else qkv.bias.detach().contiguous().float()
+    g = None if gather is None else ctypes.byref(_gather_desc(("window", *gather)))
+    _lib.check(_lib.lib().p4v_linear_frozen_forward_qkv8(
+        ctypes.byref(d), _lib.ptr(x2), _lib.ptr(b), _lib.ptr(qkv._packed), ctypes.byref(a), ctypes.byref(d1), _lib.ptr(p1),
+        p1.numel(), ctypes.byref(d2), _lib.ptr(p2), p2.numel(), _lib.ptr(planes), _lib.ptr(None if norm is None else norm.weight),
+        _lib.ptr(None if norm is None else norm.bias), 0.0 if norm is None else float(norm.eps), g,
+        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "p4v_linear_frozen_forward_qkv8")
+    return planes
+
+
+def frozen_qkv_attention(qkv, matmul1, matmul2, x, tokens, heads, head_dim, scale, scale_on_q, bias=None, mask=None,
+                         norm=None, gather=None):
+    """The attention core of frozen_attention on qkv(x) (with `norm` / `gather` as frozen_qkv_applies), for a call where
+    frozen_qkv_applies holds, in two launches: qkv's fused kernel writes q, k and v as int8 planes (frozen_qkv_planes),
+    and the short attention kernel reads them (csrc/forward_attn_tc.cu).  Bit-identical to frozen qkv followed by
+    frozen_attention; qkv's FP32 output never reaches HBM.  Returns [batch, tokens, heads * head_dim]; only the planes and
+    it are allocated."""
+    planes = frozen_qkv_planes(qkv, matmul1, matmul2, x, tokens, heads, head_dim, scale, scale_on_q, norm=norm, gather=gather)
+    p1, p2 = matmul1._frozen_pack(heads), matmul2._frozen_pack(heads)
+    dev = planes.device
+    batch = planes.shape[1]
+    out = torch.empty(batch, tokens, heads * head_dim, dtype=torch.float32, device=dev)
+    bias = None if bias is None else bias.to(dev, torch.float32).contiguous()
+    mask = None if mask is None else mask.to(dev, torch.float32).contiguous()
+    a = _attention_desc(batch, tokens, heads, head_dim, scale, scale_on_q, 0 if mask is None else mask.shape[0])
+    d1, d2 = matmul1._desc_dims(1, heads, 1, 1, 1), matmul2._desc_dims(1, heads, 1, 1, 1)
+    _lib.check(_lib.lib().p4v_attention_frozen_forward_i8(
+        ctypes.byref(a), _lib.ptr(planes), ctypes.byref(d1), _lib.ptr(p1), p1.numel(), ctypes.byref(d2), _lib.ptr(p2), p2.numel(),
+        _lib.ptr(bias), _lib.ptr(mask), _lib.ptr(out), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+        "p4v_attention_frozen_forward_i8")
     return out
 
 

@@ -63,6 +63,12 @@ flatten, transpose, cat with the cls token and pos_embed add, Swin's flatten, tr
 stores the token rows the first block reads, bit-identical to the frozen conv followed by torch's ops, so the NCHW output
 and its copies never reach HBM.  It composes with the other fusions.  A folded call skips the conv's and patch_norm's
 forward hooks, so it is opt-in; `unfuse_stem(net)` undoes it.
+`fuse_qkv(net)` folds the attention operands' quantisation into the frozen qkv of every attention block whose qkv,
+matmul1 and matmul2 are frozen and which runs fused (fuse_attention): qkv's kernel quantises its output with matmul1's and
+matmul2's step sizes and writes int8 q, k and v, which the short attention kernel reads instead of quantising the FP32
+qkv output, bit-identical.  Calls above 256 tokens keep the FP32 hand-off.  It composes with the other fusions (norm1 and
+Swin's gather into qkv, the residual into proj).  A folded call skips qkv's forward hooks, so it is opt-in;
+`unfuse_qkv(net)` undoes it.
 None of the fusions is recorded by save_quantized: apply them again after load_quantized.
 """
 import torch
@@ -285,6 +291,31 @@ def unfuse_stem(net):
     for m in net.modules():
         if _stem_site(m) is not None:
             m.fold_stem = False
+
+
+def fuse_qkv(net):
+    """Mark every `Attention` and `WindowAttention` of `net` whose qkv is a frozen Linear layer and whose matmul1 and
+    matmul2 are frozen MatMul modules: each call that also runs fused (fuse_attention) and qualifies
+    (quant_layers.matmul.frozen_qkv_applies: the short attention kernel, no gradient wanted, the conditions of the norm1
+    or gather fold it carries, a shape the fused kernel holds) has qkv's kernel quantise q, k and v with the attention's
+    step sizes and write them as int8 planes, which the attention kernel reads -- with the bits of the unfolded call, and
+    qkv's FP32 output never reaches HBM; any other call runs the modules as before.  A folded call skips qkv's forward
+    hooks, which is why the fold is opt-in.  It composes with every other fusion; save_quantized / load_quantized do not
+    record it.  Returns the names of the attention modules left unfolded."""
+    left = []
+    for name, m in net.named_modules():
+        if isinstance(m, (Attention, WindowAttention)):
+            m.fold_qkv = isinstance(m.qkv, MinMaxQuantLinear) and m.qkv.frozen and \
+                all(isinstance(mm, MinMaxQuantMatMul) and mm.frozen for mm in (m.matmul1, m.matmul2))
+            if not m.fold_qkv:
+                left.append(name)
+    return left
+
+
+def unfuse_qkv(net):
+    for m in net.modules():
+        if isinstance(m, (Attention, WindowAttention)):
+            m.fold_qkv = False
 
 
 def _to(v, device):

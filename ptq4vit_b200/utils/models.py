@@ -9,7 +9,7 @@ from ..quant_layers.conv import frozen_stem, frozen_stem_applies
 from ..quant_layers.linear import (frozen_gather_applies, frozen_gather_linear, frozen_mlp, frozen_mlp_applies,
                                    frozen_mlp_norm_ok, frozen_norm_applies, frozen_norm_linear, frozen_residual_applies,
                                    frozen_residual_linear)
-from ..quant_layers.matmul import frozen_attention, frozen_attention_applies
+from ..quant_layers.matmul import frozen_attention, frozen_attention_applies, frozen_qkv_applies, frozen_qkv_attention
 
 
 def _norm_linear(norm, lin, x):
@@ -47,11 +47,17 @@ class Attention(nn.Module):
     fused = False      # set by utils.deploy.fuse_attention: run the frozen attention core as one kernel when it applies
     fused_max_tokens = 256   # set by utils.deploy.fuse_attention: sequences up to this length run fused (the long
                              # kernel above 256 tokens)
+    fold_qkv = False   # set by utils.deploy.fuse_qkv: with `fused`, qkv writes int8 q, k and v for the short attention
+                       # kernel when it applies
 
     def forward(self, x, norm=None, residual=None):
         """norm: a LayerNorm to apply to x first (Block with fold_norm1), folded into qkv when it applies.  residual: a
         tensor to add to the output (Block with fold_residual), folded into proj when it applies."""
         B, N, C = x.shape
+        H, D = self.num_heads, C // self.num_heads
+        if self.fold_qkv and self.fused and frozen_qkv_applies(self.qkv, self.matmul1, self.matmul2, x, N, H, D, norm=norm):
+            return _linear_res(self.proj, frozen_qkv_attention(self.qkv, self.matmul1, self.matmul2, x, N, H, D, self.scale,
+                                                               scale_on_q=False, norm=norm), residual)
         y = self.qkv(x) if norm is None else _norm_linear(norm, self.qkv, x)
         if self.fused and frozen_attention_applies(self.matmul1, self.matmul2, N, C // self.num_heads, y,
                                                    max_tokens=self.fused_max_tokens):
@@ -226,6 +232,7 @@ class WindowAttention(nn.Module):
         self.matmul2 = MatMul()
 
     fused = False      # set by utils.deploy.fuse_attention, as Attention.fused
+    fold_qkv = False   # set by utils.deploy.fuse_qkv, as Attention.fold_qkv
 
     def forward(self, x, mask=None, residual=None, layout=None, norm=None, gather=None):
         """residual, layout: (SwinBlock with fold_residual) return residual + the image of the output windows under
@@ -234,6 +241,15 @@ class WindowAttention(nn.Module):
         the block's input [images, height * width, C] and the windows are those of roll(norm(x), (-shift, -shift)) under
         gather = (images, height, width, window, shift), with the LayerNorm, roll and partition folded into qkv when it
         applies."""
+        if self.fold_qkv and self.fused:
+            N = x.shape[1] if gather is None else gather[3] * gather[3]
+            H, D = self.num_heads, x.shape[-1] // self.num_heads
+            if frozen_qkv_applies(self.qkv, self.matmul1, self.matmul2, x, N, H, D, self.relative_position_bias_table, mask,
+                                  norm=norm, gather=gather):
+                bias = self.relative_position_bias_table[self.relative_position_index.view(-1)].view(N, N, -1).permute(2, 0, 1).contiguous()
+                return self._proj(frozen_qkv_attention(self.qkv, self.matmul1, self.matmul2, x, N, H, D, self.scale,
+                                                       scale_on_q=True, bias=bias, mask=mask, norm=norm, gather=gather),
+                                  residual, layout)
         if gather is None:
             B_, N, C = x.shape
             y = self.qkv(x)
